@@ -9,7 +9,7 @@ scenes are independent, no collective on the inference path; SURVEY.md 8e).  ONE
   value          whole-job scenes/s, inputs resident in HBM, device-timed, max over ranks
   e2e            the same metric through the public pipeline with pinned HOST grids (H2D + D2H inside the timed region); `forward_api`
                  inside it = NeRFRegionProposalNetwork.forward itself with the reference's own methodology (run_rpn.py:594-617)
-  roofline       dominant kernel (tcgen05 implicit-GEMM conv, one RPN-head layer over P2..P5) timed live with CUDA events
+  roofline       dominant kernel (wgmma implicit-GEMM conv, one RPN-head layer over P2..P5) timed live with CUDA events
   variants       other loads on the same box: seed-0 weights (round-1 line), rotated boxes (--rotated_bbox: polygon-clip NMS), one scene per
                  launch, bf16 (BASELINE's dtype, 8e-3 feature parity)
   train          BASELINE config 4: one training step (forward + losses + backward + clip + AdamW) per rank on one 160x256x256 scene with
@@ -45,7 +45,9 @@ FLOPS_PER_SCENE = 3.913e12        # SURVEY.md 8(d): conv FLOPs (2*MAC) of the re
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=40)
+    ap.add_argument("--steps", type=int, default=40,
+                    help="timed steps of the headline loop (and of the end-to-end pipeline leg); the extra legs keep their own counts: "
+                         "variants max(8, steps // 4), training 8, forward API 100 repetitions")
     ap.add_argument("--warmup", type=int, default=4)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--precision", default=None, choices=["bf16", "fp16", "fp16_w2"],
@@ -65,6 +67,9 @@ def parse():
                          "200x200x130; 5 = oriented IoU + NMS sweep 1k..1M boxes")
     ap.add_argument("--weights", default="spread", choices=["spread", "seed0"], help="headline weights: spread objectness (default) or plain seed-0 init")
     ap.add_argument("--rotated", action="store_true", help="headline with --rotated_bbox (8 deltas, OBB decode, polygon-clip NMS)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (proposals, scores, levels per scene and a fixed, "
+                         "seeded sample of every feature level) as DIR/<name>.npy; headline inference run only (--mode infer --config 2)")
     return ap.parse_args()
 
 
@@ -161,7 +166,7 @@ _CPU = {}
 
 def _cpu_state():
     """The reference on the host: its own modules (oracle/_ref, eval mode, AABB head: no native op on that path) when staged, else the
-    oracle's fp32 port.  Same seed-0 + spread weights and scene as the B200 arm."""
+    oracle's fp32 port.  Same seed-0 + spread weights and scene as the CUDA arm."""
     if _CPU:
         return _CPU
     import torch
@@ -207,10 +212,10 @@ def cpu_run(x_extent, n_threads, repeats=1, y_extent=None):
 
 
 def best_cpu_threads():
-    """Intra-op thread count that makes the CPU run fastest on this host: all cores is NOT it on a 128-thread box (measured on the B200 host:
-    full scene 4.2 s with 32 threads vs 33 s with 128 -- profiles/r01_cpu_port_threads.txt). Sweeps {all, 64, 32, 16, 8} on a small block."""
+    """Intra-op thread count that makes the CPU run fastest on this host: all cores is not always it on hosts with many hardware threads
+    (oversubscribed intra-op pools slow the fp32 port down). Sweeps {all, 64, 32, 16, 8} on a small block."""
     cores = os.cpu_count() or 1
-    # more than 64 intra-op threads only ever lost on the B200 host (128 threads: 45 s per block vs 0.5 s with 16): not swept
+    # more than 64 intra-op threads are not swept
     cands = sorted({c for c in (min(cores, 64), 32, 16, 8) if 1 <= c <= cores}, reverse=True)
     cpu_run(32, min(cands), y_extent=64)                       # library warm-up (oneDNN JIT, thread pool), not timed
     sweep = {}
@@ -262,14 +267,14 @@ def run_reference(args):
     _emit(out)
 
 
-# ------------------------------------------------------------------------------------------------ B200 arm
+# ------------------------------------------------------------------------------------------------ CUDA arm
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), "measured (MEASURED_PEAKS.json)"
-    return 1590.0, 1400.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops", 989.0), d.get("bf16_tflops_sustained", 989.0), "measured (MEASURED_PEAKS.json)"
+    return 989.0, 989.0, "fallback: NVIDIA H100 SXM data sheet, dense bf16 (not measured)"
 
 
 def time_dominant_kernel(plan, reps=10):
@@ -288,6 +293,32 @@ def time_dominant_kernel(plan, reps=10):
     vox = plan.n * sum(d[0] * d[1] * d[2] for d in plan.feat_dims)
     flops = 2.0 * vox * 256 * 256 * 27
     return statistics.mean(times), min(times), flops
+
+
+FEATURE_SAMPLE = 1 << 18          # elements kept per feature level by --dump-outputs (seeded, identical from run to run)
+
+
+def dump_outputs(plan, out_dir):
+    """Writes the arrays the last engine step returned to its caller as float32 .npy files: per scene the proposals, their scores and pyramid
+    levels (the first `count` rows), and for every feature level a fixed sample of FEATURE_SAMPLE elements (indices from a seeded generator)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.current_stream().wait_event(plan.done)
+    torch.cuda.synchronize()
+    counts = plan.out_count.reshape(-1).tolist()
+    for b, n in enumerate(counts):
+        n = int(n)
+        np.save(os.path.join(out_dir, f"proposals_{b}.npy"), plan.out_boxes[b, :n].float().cpu().numpy())
+        np.save(os.path.join(out_dir, f"scores_{b}.npy"), plan.out_scores[b, :n].float().cpu().numpy())
+        if plan.out_levels is not None:
+            np.save(os.path.join(out_dir, f"levels_{b}.npy"), plan.out_levels[b, :n].float().cpu().numpy())
+    g = torch.Generator().manual_seed(0)
+    for i, f in enumerate(plan.features):
+        flat = f.reshape(-1)
+        idx = torch.randint(0, flat.numel(), (min(FEATURE_SAMPLE, flat.numel()),), generator=g)
+        np.save(os.path.join(out_dir, f"feature_{i}_sample.npy"), flat[idx.to(flat.device)].float().cpu().numpy())
+        np.save(os.path.join(out_dir, f"feature_{i}_sample_index.npy"), idx.double().numpy())
 
 
 def device_throughput(model, dev_batches, K, W, barrier, sampler=None):
@@ -313,7 +344,7 @@ def device_throughput(model, dev_batches, K, W, barrier, sampler=None):
 
 def train_leg(rank, local, world, barrier, steps=8, warm=4):       # warm-up covers the two eager steps + the graph capture of the launch lists
     """BASELINE config 4: ResNet50-FPN + anchor head, --rotated_bbox, one 160x256x256 scene per rank per step, data parallel: forward,
-    target assignment + sampling + losses, backward (dgrad / wgrad on tcgen05), NCCL all-reduce of the flat gradient bucket overlapped
+    target assignment + sampling + losses, backward (dgrad / wgrad on wgmma), NCCL all-reduce of the flat gradient bucket overlapped
     with the backward pass, clip_grad_norm_(0.1) + AdamW.  bf16 activations / gradients, fp32 master weights and accumulation."""
     import torch
     import torch.distributed as dist
@@ -379,7 +410,7 @@ def run_b200(args):
     local = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if not torch.cuda.is_available():
-        raise RuntimeError("bench.py: no CUDA device -- the B200 arm has no CPU fallback (use --impl reference for the CPU reference)")
+        raise RuntimeError("bench.py: no CUDA device -- the CUDA arm has no CPU fallback (use --impl reference for the CPU reference)")
     torch.cuda.set_device(local)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device(f"cuda:{local}"))
@@ -390,7 +421,7 @@ def run_b200(args):
     model = build_model(rotated=args.rotated, spread=spread, precision=args.precision).cuda().eval()
     eng = model.engine()
     B = max(1, args.scenes_per_step)
-    n_pool = 4                                             # 4 x 168 MB of distinct inputs (> 126 MB L2)
+    n_pool = 4                                             # 4 x 168 MB of distinct inputs (> 50 MB L2)
     if args.input_layout == "dataset_u8":   # raw uint8 (W,L,H,4) arrays as stored in uint8 npz files
         host = [(synth_scene(rank * 1000 + i, "dataset").permute(1, 2, 3, 0) * 255.0).round().to(torch.uint8).contiguous().pin_memory()
                 .permute(3, 0, 1, 2) for i in range(n_pool)]
@@ -416,6 +447,8 @@ def run_b200(args):
     sampler = ClockSampler(local)
     ms, plan, count = device_throughput(model, dev, K, W, barrier, sampler if rank == 0 else None)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(plan, args.dump_outputs)
 
     # ---- end to end through the streaming pipeline (pinned host grids in, proposals out on the host)
     with torch.no_grad():
@@ -444,17 +477,10 @@ def run_b200(args):
         k_mean, k_min, k_flops = time_dominant_kernel(plan)
         burst, sustained, how = measured_peaks()
         achieved = k_flops / (k_mean * 1e-3) / 1e12
-        traffic = None
-        try:
-            with open(os.path.join(ROOT, "profiles", "r02_ncu_full_summary.json")) as f:
-                for row in json.load(f):
-                    if row.get("capture") == "head":
-                        traffic = (row["dram_read_B"] + row["dram_write_B"]) * B
-        except (OSError, ValueError, KeyError):
-            traffic = None
+        traffic = None                                     # DRAM bytes need hardware counters: not measured here
         roofline = {"bound": "tensor", "kernel": "conv3d_igemm_kernel<256,4> (RPN head layer, 3x3x3 256->256 + bias + ReLU over P2..P5)",
                     "achieved": achieved, "peak": burst, "unit": "TFLOP/s", "frac": achieved / burst, "traffic": traffic,
-                    "traffic_source": "profiles/r02_ncu_full_summary.json (dram__bytes_read.sum + dram__bytes_write.sum of an ncu --set full capture, 1 scene/launch) x scenes per launch; a profile number, not measured in this run",
+                    "traffic_source": "not measured (DRAM byte counters are not read by this benchmark)",
                     "peak_source": how + ", burst figure (kernel timed alone, L2 flushed between launches)",
                     "launch_ms": k_mean, "flops_per_launch": k_flops,
                     "whole_step_frac_of_sustained": (FLOPS_PER_SCENE * world * K * B / (ms * 1e-3) / 1e12) / (sustained * world)}
@@ -502,7 +528,7 @@ def run_b200(args):
         if args.skip_cpu_baseline or world > 1:            # the CPU baseline is timed on rank 0 of the single-GPU run only
             cpu_t, cpu_sample, cpu_kind = float("nan"), "not timed in this run (N > 1 or --skip-cpu-baseline)", "port"
         else:
-            cores, sweep = best_cpu_threads()              # all 128 hardware threads are 8x SLOWER than 32 on the B200 host
+            cores, sweep = best_cpu_threads()              # the fastest intra-op thread count of a small sweep, not all hardware threads
             cpu_t = statistics.mean(cpu_run(160, cores, repeats=2))
             cpu_kind = _cpu_state()["kind"]
             cpu_sample = f"2 full scenes 160x256x256, mean ({_cpu_desc(cores, sweep)})"
@@ -513,7 +539,7 @@ def run_b200(args):
                           "precision": args.precision, "feature_map_parity": "<= 1e-3 norm-wise vs the reference's fp32 on this GPU at 160x256x256 "
                           "(tests/test_gpu_reference.py)" if args.precision == "fp16_w2" else "see DESIGN.md section 4",
                           "scenes_per_step_per_gpu": B, "parallelism": f"dp{world} (scenes shard over ranks, no collective on the inference path)",
-                          "l2": "4 distinct 168 MB input grids per rank cycled (> 126 MB L2); activations stream ~1.5 GB/scene",
+                          "l2": "4 distinct 168 MB input grids per rank cycled (> 50 MB L2); activations stream ~1.5 GB/scene",
                           "proposals_last_scene": count,
                           "input_layout": {"dataset": "fp32 (4,W,L,H) views of (W,L,H,4) arrays, as datasets.py:55-56 yields",
                                            "dataset_u8": "raw uint8 (4,W,L,H) views of (W,L,H,4) arrays, normalised on the device",
@@ -541,7 +567,7 @@ def _cfg_dist():
     import torch.distributed as dist
     rank, local, world = int(os.environ.get("RANK", "0")), int(os.environ.get("LOCAL_RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     if not torch.cuda.is_available():
-        raise RuntimeError("bench.py: no CUDA device -- the B200 arm has no CPU fallback")
+        raise RuntimeError("bench.py: no CUDA device -- the CUDA arm has no CPU fallback")
     torch.cuda.set_device(local)
     if world > 1 and not dist.is_initialized():
         dist.init_process_group("nccl", device_id=torch.device(f"cuda:{local}"))
@@ -614,9 +640,9 @@ def run_config(args):
     burst, sustained, how = measured_peaks()
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            hbm = float(json.load(f).get("hbm_gbs", 6570.0))
+            hbm = float(json.load(f).get("hbm_gbs", 3350.0))
     except (OSError, ValueError):
-        hbm = 6570.0
+        hbm = 3350.0          # NVIDIA H100 SXM data sheet HBM3 rate (not measured)
     sampler = ClockSampler(local)
     if args.config in (1, 3):
         sys.path.insert(0, os.path.join(ROOT, "tools"))
@@ -671,17 +697,17 @@ def run_config(args):
                                            3: "BASELINE config 3: Swin-S 3D window attention + FPN + FCOS head (OBB), 200x200x130 RGBsigma grid"}[args.config],
                               "precision": model.precision, "scenes_per_step_per_gpu": 1, "parallelism": f"dp{world} (independent scenes per rank)",
                               "l2": "3 distinct input grids cycled" + ("; the 32^3 working set is L2-resident by nature of the configuration" if args.config == 1 else
-                                                                       " (3 x 83 MB) and ~1 GB of activations per scene stream through the 126 MB L2"),
+                                                                       " (3 x 83 MB) and ~1 GB of activations per scene stream through the 50 MB L2"),
                               "proposals_last_scene": int(plan.out_count[0].item())},
                    "clocks": clocks,
                    "e2e": {"value": world * K / (ms_e2e * 1e-3), "unit": "scenes/s", "ms_per_step": ms_e2e / K, "h2d_bytes_per_step": int(host[0].numel() * 4),
                            "d2h_bytes_per_step": int(d2h), "api": type(model).__name__ + ".forward([grid]) with the grid copied from pinned host memory and the proposals read back"},
                    "gpu_launches": plan.num_launches() * K,
-                   "roofline": {"bound": "tensor", "kernel": "whole step (all tcgen05 implicit-GEMM / attention launches of one scene)", "achieved": tf, "peak": sustained,
+                   "roofline": {"bound": "tensor", "kernel": "whole step (all wgmma implicit-GEMM / attention launches of one scene)", "achieved": tf, "peak": sustained,
                                 "unit": "TFLOP/s", "frac": tf / sustained, "traffic": None, "flops_per_step": flops,
                                 "peak_source": how + ", sustained figure (kernels timed inside a long step)",
-                                "note": "config 1 is launch-latency bound: 32^3 voxels keep a fraction of the 148 SMs busy" if args.config == 1 else
-                                        "per-kernel rows in profiles/r01_ncu_per_kernel_config3.md"},
+                                "note": "config 1 is launch-latency bound: 32^3 voxels keep a fraction of the 132 SMs busy" if args.config == 1 else
+                                        "whole-step figure; per-kernel times are not recorded"},
                    "cpu_baseline": cpu}
     else:
         # ---- config 5: oriented 3-D IoU + NMS, n = 1k .. 1M boxes of one scene (tools/nms_sweep.py distribution), threshold 0.3
@@ -757,7 +783,7 @@ def run_config(args):
                                 "achieved": top["gb_per_s"], "peak": hbm, "unit": "GB/s", "frac": top["gb_per_s"] / hbm, "traffic": None,
                                 "algorithmic_bytes": "32 B per input box + 8 B per kept index (SURVEY 8d)",
                                 "note": "greedy NMS is bound by the pair tests (cull arithmetic + polygon clips) and their dependency chain, not by HBM: the fraction is "
-                                        "reported because the contract asks for it; the per-kernel split is in profiles/"},
+                                        "reported for completeness; per-kernel times are not recorded"},
                    "cpu_baseline": {"value": nb / cpu_s, "unit": "boxes/s", "cores": 1, "kind": "port",
                                     "sample": f"oracle/box.py nms (C restatement of utils.py:215-265 + cal_iou_3d) on {nb} boxes of the same distribution: {cpu_s:.1f} s; "
                                               "the cost grows ~ n x kept, so boxes/s at 1M would be far lower"}}
@@ -877,7 +903,7 @@ def run_train(args):
                "gpu_launches": None,
                "roofline": {"bound": "tensor", "kernel": "whole training step (forward + dgrad + wgrad = 3 x the forward's convolution FLOPs)", "achieved": tf,
                             "peak": sustained, "unit": "TFLOP/s", "frac": tf / sustained, "traffic": None, "flops_per_step": 3.0 * FLOPS_PER_SCENE,
-                            "peak_source": how + ", sustained figure", "note": "per-kernel split: profiles/r02_train_step_kernels.md"},
+                            "peak_source": how + ", sustained figure", "note": "whole-step figure; per-kernel times are not recorded"},
                "cpu_baseline": cpu}
         _emit(out)
     del eng, model
@@ -912,6 +938,8 @@ def main():
         _emit(_train_reference_cpu())
     elif args.impl == "reference":
         run_reference(args)
+    elif args.dump_outputs and (args.mode != "infer" or args.config != 2):
+        raise SystemExit("bench.py: --dump-outputs is implemented for the headline inference run (--mode infer --config 2)")
     elif args.mode == "train":
         run_train(args)
     elif args.config != 2:

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Launch one of the reference's UNMODIFIED drivers (run_rpn.py / run_fcos.py) on the B200 path:
+"""Launch one of the reference's UNMODIFIED drivers (run_rpn.py / run_fcos.py) on this package's CUDA path:
 
     python dropin/run.py /path/to/NeRF_RPN/nerf_rpn/run_rpn.py --mode eval --backbone_type resnet ...
 

@@ -1,5 +1,5 @@
 /*
- * nerf_rpn_b200.h -- C ABI of the B200-native NeRF-RPN hot path (libnerf_rpn_b200.so).
+ * nerf_rpn_b200.h -- C ABI of the NeRF-RPN hot path (libnerf_rpn_b200.so).
  *
  * The reference (lyclyc52/NeRF_RPN) has no FFI registry: its drop-in surface is Python module paths plus
  * ONE native pybind module, `sort_vertices` (nerf_rpn/model/rotated_iou/cuda_op/sort_vert.cpp:6-34).
@@ -9,7 +9,7 @@
  *   - owns no caller memory (the caller allocates inputs, outputs and workspaces),
  *   - returns 0 on success or a negative nrpn_status; it never calls exit() (the reference's
  *     CUDA_CHECK_ERRORS does, cuda_utils.h:26-35).
- * All pointers are device pointers unless marked "host".  Kernels are compiled for sm_100a only.
+ * All pointers are device pointers unless marked "host".  Kernels are compiled for sm_90a (H100) only.
  */
 #ifndef NERF_RPN_B200_H
 #define NERF_RPN_B200_H
@@ -29,7 +29,7 @@ typedef enum {
     NRPN_ERR_UNSUPPORTED = -2,  /* shape outside what the kernels were built for */
     NRPN_ERR_WORKSPACE = -3,    /* workspace too small */
     NRPN_ERR_CUDA = -4,         /* CUDA runtime / driver error (see nrpn_last_cuda_error) */
-    NRPN_ERR_NO_DEVICE = -5     /* no sm_100 device or driver entry point unavailable */
+    NRPN_ERR_NO_DEVICE = -5     /* no sm_90 device or driver entry point unavailable */
 } nrpn_status;
 
 int nrpn_version(void);
@@ -92,7 +92,7 @@ int nrpn_nms(const float *boxes, int box_dim, const float *scores, const int32_t
              int64_t *keep, int32_t *n_keep, void *workspace, size_t workspace_bytes, nrpn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
- * 3-D convolution as an implicit GEMM on tcgen05 tensor cores (replaces every nn.Conv3d (+BatchNorm3d
+ * 3-D convolution as an implicit GEMM on wgmma tensor cores (replaces every nn.Conv3d (+BatchNorm3d
  * +ReLU +residual / FPN top-down add) on the path: feature_extractor.py:31-68,145-235, anchor.py:177-213).
  *
  * Layouts (all bf16 unless stated):
@@ -305,8 +305,8 @@ int nrpn_assign_targets(const float *anchors, int n_anchors, const float *gt, in
                         int64_t *matched_idxs, void *workspace, size_t workspace_bytes, nrpn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------ weight gradient
- * dW[tap][co][ci] = sum_v dY[v][co] * X[v + tap_off][ci] of a stride-1 convolution (training, SURVEY.md 8(a) a18) on tcgen05.
- * operand_layout 1 (what the training engine uses): both operands are read channels-last where they live (MN-major tcgen05 operands).
+ * dW[tap][co][ci] = sum_v dY[v][co] * X[v + tap_off][ci] of a stride-1 convolution (training, SURVEY.md 8(a) a18) on wgmma.
+ * operand_layout 1 (what the training engine uses): both operands are read channels-last where they live (MN-major wgmma operands).
  * operand_layout 0: both operands in PLANAR layout (N, C, X, Y, z_pitch), 16-bit (nrpn_transpose_to_planar converts a channels-last tensor);
  * levels that share the weights (RPN head on P2..P5) accumulate into the same dW.  dw: fp32 (taps, cout, cin), overwritten.
  * cout % 128 == 0; cin % 32 == 0, cin <= 256; tap z offsets in {-1, 0, +1}.  Deterministic (fixed-order reduction of the K-split partial tiles). */

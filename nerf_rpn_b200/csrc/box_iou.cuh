@@ -7,7 +7,7 @@
 //
 // Arithmetic contract: every fp32 operation is an explicitly rounded intrinsic in the reference's operation order.  Three steps
 // of the reference chain round differently on its CPU and CUDA builds; NRPN_IOU_MODE selects which build is reproduced
-// (measured on the B200 against the unmodified reference + its own K1 binary: tools/ref_gpu_probe.py, profiles/r02_ref_gpu_probe.json):
+// (measured on the GPU against the unmodified reference + its own K1 binary: tools/ref_gpu_probe.py):
 //   bit 0 (operation order of the torch-CUDA kernels): box2corners_th's 4x2 * 2x2 torch.bmm = fma(y4, r1, x4 * r0); torch.sum over
 //         the 24 masked vertices = four interleaved accumulators, ((a0 + a1) + a2) + a3; torch.sum over the 8 shoelace terms =
 //         (t0+t4 + t2+t6) + (t1+t5 + t3+t7).  Mode bit clear: separately rounded mul/mul/add and left-to-right sums, the order of

@@ -1,4 +1,4 @@
-// 3-D convolution as an implicit GEMM on tcgen05 tensor cores (sm_100a).
+// 3-D convolution as an implicit GEMM on Hopper warpgroup MMA (wgmma, sm_90a).
 //
 // Replaces every nn.Conv3d (+ BatchNorm3d + ReLU + residual / FPN top-down add) of the reference path
 // (feature_extractor.py:31-68,145-235; anchor.py:177-213), which runs them as separate cuDNN / ATen kernels on
@@ -8,23 +8,25 @@
 //   - M tile  = a brick of bx*by*bz = 128 output voxels.  The A operand of one (tap, 64-channel) k-block is the
 //     same brick shifted by the tap offset: ONE 5-D TMA box load {64 ch, bz, by, bx, 1} from the channels-last
 //     activation tensor, out-of-bounds voxels zero-filled by TMA (= the convolution's zero padding).  The box
-//     lands in shared memory as 128 rows x 128 bytes in the 128B-swizzled K-major layout tcgen05.mma consumes:
+//     lands in shared memory as 128 rows x 128 bytes in the 128B-swizzled K-major layout wgmma consumes:
 //     no im2col buffer, no index arithmetic on the SM.
 //   - N tile  = 64 / 128 / 256 output channels; W is pre-packed (tap, Cout, Cin) so a k-block of weights is a
 //     3-D TMA box {64, N, 1}.
-//   - warp 0 = TMA producer, warp 1 = tcgen05.mma issuer (converged warps, one elect.sync lane issues the async
-//     instructions), warps 2-5 = epilogue.  smem ring of 2-8 stages (full/empty mbarriers), accumulators double-buffered
-//     in TMEM (2 x N columns) so the epilogue of tile i overlaps the main loop of tile i+1.  Persistent CTAs walk a static
+//   - warps 0-7 = two consumer warpgroups (rows 0-63 / 64-127 of the tile: m64nNk16 wgmma into register accumulators,
+//     then the epilogue straight from those registers), warp 8 = TMA producer (one elect.sync lane issues the loads).  smem
+//     ring of 2-8 stages (full/empty mbarriers); a stage is released once the MMAs that read it have retired (wait_group 1),
+//     so the producer streams the next tile's operands while the consumers run the epilogue.  Persistent CTAs walk a static
 //     tile list that may span up to 4 pyramid levels sharing the same weights (the RPN head on P2..P5 is ONE launch per
-//     layer).  Prologue (barriers, TMEM, tensor-map prefetch) runs ahead of griddepcontrol.wait (programmatic dependent launch).
+//     layer).  Prologue (barriers, tensor-map prefetch) runs ahead of griddepcontrol.wait (programmatic dependent launch).
 //   - epilogue (fused): + shift (bias / folded BN), + residual (same shape, or nearest-upsampled coarser level for the FPN
-//     top-down path), ReLU / GELU, convert to bf16 / fp16 / fp32; 256-bit register stores, or -- TMA_EPI variant of the 1^3
-//     layers -- residual tiles prefetched by TMA into shared memory and output tiles stored with cp.async.bulk.tensor.
+//     top-down path), ReLU / GELU, convert to bf16 / fp16 / fp32; or -- TMA_EPI variant of the 1^3 layers -- residual tiles
+//     prefetched by TMA into shared memory and output tiles stored with cp.async.bulk.tensor.
 //   - variants: <256,4,1> <128,6,1> <64,8,1> (long reductions; <64,8,1> also for layers with fewer tiles than SMs),
-//     <64,2,3> / <64,2,2,TMA_EPI> (reductions of at most 8 k-blocks), optional split-K (NRPN_SPLITK=1, measured slower).
+//     <64,2,3> / <64,2,2,TMA_EPI> (reductions of at most 8 k-blocks), optional split-K (NRPN_SPLITK=1, off by default).
 #include <cstdlib>
+#include <type_traits>
 #include "common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 #include "conv_internal.cuh"
 
 namespace nrpn {
@@ -33,6 +35,8 @@ constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
 constexpr int kUmmaK = 16;
 constexpr int kABytes = kBlockM * kBlockK * 2;       // 16 KB
+constexpr int kConsumerThreads = 256;                // two warpgroups of 64 accumulator rows each
+constexpr int kConvThreads = kConsumerThreads + 32;  // + the TMA producer warp
 
 struct ConvLevelDev {
     int n, xo, yo, zo;
@@ -42,7 +46,6 @@ struct ConvLevelDev {
     int xr, yr, zr;          // residual extent
     float rsx, rsy, rsz;     // nearest-neighbour scale = in / out
     int ldy, ldr;
-    int wide_y, wide_r;      // rows of y / res are 32-byte aligned: 256-bit stores / loads
     int res_tma;             // TMA-epilogue variant: the residual has the output's extent and arrives through maps.r
     void* y;
     const __nv_bfloat16* res;
@@ -66,34 +69,68 @@ struct ConvMaps {
     CUtensorMap r[NRPN_CONV_MAX_LEVELS];      // ... and same-shape residual tiles are prefetched by the producer warp
 };
 
-__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&v);
+constexpr int kEpiTileBytes = kBlockM * 64 * 2;      // one 128 x 64 bf16 tile (residual in / output out of the TMA epilogue)
+
+struct TilePos { int l, tix, tiy, tiz, nb; };
+
+__device__ __forceinline__ TilePos tile_pos(const ConvDev& P, int m_tile) {
+    TilePos p;
+    p.l = 0;
+#pragma unroll
+    for (int i = 1; i < NRPN_CONV_MAX_LEVELS; ++i) if (i < P.n_levels && m_tile >= P.lv[i].tile_begin) p.l = i;
+    const ConvLevelDev& L = P.lv[p.l];
+    int t = m_tile - L.tile_begin;
+    p.tiz = t % L.tz; t /= L.tz;
+    p.tiy = t % L.ty; t /= L.ty;
+    p.tix = t % L.tx; p.nb = t / L.tx;
+    return p;
 }
 
-constexpr int kEpiTileBytes = kBlockM * 64 * 2;      // one 128 x 64 bf16 tile (residual in / output out of the TMA epilogue)
+// Output voxel of accumulator row `row` of a tile, and the residual row that is added to it (nullptr: none).
+struct RowPos { bool valid; size_t vox; const __nv_bfloat16* rrow; };
+
+__device__ __forceinline__ RowPos row_pos(const ConvLevelDev& L, const TilePos& p, int row) {
+    RowPos r;
+    const int zi = row % L.bz, yi = (row / L.bz) % L.by, xi = row / (L.bz * L.by);
+    const int gx = p.tix * L.bx + xi, gy = p.tiy * L.by + yi, gz = p.tiz * L.bz + zi;
+    r.valid = gx < L.xo && gy < L.yo && gz < L.zo;
+    r.vox = (((size_t)p.nb * L.xo + gx) * L.yo + gy) * L.zo + gz;
+    r.rrow = nullptr;
+    if (L.res != nullptr && r.valid) {
+        int rx = gx, ry = gy, rz = gz;
+        if (L.xr != L.xo || L.yr != L.yo || L.zr != L.zo) {   // F.interpolate(mode='nearest', size=...)
+            rx = min((int)floorf((float)gx * L.rsx), L.xr - 1);
+            ry = min((int)floorf((float)gy * L.rsy), L.yr - 1);
+            rz = min((int)floorf((float)gz * L.rsz), L.zr - 1);
+        }
+        r.rrow = L.res + ((((size_t)p.nb * L.xr + rx) * L.yr + ry) * L.zr + rz) * L.ldr;
+    }
+    return r;
+}
+
+__device__ __forceinline__ float activate(float v, int relu) {
+    if (relu == 1) return fmaxf(v, 0.0f);
+    if (relu == 2) return 0.5f * v * (1.0f + erff(v * 0.70710678118654752f));     // exact (erf) GELU: Swin MLP, feature_extractor.py:635
+    return v;
+}
 
 // TMA_EPI (N = 64 tiles of the HBM-bound 1^3 layers, bf16 output, Cout % 64 == 0): the epilogue never touches global memory
 // from a register.  The producer warp prefetches the residual tile of a same-shape skip connection into shared memory
-// (2-deep ring) together with the operands; the epilogue warps add it from shared memory, write the bf16 tile into a
-// swizzled staging buffer and one elected thread stores it with cp.async.bulk.tensor (hardware clips partial bricks).
-// With per-thread 16/32-byte global loads and stores the same layers sat at ~45 % of the HBM rate (ncu: lts 45 %, 2-3x the
-// compulsory L2 sectors, a DRAM-latency chain per tile).
+// (2-deep ring) together with the operands; the consumers add it from shared memory, write the 16-bit tile into a
+// swizzled staging buffer and one thread stores it with cp.async.bulk.tensor (hardware clips partial bricks).
 //
 // WS (weight split, the <=1e-3 parity mode of the backbone): every weight is the sum of TWO 16-bit numbers, w = hi + lo with
 // lo = round16(w - hi), packed as (taps, 2, CoutPad, Cin).  One TMA box {64, BLOCK_N, 2} brings both planes of a k-block; the
-// issuer runs the k-block's MMAs twice on the SAME activation tile (B = hi, then B = lo) into the same accumulator, so the
+// consumers run the k-block's MMAs twice on the SAME activation tile (B = hi, then B = lo) into the same accumulator, so the
 // weights enter the fp32 accumulation with ~22 significant bits and only the activations carry 16-bit rounding error.
 template <int BLOCK_N, int STAGES, int MIN_BLOCKS, bool TMA_EPI = false, bool WS = false>
-__global__ void __launch_bounds__(192, MIN_BLOCKS) conv3d_igemm_kernel(const __grid_constant__ ConvMaps maps, const ConvDev P) {
+__global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(const __grid_constant__ ConvMaps maps, const ConvDev P) {
     static_assert(!TMA_EPI || BLOCK_N == 64, "the TMA epilogue stages 128 x 64 tiles");
     constexpr int kBPlane = BLOCK_N * kBlockK * 2;
     constexpr int kBBytes = kBPlane * (WS ? 2 : 1);
     constexpr int kStageBytes = kABytes + kBBytes;
     constexpr int RES_SLOTS = (TMA_EPI && WS) ? 1 : 2;              // residual prefetch depth (shared-memory budget of 2 CTAs / SM)
     constexpr int kEpiBytes = TMA_EPI ? (RES_SLOTS + 1) * kEpiTileBytes : 0;      // residual ring + output staging (1)
-    constexpr uint32_t kTmemCols = 2 * BLOCK_N;
-    const uint32_t kIdesc = P.fp16 ? ptx::make_idesc_f16(kBlockM, BLOCK_N) : ptx::make_idesc_bf16(kBlockM, BLOCK_N);
 
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -102,382 +139,227 @@ __global__ void __launch_bounds__(192, MIN_BLOCKS) conv3d_igemm_kernel(const __g
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * kStageBytes + kEpiBytes);
     uint64_t* full_bar = bars;
     uint64_t* empty_bar = bars + STAGES;
-    uint64_t* tfull_bar = bars + 2 * STAGES;
-    uint64_t* tempty_bar = bars + 2 * STAGES + 2;
-    uint64_t* rfull_bar = bars + 2 * STAGES + 4;
-    uint64_t* rempty_bar = bars + 2 * STAGES + 6;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 8);
+    uint64_t* rfull_bar = bars + 2 * STAGES;
+    uint64_t* rempty_bar = bars + 2 * STAGES + 2;
+    uint32_t* ticket_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-        for (int a = 0; a < 2; ++a) { ptx::mbar_init(&tfull_bar[a], 1); ptx::mbar_init(&tempty_bar[a], 128); }
-        for (int a = 0; a < 2; ++a) { ptx::mbar_init(&rfull_bar[a], 1); ptx::mbar_init(&rempty_bar[a], 128); }
+        for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 2); }   // one arrival per consumer warpgroup
+        for (int a = 0; a < 2; ++a) { ptx::mbar_init(&rfull_bar[a], 1); ptx::mbar_init(&rempty_bar[a], 1); }
         ptx::fence_barrier_init();
         for (int l = 0; l < P.n_levels; ++l) ptx::prefetch_tmap(&maps.x[l]);
         if (TMA_EPI) for (int l = 0; l < P.n_levels; ++l) { ptx::prefetch_tmap(&maps.y[l]); ptx::prefetch_tmap(&maps.r[l]); }
         ptx::prefetch_tmap(&maps.w);
     }
-    if (warp == 1) { ptx::tmem_alloc(tmem_slot, kTmemCols); ptx::tmem_relinquish(); }
     ptx::pdl_trigger();                 // the next layer may start its own prologue as our CTAs retire
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     ptx::pdl_wait();                    // everything above overlapped the previous layer's tail; its outputs are visible from here
 
     const int total_tiles = P.total_m_tiles * P.n_tiles_n * P.splits;     // work items = (output tile, k-split)
     const int kblocks = P.n_taps * P.kc_blocks;
-    uint32_t* ticket_slot = tmem_slot + 1;
 
-    if (warp == 0) {
+    if (warp == kConsumerThreads / 32) {
         // ------------------------------------------------------------------ TMA producer (whole warp walks, one elected lane issues)
-        {
-            const bool leader = ptx::elect_one();
-            int stage = 0; uint32_t phase = 0;
-            int rslot = 0; uint32_t rphase = 0;
-            for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
-                const int split = item % P.splits, tile = item / P.splits;
-                const int kb0 = (kblocks * split) / P.splits, kb1 = (kblocks * (split + 1)) / P.splits;
-                const int n_tile = tile % P.n_tiles_n, m_tile = tile / P.n_tiles_n;
-                int l = 0;
-#pragma unroll
-                for (int i = 1; i < NRPN_CONV_MAX_LEVELS; ++i) if (i < P.n_levels && m_tile >= P.lv[i].tile_begin) l = i;
-                const ConvLevelDev& L = P.lv[l];
-                int t = m_tile - L.tile_begin;
-                const int tiz = t % L.tz; t /= L.tz;
-                const int tiy = t % L.ty; t /= L.ty;
-                const int tix = t % L.tx; const int nb = t / L.tx;
-                const int x0 = tix * L.bx, y0 = tiy * L.by, z0 = tiz * L.bz, n0 = n_tile * BLOCK_N;
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    const int tap = kb / P.kc_blocks, kc = kb - tap * P.kc_blocks;
-                    const int dx = P.tap[tap][0], dy = P.tap[tap][1], dz = P.tap[tap][2];
-                    ptx::mbar_wait(&empty_bar[stage], phase ^ 1u);
-                    if (leader) {
-                        uint8_t* sa = smem + stage * kStageBytes;
-                        uint8_t* sb = sa + kABytes;
-                        ptx::mbar_expect_tx(&full_bar[stage], kStageBytes);
-                        ptx::tma_load_5d(sa, &maps.x[l], &full_bar[stage], kc * kBlockK, z0 + dz, y0 + dy, x0 + dx, nb);
-                        ptx::tma_load_3d(sb, &maps.w, &full_bar[stage], kc * kBlockK, n0, WS ? 2 * tap : tap);   // WS: box depth 2 = hi, lo
-                    }
-                    __syncwarp();
-                    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-                }
-                if (TMA_EPI && L.res_tma) {                          // residual tile of this output tile, two tiles ahead of its use
-                    ptx::mbar_wait(&rempty_bar[rslot], rphase ^ 1u);
-                    if (leader) {
-                        ptx::mbar_expect_tx(&rfull_bar[rslot], kEpiTileBytes);
-                        ptx::tma_load_5d(smem_res + rslot * kEpiTileBytes, &maps.r[l], &rfull_bar[rslot], n0, z0, y0, x0, nb);
-                    }
-                    __syncwarp();
-                    if (++rslot == RES_SLOTS) { rslot = 0; rphase ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer
-        // The whole warp walks the warp-uniform loops and waits; one elected lane (elect.sync) issues tcgen05.mma and
-        // tcgen05.commit, which keeps descriptors in uniform registers (no per-instruction waterfall loop: at N = 64 an
-        // MMA lasts 48 clk and a divergent `if (lane == 0)` issue path costs more than that, profiles/r01_ncu_slab_*.md).
-        {
-            const bool leader = ptx::elect_one();
-            int stage = 0; uint32_t phase = 0;
-            int acc = 0; uint32_t acc_phase = 0;
-            for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
-                const int split = item % P.splits;
-                const int nkb = (kblocks * (split + 1)) / P.splits - (kblocks * split) / P.splits;
-                ptx::mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-                ptx::tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BLOCK_N);
-                for (int kb = 0; kb < nkb; ++kb) {
-                    ptx::mbar_wait(&full_bar[stage], phase);
-                    ptx::tc_fence_after();
-                    const uint32_t sa = ptx::smem_u32(smem + stage * kStageBytes);
-                    const uint64_t da = ptx::make_desc_sw128(sa);
-                    const uint64_t db = ptx::make_desc_sw128(sa + kABytes);
-                    if (leader) {
-#pragma unroll
-                        for (int h = 0; h < (WS ? 2 : 1); ++h) {
-#pragma unroll
-                            for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-                                // advance 16 elements (32 bytes) along K inside the 128-byte swizzle atom: +2 in the >>4 address field
-                                ptx::umma_bf16(d_tmem, da + (uint64_t)(2 * k), db + (uint64_t)(h * (kBPlane >> 4) + 2 * k), kIdesc, (kb | k | h) ? 1u : 0u);
-                            }
-                        }
-                        ptx::umma_commit(&empty_bar[stage]);        // frees the smem slot once the MMAs have read it
-                    }
-                    __syncwarp();
-                    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-                }
-                if (leader) ptx::umma_commit(&tfull_bar[acc]);      // accumulator complete -> epilogue
-                __syncwarp();
-                if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-            }
-        }
-    } else {
-        // ------------------------------------------------------------------ epilogue (warps 2..5)
-        const int q = warp & 3;                          // TMEM lane quarter this warp may access
-        const int row = q * 32 + lane;                   // accumulator row == voxel inside the brick
-        int acc = 0; uint32_t acc_phase = 0;
+        const bool leader = ptx::elect_one();
+        int stage = 0; uint32_t phase = 0;
         int rslot = 0; uint32_t rphase = 0;
         for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
-            const int tile = item / P.splits;
+            const int split = item % P.splits, tile = item / P.splits;
+            const int kb0 = (kblocks * split) / P.splits, kb1 = (kblocks * (split + 1)) / P.splits;
             const int n_tile = tile % P.n_tiles_n, m_tile = tile / P.n_tiles_n;
-            int l = 0;
-#pragma unroll
-            for (int i = 1; i < NRPN_CONV_MAX_LEVELS; ++i) if (i < P.n_levels && m_tile >= P.lv[i].tile_begin) l = i;
-            const ConvLevelDev& L = P.lv[l];
-            int t = m_tile - L.tile_begin;
-            const int tiz = t % L.tz; t /= L.tz;
-            const int tiy = t % L.ty; t /= L.ty;
-            const int tix = t % L.tx; const int nb = t / L.tx;
-            const int zi = row % L.bz, yi = (row / L.bz) % L.by, xi = row / (L.bz * L.by);
-            const int gx = tix * L.bx + xi, gy = tiy * L.by + yi, gz = tiz * L.bz + zi;
-            const bool valid = gx < L.xo && gy < L.yo && gz < L.zo;
-            const size_t vox = (((size_t)nb * L.xo + gx) * L.yo + gy) * L.zo + gz;
-            const __nv_bfloat16* rrow = nullptr;
-            if (L.res != nullptr && valid) {
-                int rx = gx, ry = gy, rz = gz;
-                if (L.xr != L.xo || L.yr != L.yo || L.zr != L.zo) {   // F.interpolate(mode='nearest', size=...)
-                    rx = min((int)floorf((float)gx * L.rsx), L.xr - 1);
-                    ry = min((int)floorf((float)gy * L.rsy), L.yr - 1);
-                    rz = min((int)floorf((float)gz * L.rsz), L.zr - 1);
+            const TilePos tp = tile_pos(P, m_tile);
+            const ConvLevelDev& L = P.lv[tp.l];
+            const int x0 = tp.tix * L.bx, y0 = tp.tiy * L.by, z0 = tp.tiz * L.bz, n0 = n_tile * BLOCK_N;
+            for (int kb = kb0; kb < kb1; ++kb) {
+                const int tap = kb / P.kc_blocks, kc = kb - tap * P.kc_blocks;
+                const int dx = P.tap[tap][0], dy = P.tap[tap][1], dz = P.tap[tap][2];
+                ptx::mbar_wait(&empty_bar[stage], phase ^ 1u);
+                if (leader) {
+                    uint8_t* sa = smem + stage * kStageBytes;
+                    uint8_t* sb = sa + kABytes;
+                    ptx::mbar_expect_tx(&full_bar[stage], kStageBytes);
+                    ptx::tma_load_5d(sa, &maps.x[tp.l], &full_bar[stage], kc * kBlockK, z0 + dz, y0 + dy, x0 + dx, tp.nb);
+                    ptx::tma_load_3d(sb, &maps.w, &full_bar[stage], kc * kBlockK, n0, WS ? 2 * tap : tap);   // WS: box depth 2 = hi, lo
                 }
-                rrow = L.res + ((((size_t)nb * L.xr + rx) * L.yr + ry) * L.zr + rz) * L.ldr;
+                __syncwarp();
+                if (++stage == STAGES) { stage = 0; phase ^= 1u; }
             }
-            const int n0 = n_tile * BLOCK_N;
+            if (TMA_EPI && L.res_tma) {                          // residual tile of this output tile, two tiles ahead of its use
+                ptx::mbar_wait(&rempty_bar[rslot], rphase ^ 1u);
+                if (leader) {
+                    ptx::mbar_expect_tx(&rfull_bar[rslot], kEpiTileBytes);
+                    ptx::tma_load_5d(smem_res + rslot * kEpiTileBytes, &maps.r[tp.l], &rfull_bar[rslot], n0, z0, y0, x0, tp.nb);
+                }
+                __syncwarp();
+                if (++rslot == RES_SLOTS) { rslot = 0; rphase ^= 1u; }
+            }
+        }
+        return;
+    }
 
-            if (P.splits > 1) {
-                // ---- split-K (deterministic): every CTA stores its partial tile into its own fp32 slab of the workspace with
-                // plain stores; the last CTA to arrive sums the slabs in split order and runs the normal epilogue.
-                const int split = item % P.splits;
-                float* slab0 = P.ws + ((size_t)tile * P.splits) * (kBlockM * BLOCK_N);          // slabs of this output tile
-                float* wrow = slab0 + (size_t)split * (kBlockM * BLOCK_N) + (size_t)row * BLOCK_N;
-                ptx::mbar_wait(&tfull_bar[acc], acc_phase);
-                ptx::tc_fence_after();
-                const uint32_t t_base = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BLOCK_N);
-#pragma unroll 1
-                for (int c = 0; c < BLOCK_N / 32; ++c) {
-                    uint32_t r[32];
-                    ptx::tmem_ld_32x32(t_base + (uint32_t)(c * 32), r);
-                    ptx::tmem_ld_wait();
-                    if (valid) {
+    // ---------------------------------------------------------------------- consumers (warpgroups 0 and 1): MMA + epilogue
+    const int t = threadIdx.x & 127, wg = threadIdx.x >> 7;
+    int stage = 0; uint32_t phase = 0;
+    int rslot = 0; uint32_t rphase = 0;
+    float acc[BLOCK_N / 2];
+    for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
+        const int split = item % P.splits, tile = item / P.splits;
+        const int nkb = (kblocks * (split + 1)) / P.splits - (kblocks * split) / P.splits;
+        const int n_tile = tile % P.n_tiles_n, m_tile = tile / P.n_tiles_n;
+        const TilePos tp = tile_pos(P, m_tile);
+        const ConvLevelDev& L = P.lv[tp.l];
+        const int n0 = n_tile * BLOCK_N;
+
+        ptx::reg_fence(acc);
+        int prev = 0;
+        for (int kb = 0; kb < nkb; ++kb) {
+            ptx::mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa = ptx::smem_u32(smem + stage * kStageBytes);
+            const uint64_t da = ptx::make_desc_sw128(sa + (uint32_t)(wg * (kABytes / 2)));      // this warpgroup's 64 rows
+            const uint64_t db = ptx::make_desc_sw128(sa + kABytes);
+            // one branch per k-block on the activation format, so that each path is an unbroken chain of MMAs
+            auto issue = [&](auto f16) {
+                ptx::wgmma_fence();
 #pragma unroll
-                        for (int j = 0; j < 32; j += 4)
-                            __stcg(reinterpret_cast<float4*>(wrow + c * 32 + j),
-                                   make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3])));
-                    }
+                for (int h = 0; h < (WS ? 2 : 1); ++h) {
+#pragma unroll
+                    for (int k = 0; k < kBlockK / kUmmaK; ++k)
+                        // advance 16 elements (32 bytes) along K inside the 128-byte swizzle atom: +2 in the >>4 address field
+                        ptx::Wgmma<BLOCK_N, decltype(f16)::value>::template ss<0, 0>(
+                            acc, da + (uint64_t)(2 * k), db + (uint64_t)(h * (kBPlane >> 4) + 2 * k), (kb | k | h) ? 1u : 0u);
                 }
-                ptx::tc_fence_before();
-                ptx::mbar_arrive(&tempty_bar[acc]);
-                if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
+                ptx::wgmma_commit();
+            };
+            if (P.fp16) issue(std::true_type{}); else issue(std::false_type{});
+            ptx::wgmma_wait<1>();                            // the previous k-block's MMAs have retired: its stage is free
+            if (kb > 0 && t == 0) ptx::mbar_arrive(&empty_bar[prev]);
+            prev = stage;
+            if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+        }
+        ptx::wgmma_wait<0>();
+        ptx::reg_fence(acc);
+        if (nkb > 0 && t == 0) ptx::mbar_arrive(&empty_bar[prev]);
+
+        if (P.splits > 1) {
+            // ---- split-K (deterministic): every CTA stores its partial tile into its own fp32 slab of the workspace with
+            // plain stores; the last CTA to arrive sums the slabs in split order and runs the normal epilogue.
+            float* slab0 = P.ws + ((size_t)tile * P.splits) * (kBlockM * BLOCK_N);          // slabs of this output tile
+            float* wslab = slab0 + (size_t)split * (kBlockM * BLOCK_N);
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    __stcg(reinterpret_cast<float2*>(wslab + (size_t)(wg * 64 + ptx::frag_row(t, h)) * BLOCK_N + ptx::frag_col(t, j)),
+                           make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
+            __threadfence();
+            ptx::named_barrier(1, kConsumerThreads);
+            if (threadIdx.x == 0) *ticket_slot = atomicAdd(P.counters + tile, 1u);
+            ptx::named_barrier(1, kConsumerThreads);
+            const bool last = (*ticket_slot == (uint32_t)(P.splits - 1));
+            if (last && threadIdx.x < kBlockM) {
                 __threadfence();
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                if (row == 0) *ticket_slot = atomicAdd(P.counters + tile, 1u);
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                const bool last = (*ticket_slot == (uint32_t)(P.splits - 1));
-                if (last) {
-                    __threadfence();
-                    if (valid) {
-                        const float* rrow0 = slab0 + (size_t)row * BLOCK_N;
-                        for (int ch = n0; ch < n0 + BLOCK_N && ch < P.cout; ch += 8) {
-                            float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), a1 = a0;
-                            for (int sp = 0; sp < P.splits; ++sp) {                                  // fixed order => reproducible
-                                const float* wp = rrow0 + (size_t)sp * (kBlockM * BLOCK_N) + (ch - n0);
-                                const float4 b0 = __ldcg(reinterpret_cast<const float4*>(wp));
-                                const float4 b1 = __ldcg(reinterpret_cast<const float4*>(wp + 4));
-                                a0.x += b0.x; a0.y += b0.y; a0.z += b0.z; a0.w += b0.w;
-                                a1.x += b1.x; a1.y += b1.y; a1.z += b1.z; a1.w += b1.w;
-                            }
-                            const float4 s0 = __ldg(reinterpret_cast<const float4*>(P.shift + ch));
-                            const float4 s1 = __ldg(reinterpret_cast<const float4*>(P.shift + ch + 4));
-                            float v[8] = {a0.x + s0.x, a0.y + s0.y, a0.z + s0.z, a0.w + s0.w, a1.x + s1.x, a1.y + s1.y, a1.z + s1.z, a1.w + s1.w};
-                            if (rrow != nullptr) {
-                                const uint4 rv4 = __ldg(reinterpret_cast<const uint4*>(rrow + ch));
-                                const uint32_t* rb = reinterpret_cast<const uint32_t*>(&rv4);
-#pragma unroll
-                                for (int i = 0; i < 4; ++i) { const float2 f = unpack_act2(rb[i], P.fp16); v[2 * i] += f.x; v[2 * i + 1] += f.y; }
-                            }
-                            if (P.relu == 1) {
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) v[i] = fmaxf(v[i], 0.0f);
-                            } else if (P.relu == 2) {
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) v[i] = 0.5f * v[i] * (1.0f + erff(v[i] * 0.70710678118654752f));
-                            }
-                            if (P.out_fp32) {
-                                float* o = reinterpret_cast<float*>(L.y) + vox * L.ldy + ch;
-                                *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
-                                *reinterpret_cast<float4*>(o + 4) = make_float4(v[4], v[5], v[6], v[7]);
-                            } else {
-                                __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(L.y) + vox * L.ldy + ch;
-                                *reinterpret_cast<uint4*>(o) = make_uint4(pack_act2(v[0], v[1], P.fp16), pack_act2(v[2], v[3], P.fp16),
-                                                                          pack_act2(v[4], v[5], P.fp16), pack_act2(v[6], v[7], P.fp16));
-                            }
+                const int row = threadIdx.x;                 // one accumulator row per thread
+                const RowPos rp = row_pos(L, tp, row);
+                if (rp.valid) {
+                    const float* rrow0 = slab0 + (size_t)row * BLOCK_N;
+                    for (int ch = n0; ch < n0 + BLOCK_N && ch < P.cout; ch += 8) {
+                        float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), a1 = a0;
+                        for (int sp = 0; sp < P.splits; ++sp) {                                  // fixed order => reproducible
+                            const float* wp = rrow0 + (size_t)sp * (kBlockM * BLOCK_N) + (ch - n0);
+                            const float4 b0 = __ldcg(reinterpret_cast<const float4*>(wp));
+                            const float4 b1 = __ldcg(reinterpret_cast<const float4*>(wp + 4));
+                            a0.x += b0.x; a0.y += b0.y; a0.z += b0.z; a0.w += b0.w;
+                            a1.x += b1.x; a1.y += b1.y; a1.z += b1.z; a1.w += b1.w;
                         }
-                    }
-                    if (row == 0) P.counters[tile] = 0u;
-                }
-                asm volatile("bar.sync 1, 128;" ::: "memory");     // ticket_slot is reused by the next work item
-                continue;
-            }
-            if constexpr (TMA_EPI) {
-                // ---- shared-memory epilogue: residual from the TMA-fed ring, output through a swizzled staging tile + TMA store
-                const bool res_smem = L.res_tma != 0;
-                ptx::mbar_wait(&tfull_bar[acc], acc_phase);
-                if (res_smem) ptx::mbar_wait(&rfull_bar[rslot], rphase);
-                ptx::tc_fence_after();
-                // the staging tile is free once the previous tile's bulk store has finished READING it
-                if (threadIdx.x == 64) ptx::bulk_wait_read0();
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                const uint32_t t_base = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BLOCK_N);
-                const uint8_t* rsm = smem_res + rslot * kEpiTileBytes + row * 128;
-                uint8_t* osm = smem_out + row * 128;
-                const int sw = row & 7;
-#pragma unroll 1
-                for (int c = 0; c < 2; ++c) {
-                    uint32_t r[32];
-                    ptx::tmem_ld_32x32(t_base + (uint32_t)(c * 32), r);
-                    ptx::tmem_ld_wait();
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const int j = c * 4 + g;                     // 16-byte chunk (8 channels) inside the 128-byte row
-                        const int ch = n0 + j * 8;
                         const float4 s0 = __ldg(reinterpret_cast<const float4*>(P.shift + ch));
                         const float4 s1 = __ldg(reinterpret_cast<const float4*>(P.shift + ch + 4));
-                        float v[8] = {__uint_as_float(r[g * 8 + 0]) + s0.x, __uint_as_float(r[g * 8 + 1]) + s0.y,
-                                      __uint_as_float(r[g * 8 + 2]) + s0.z, __uint_as_float(r[g * 8 + 3]) + s0.w,
-                                      __uint_as_float(r[g * 8 + 4]) + s1.x, __uint_as_float(r[g * 8 + 5]) + s1.y,
-                                      __uint_as_float(r[g * 8 + 6]) + s1.z, __uint_as_float(r[g * 8 + 7]) + s1.w};
-                        if (res_smem || rrow != nullptr) {
-                            const uint4 rv4 = res_smem ? *reinterpret_cast<const uint4*>(rsm + ((j ^ sw) << 4))
-                                                       : __ldg(reinterpret_cast<const uint4*>(rrow + ch));
+                        float v[8] = {a0.x + s0.x, a0.y + s0.y, a0.z + s0.z, a0.w + s0.w, a1.x + s1.x, a1.y + s1.y, a1.z + s1.z, a1.w + s1.w};
+                        if (rp.rrow != nullptr) {
+                            const uint4 rv4 = __ldg(reinterpret_cast<const uint4*>(rp.rrow + ch));
                             const uint32_t* rb = reinterpret_cast<const uint32_t*>(&rv4);
 #pragma unroll
                             for (int i = 0; i < 4; ++i) { const float2 f = unpack_act2(rb[i], P.fp16); v[2 * i] += f.x; v[2 * i + 1] += f.y; }
                         }
-                        if (P.relu == 1) {
 #pragma unroll
-                            for (int i = 0; i < 8; ++i) v[i] = fmaxf(v[i], 0.0f);
-                        } else if (P.relu == 2) {
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) v[i] = 0.5f * v[i] * (1.0f + erff(v[i] * 0.70710678118654752f));
-                        }
-                        *reinterpret_cast<uint4*>(osm + ((j ^ sw) << 4)) =
-                            make_uint4(pack_act2(v[0], v[1], P.fp16), pack_act2(v[2], v[3], P.fp16), pack_act2(v[4], v[5], P.fp16), pack_act2(v[6], v[7], P.fp16));
-                    }
-                }
-                ptx::tc_fence_before();
-                ptx::mbar_arrive(&tempty_bar[acc]);
-                if (res_smem) { ptx::mbar_arrive(&rempty_bar[rslot]); if (++rslot == RES_SLOTS) { rslot = 0; rphase ^= 1u; } }
-                if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-                ptx::fence_proxy_async();                            // generic-proxy smem writes -> visible to the TMA engine
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                if (threadIdx.x == 64) {
-                    ptx::tma_store_5d(&maps.y[l], smem_out, n0, tiz * L.bz, tiy * L.by, tix * L.bx, nb);
-                    ptx::bulk_commit();
-                }
-                continue;
-            }
-            // residual rows are fetched one 32-channel chunk ahead (2 x 32 B or 4 x 16 B per thread in flight) so that the DRAM
-            // latency of chunk c+1 hides behind the TMEM load + math + stores of chunk c
-            uint4 rv[4];
-            auto load_res = [&](int c, uint4 (&dst)[4]) {
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int ch = n0 + c * 32 + h * 16;
-                    if (rrow != nullptr && L.wide_r && ch + 16 <= P.cout) {
-                        ptx::ld_global_nc_v8(rrow + ch, dst[2 * h], dst[2 * h + 1]);
-                    } else {
-                        dst[2 * h] = (rrow != nullptr && ch < P.cout) ? __ldg(reinterpret_cast<const uint4*>(rrow + ch)) : make_uint4(0u, 0u, 0u, 0u);
-                        dst[2 * h + 1] = (rrow != nullptr && ch + 8 < P.cout) ? __ldg(reinterpret_cast<const uint4*>(rrow + ch + 8)) : make_uint4(0u, 0u, 0u, 0u);
-                    }
-                }
-            };
-            load_res(0, rv);
-            uint4 rn[4];
-            if (BLOCK_N == 64) load_res(1, rn);          // N = 64 (HBM-bound 1^3 layers): the whole residual row is in flight before the wait
-            ptx::mbar_wait(&tfull_bar[acc], acc_phase);
-            ptx::tc_fence_after();
-            const uint32_t t_base = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BLOCK_N);
-#pragma unroll 1
-            for (int c = 0; c < BLOCK_N / 32; ++c) {
-                uint32_t r[32];
-                ptx::tmem_ld_32x32(t_base + (uint32_t)(c * 32), r);
-                if (BLOCK_N != 64 && c + 1 < BLOCK_N / 32) load_res(c + 1, rn);
-                ptx::tmem_ld_wait();
-                const int ch0 = n0 + c * 32;
-                if (valid && ch0 < P.cout) {
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {            // 2 halves of 16 channels = 32 bytes of bf16
-                        const int chh = ch0 + h * 16;
-                        if (chh >= P.cout) break;
-                        float v[16];
-#pragma unroll
-                        for (int g = 0; g < 2; ++g) {
-                            const int ch = chh + g * 8;
-                            if (ch < P.cout) {
-                                const float4 s0 = __ldg(reinterpret_cast<const float4*>(P.shift + ch));
-                                const float4 s1 = __ldg(reinterpret_cast<const float4*>(P.shift + ch + 4));
-                                const uint32_t* rr = r + h * 16 + g * 8;
-                                float* vv = v + g * 8;
-                                vv[0] = __uint_as_float(rr[0]) + s0.x; vv[1] = __uint_as_float(rr[1]) + s0.y;
-                                vv[2] = __uint_as_float(rr[2]) + s0.z; vv[3] = __uint_as_float(rr[3]) + s0.w;
-                                vv[4] = __uint_as_float(rr[4]) + s1.x; vv[5] = __uint_as_float(rr[5]) + s1.y;
-                                vv[6] = __uint_as_float(rr[6]) + s1.z; vv[7] = __uint_as_float(rr[7]) + s1.w;
-                                if (rrow != nullptr) {
-                                    const uint32_t* rb = reinterpret_cast<const uint32_t*>(&rv[2 * h + g]);
-#pragma unroll
-                                    for (int i = 0; i < 4; ++i) { const float2 f = unpack_act2(rb[i], P.fp16); vv[2 * i] += f.x; vv[2 * i + 1] += f.y; }
-                                }
-                            } else {
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) v[g * 8 + i] = 0.0f;
-                            }
-                        }
-                        if (P.relu == 1) {
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.0f);
-                        } else if (P.relu == 2) {            // exact (erf) GELU: Swin MLP, feature_extractor.py:635
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) v[i] = 0.5f * v[i] * (1.0f + erff(v[i] * 0.70710678118654752f));
-                        }
-                        const bool both = chh + 16 <= P.cout;
+                        for (int i = 0; i < 8; ++i) v[i] = activate(v[i], P.relu);
                         if (P.out_fp32) {
-                            float* o = reinterpret_cast<float*>(L.y) + vox * L.ldy + chh;
-#pragma unroll
-                            for (int g = 0; g < 2; ++g) {
-                                if (chh + g * 8 >= P.cout) break;
-                                const uint4 lo = make_uint4(__float_as_uint(v[g * 8 + 0]), __float_as_uint(v[g * 8 + 1]), __float_as_uint(v[g * 8 + 2]), __float_as_uint(v[g * 8 + 3]));
-                                const uint4 hi = make_uint4(__float_as_uint(v[g * 8 + 4]), __float_as_uint(v[g * 8 + 5]), __float_as_uint(v[g * 8 + 6]), __float_as_uint(v[g * 8 + 7]));
-                                if (L.wide_y) ptx::st_global_v8(o + g * 8, lo, hi);
-                                else { *reinterpret_cast<uint4*>(o + g * 8) = lo; *reinterpret_cast<uint4*>(o + g * 8 + 4) = hi; }
-                            }
+                            float* o = reinterpret_cast<float*>(L.y) + rp.vox * L.ldy + ch;
+                            *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
+                            *reinterpret_cast<float4*>(o + 4) = make_float4(v[4], v[5], v[6], v[7]);
                         } else {
-                            __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(L.y) + vox * L.ldy + chh;
-                            const uint4 lo = make_uint4(pack_act2(v[0], v[1], P.fp16), pack_act2(v[2], v[3], P.fp16), pack_act2(v[4], v[5], P.fp16), pack_act2(v[6], v[7], P.fp16));
-                            const uint4 hi = make_uint4(pack_act2(v[8], v[9], P.fp16), pack_act2(v[10], v[11], P.fp16), pack_act2(v[12], v[13], P.fp16), pack_act2(v[14], v[15], P.fp16));
-                            if (both && L.wide_y) ptx::st_global_v8(o, lo, hi);
-                            else { *reinterpret_cast<uint4*>(o) = lo; if (both) *reinterpret_cast<uint4*>(o + 8) = hi; }
+                            __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(L.y) + rp.vox * L.ldy + ch;
+                            *reinterpret_cast<uint4*>(o) = make_uint4(pack_act2(v[0], v[1], P.fp16), pack_act2(v[2], v[3], P.fp16),
+                                                                      pack_act2(v[4], v[5], P.fp16), pack_act2(v[6], v[7], P.fp16));
                         }
                     }
                 }
-                if (c + 1 < BLOCK_N / 32) {
+                if (row == 0) P.counters[tile] = 0u;
+            }
+            ptx::named_barrier(1, kConsumerThreads);         // ticket_slot is reused by the next work item
+            continue;
+        }
+        if constexpr (TMA_EPI) {
+            // ---- shared-memory epilogue: residual from the TMA-fed ring, output through a swizzled staging tile + TMA store
+            const bool res_smem = L.res_tma != 0;
+            if (res_smem) ptx::mbar_wait(&rfull_bar[rslot], rphase);
+            // the staging tile is free once the previous tile's bulk store has finished READING it
+            if (threadIdx.x == 0) ptx::bulk_wait_read0();
+            ptx::named_barrier(1, kConsumerThreads);
+            const uint8_t* rsm = smem_res + rslot * kEpiTileBytes;
 #pragma unroll
-                    for (int g = 0; g < 4; ++g) rv[g] = rn[g];
+            for (int h = 0; h < 2; ++h) {
+                const int row = wg * 64 + ptx::frag_row(t, h);
+                const RowPos rp = res_smem ? RowPos{true, 0, nullptr} : row_pos(L, tp, row);
+                const int sw = row & 7;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {                 // 16-byte chunk j (8 channels) of the 128-byte row
+                    const int col = ptx::frag_col(t, j), ch = n0 + col;
+                    const uint32_t off = (uint32_t)(row * 128 + ((j ^ sw) << 4) + (col & 7) * 2);
+                    const float2 s = __ldg(reinterpret_cast<const float2*>(P.shift + ch));
+                    float v0 = acc[4 * j + 2 * h] + s.x, v1 = acc[4 * j + 2 * h + 1] + s.y;
+                    if (res_smem || rp.rrow != nullptr) {
+                        const uint32_t rv = res_smem ? *reinterpret_cast<const uint32_t*>(rsm + off)
+                                                     : __ldg(reinterpret_cast<const unsigned int*>(rp.rrow + ch));
+                        const float2 f = unpack_act2(rv, P.fp16);
+                        v0 += f.x; v1 += f.y;
+                    }
+                    *reinterpret_cast<uint32_t*>(smem_out + off) = pack_act2(activate(v0, P.relu), activate(v1, P.relu), P.fp16);
                 }
             }
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&tempty_bar[acc]);
-            if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
+            ptx::fence_proxy_async();                            // generic-proxy smem writes -> visible to the TMA engine
+            ptx::named_barrier(1, kConsumerThreads);
+            if (threadIdx.x == 0) {
+                if (res_smem) ptx::mbar_arrive(&rempty_bar[rslot]);
+                ptx::tma_store_5d(&maps.y[tp.l], smem_out, n0, tp.tiz * L.bz, tp.tiy * L.by, tp.tix * L.bx, tp.nb);
+                ptx::bulk_commit();
+            }
+            if (res_smem && ++rslot == RES_SLOTS) { rslot = 0; rphase ^= 1u; }
+            continue;
+        }
+        // ---- register epilogue: each thread owns 2 channels of every 8-channel group in two rows of the tile
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const RowPos rp = row_pos(L, tp, wg * 64 + ptx::frag_row(t, h));
+            if (!rp.valid) continue;
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
+                const int ch = n0 + ptx::frag_col(t, j);
+                if (ch >= P.cout) continue;                  // Cout % 8 == 0: the pair is wholly in or out
+                const float2 s = __ldg(reinterpret_cast<const float2*>(P.shift + ch));
+                float v0 = acc[4 * j + 2 * h] + s.x, v1 = acc[4 * j + 2 * h + 1] + s.y;
+                if (rp.rrow != nullptr) {
+                    const float2 f = unpack_act2(__ldg(reinterpret_cast<const unsigned int*>(rp.rrow + ch)), P.fp16);
+                    v0 += f.x; v1 += f.y;
+                }
+                v0 = activate(v0, P.relu); v1 = activate(v1, P.relu);
+                if (P.out_fp32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(L.y) + rp.vox * L.ldy + ch) = make_float2(v0, v1);
+                else *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(L.y) + rp.vox * L.ldy + ch) = pack_act2(v0, v1, P.fp16);
+            }
         }
     }
-
-    if (TMA_EPI && threadIdx.x == 64) ptx::bulk_wait_all();          // the staging tile must outlive its last bulk store
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) { ptx::tc_fence_after(); ptx::tmem_dealloc(tmem_base, kTmemCols); }
+    if (TMA_EPI && threadIdx.x == 0) ptx::bulk_wait_all();          // the staging tile must outlive its last bulk store
 }
 
 // ------------------------------------------------------------------------------------------------ host
@@ -485,7 +367,6 @@ template <int BLOCK_N, int STAGES, int MIN_BLOCKS, bool TMA_EPI = false, bool WS
 static int launch_conv(const ConvMaps& maps, const ConvDev& P, int total_tiles, cudaStream_t st) {
     constexpr int smem = STAGES * (kABytes + BLOCK_N * kBlockK * 2 * (WS ? 2 : 1)) + (TMA_EPI ? ((WS ? 1 : 2) + 1) * kEpiTileBytes : 0) + 1024 + 256;
     static_assert((smem + 1024) * MIN_BLOCKS <= 228 * 1024, "shared memory budget");
-    static_assert(2 * BLOCK_N * MIN_BLOCKS <= 512, "TMEM budget: 512 columns per SM");
     static bool attr_set = false;
     if (!attr_set) {
         NRPN_CUDA_TRY(cudaFuncSetAttribute(conv3d_igemm_kernel<BLOCK_N, STAGES, MIN_BLOCKS, TMA_EPI, WS>,
@@ -494,7 +375,7 @@ static int launch_conv(const ConvMaps& maps, const ConvDev& P, int total_tiles, 
     }
     const int slots = num_sms() * MIN_BLOCKS;
     const int grid = total_tiles < slots ? total_tiles : slots;
-    NRPN_CUDA_TRY(launch_pdl(conv3d_igemm_kernel<BLOCK_N, STAGES, MIN_BLOCKS, TMA_EPI, WS>, dim3(grid), dim3(192), smem, st, total_tiles <= 2 * slots, maps, P));
+    NRPN_CUDA_TRY(launch_pdl(conv3d_igemm_kernel<BLOCK_N, STAGES, MIN_BLOCKS, TMA_EPI, WS>, dim3(grid), dim3(kConvThreads), smem, st, total_tiles <= 2 * slots, maps, P));
     NRPN_LAUNCH_CHECK();
     return NRPN_OK;
 }
@@ -515,9 +396,8 @@ static void choose_brick(int xo, int yo, int zo, int& bx, int& by, int& bz) {
 // Split-K: layers with far fewer output tiles than SMs and a long reduction (late ResNet stages: 5x8x8 .. 10x16x16 voxels,
 // K up to 13 824) are latency bound on streaming their weights through a handful of CTAs. The kernel can spread the
 // k-blocks of each tile over `splits` CTAs (per-split fp32 slabs, last CTA reduces in a fixed order: bit-reproducible).
-// MEASURED on B200 (profiles/r01_layers_splitk_*.txt): the single-CTA slab reduction costs more than the split saves
-// (L3.c2 512->512 3^3 at 5x8x8: 0.101 ms unsplit, 0.175 ms with 24 splits), so it is OFF unless NRPN_SPLITK=1 is set;
-// batching several scenes per launch (bench.py --scenes-per-step) is what feeds these layers instead.
+// The single-CTA slab reduction is serial, so the split is OFF unless NRPN_SPLITK=1 is set; batching several scenes per
+// launch (bench.py --scenes-per-step) is what feeds these layers instead.
 static int choose_splits(int total_tiles, int kblocks, bool short_k) {
     static const bool enabled = [] { const char* e = getenv("NRPN_SPLITK"); return e && e[0] == '1'; }();
     if (!enabled) return 1;
@@ -547,13 +427,14 @@ static int conv_geometry(const nrpn_conv_desc* d, ConvGeom& g) {
     }
     g.m_tiles = tiles;
     // Late ResNet stages (5x8x8 .. 10x16x16 voxels, K up to 13 824): a handful of 128 x 256 tiles leaves most SMs idle while each
-    // tile runs a long reduction.  When even 64-wide tiles fit in one wave, use them: 4x the CTAs, each 128 x 64 MMA lasts 48 clk
-    // instead of 128 (same reduction order per output element, bit-identical results).
-    if (!g.short_k && g.block_n > 64 && tiles * (g.cout_pad / 64) <= num_sms()) {
+    // tile runs a long reduction.  Two remedies: split-K over the full-width tiles (opt-in, NRPN_SPLITK=1, decided first so that it
+    // reaches the layers it is meant for), otherwise -- the default -- 64-wide tiles when even those fit in one wave: 4x the CTAs
+    // (same reduction order per output element, bit-identical results).
+    g.splits = d->wsplit ? 1 : choose_splits(tiles * g.n_tiles_n, g.kblocks, g.short_k);
+    if (g.splits == 1 && !g.short_k && g.block_n > 64 && tiles * (g.cout_pad / 64) <= num_sms()) {
         const char* e = getenv("NRPN_CONV_NARROW");
         if (!(e && e[0] == '0')) { g.block_n = 64; g.n_tiles_n = g.cout_pad / 64; }
     }
-    g.splits = d->wsplit ? 1 : choose_splits(tiles * g.n_tiles_n, g.kblocks, g.short_k);
     g.counter_bytes = align_up((size_t)tiles * g.n_tiles_n * 4, 256);
     g.ws_bytes = g.splits > 1 ? g.counter_bytes + (size_t)tiles * g.n_tiles_n * g.splits * kBlockM * g.block_n * 4 : 0;
     // shared-memory (TMA) epilogue: the HBM-bound short reductions with whole 64-channel bf16 output tiles
@@ -667,9 +548,6 @@ int nrpn_conv3d_fprop(const nrpn_conv_desc* d, nrpn_stream_t stream) {
                 if (rr != CUDA_SUCCESS) { g_last_cuda_error = (int)rr; return NRPN_ERR_CUDA; }
             } else maps.r[l] = maps.y[l];
         }
-        const size_t ybytes = (size_t)S.ldy * (d->out_fp32 ? 4 : 2);
-        L.wide_y = (ybytes % 32 == 0 && reinterpret_cast<uintptr_t>(S.y) % 32 == 0) ? 1 : 0;
-        L.wide_r = (S.res && ((size_t)S.ldr * 2) % 32 == 0 && reinterpret_cast<uintptr_t>(S.res) % 32 == 0) ? 1 : 0;
 
         // activation tensor map: (C, Z, Y, X, N), optionally sub-sampled by `stride` on the three spatial axes
         const cuuint64_t cin = (cuuint64_t)d->cin;

@@ -3,9 +3,9 @@
 // of ResNet layer1 (feature_extractor.py:31-68).
 //
 // Why a second kernel: with N = 64 output channels a tap-by-tap brick kernel (conv3d_igemm.cu) re-reads one 16 KB
-// activation box AND one 8 KB weight block from L2 for every (tap, 128-voxel tile): 24 KB per 0.5 MFMA, ~8 TB/s of L2
-// traffic at the measured 0.66 ms of the stem -- it is L2-bandwidth bound at a quarter of the tensor-pipe rate.
-// Here one CTA owns a tile of 4 x-planes x 16 (y) x 8 (z) = 512 output voxels, i.e. FOUR 128 x 64 accumulators in TMEM:
+// activation box AND one 8 KB weight block from L2 for every (tap, 128-voxel tile): 24 KB per 0.5 MFMA, so it is bound by
+// L2 bandwidth well below the tensor-core rate.
+// Here one CTA owns a tile of 4 x-planes x 16 (y) x 8 (z) = 512 output voxels, i.e. FOUR 128 x 64 accumulators:
 //   - z is the fastest spatial axis, so 8 z-neighbours x 64 channels form exactly one 1024-byte SWIZZLE_128B atom.  For
 //     each distinct z offset of the filter (a "phase") the halo slab {z0+dz .. +8, y0+dy_min .. y0+15+dy_max,
 //     x0+dx_min .. x0+3+dx_max} is streamed x-plane by x-plane (one TMA box {64 ch, 8 z, Ys y} per plane, out-of-range
@@ -14,13 +14,14 @@
 //     plane (dx - dx_min + a): a plain SWIZZLE_128B K-major descriptor with a different start address -- shifts along
 //     y and x are free, only shifts along z need their own copy of the slab;
 //   - every 8 KB weight block is used by 16 MMAs (4 accumulators x K 64/16) instead of 4.
-// L2 traffic per 128 output voxels drops from 768 KB to ~130 KB (stem) and the layer becomes tensor-pipe bound.
-// Roles: warp 0 = slab (A) producer, warp 1 = tcgen05.mma issuer, warp 2 = weight (B) producer, warps 3-6 = epilogue
-// (+ shift, ReLU, bf16, 128-byte row stores); accumulators double-buffered (2 x 4 x 64 = all 512 TMEM columns).
+// L2 traffic per 128 output voxels drops from 768 KB to ~130 KB (stem).
+// Roles: warps 0-7 = two consumer warpgroups (rows 0-63 / 64-127 of every accumulator: 4 x m64n64 wgmma accumulators in
+// registers, then + shift, ReLU, 16-bit stores), warp 8 = slab (A) producer, warp 9 = weight (B) producer.
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 #include "common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 #include "conv_internal.cuh"
 
 namespace nrpn {
@@ -32,7 +33,8 @@ constexpr int kSlabMaxSlots = 12;
 constexpr int kSlabBStages = 4;
 constexpr int kSlabBBytes = 64 * 64 * 2; // one tap of weights: 64 (Cout, padded) x 64 (Cin) bf16
 constexpr int kSlabMaxAxis = 8;          // at most 8 distinct offsets per axis
-constexpr int kSlabThreads = 224;
+constexpr int kSlabConsumers = 256;
+constexpr int kSlabThreads = kSlabConsumers + 64;
 constexpr int kSlabSmemLimit = 227 * 1024;
 
 struct SlabDev {
@@ -41,7 +43,7 @@ struct SlabDev {
     int n_phases, ndx, ndy;
     int dx0, dy0;
     int planes, slots, plane_bytes;
-    int cout, relu, ldy, wide_y, fp16;
+    int cout, relu, ldy, fp16;
     signed char dz[kSlabMaxAxis];
     unsigned char dyrel[kSlabMaxAxis];
     unsigned char widx[kSlabMaxAxis][kSlabMaxAxis][kSlabMaxAxis];     // [phase][dx index][dy index] -> tap index of the packed weights
@@ -51,13 +53,7 @@ struct SlabDev {
 
 struct SlabMaps { CUtensorMap x, w; };
 
-__device__ __forceinline__ uint32_t slab_pack_bf16(float a, float b) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&v);
-}
-
 __global__ void __launch_bounds__(kSlabThreads, 1) conv3d_slab_kernel(const __grid_constant__ SlabMaps maps, const SlabDev P) {
-    const uint32_t kIdesc = P.fp16 ? ptx::make_idesc_f16(128, 64) : ptx::make_idesc_bf16(128, 64);
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* smem_a = smem;
@@ -67,208 +63,154 @@ __global__ void __launch_bounds__(kSlabThreads, 1) conv3d_slab_kernel(const __gr
     uint64_t* a_empty = bars + kSlabMaxSlots;
     uint64_t* b_full = bars + 2 * kSlabMaxSlots;
     uint64_t* b_empty = b_full + kSlabBStages;
-    uint64_t* tfull = b_empty + kSlabBStages;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < P.slots; ++s) { ptx::mbar_init(&a_full[s], 1); ptx::mbar_init(&a_empty[s], 1); }
-        for (int s = 0; s < kSlabBStages; ++s) { ptx::mbar_init(&b_full[s], 1); ptx::mbar_init(&b_empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { ptx::mbar_init(&tfull[a], 1); ptx::mbar_init(&tempty[a], 128); }
+        for (int s = 0; s < P.slots; ++s) { ptx::mbar_init(&a_full[s], 1); ptx::mbar_init(&a_empty[s], 2); }      // one arrival per consumer warpgroup
+        for (int s = 0; s < kSlabBStages; ++s) { ptx::mbar_init(&b_full[s], 1); ptx::mbar_init(&b_empty[s], 2); }
         ptx::fence_barrier_init();
         ptx::prefetch_tmap(&maps.x);
         ptx::prefetch_tmap(&maps.w);
     }
-    if (warp == 1) { ptx::tmem_alloc(tmem_slot, 512); ptx::tmem_relinquish(); }
     ptx::pdl_trigger();
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     ptx::pdl_wait();                    // prologue overlapped the previous kernel's tail; its outputs are visible from here
 
-    if (warp == 0) {
+    if (warp == kSlabConsumers / 32) {
         // ---------------------------------------------------------------- slab producer: one x-plane per TMA
-        {
-            const bool leader = ptx::elect_one();
-            int slot = 0; uint32_t par = 0;
-            for (int tile = blockIdx.x; tile < P.total_tiles; tile += gridDim.x) {
-                int t = tile;
-                const int tiz = t % P.tz; t /= P.tz;
-                const int tiy = t % P.ty; t /= P.ty;
-                const int tix = t % P.tx; const int nb = t / P.tx;
-                const int x0 = tix * kSlabAcc + P.dx0, y0 = tiy * kSlabTileY + P.dy0, z0 = tiz * kSlabTileZ;
-                for (int ph = 0; ph < P.n_phases; ++ph) {
-                    const int z = z0 + P.dz[ph];
-                    for (int p = 0; p < P.planes; ++p) {
-                        ptx::mbar_wait(&a_empty[slot], par ^ 1u);
-                        if (leader) {
-                            ptx::mbar_expect_tx(&a_full[slot], (uint32_t)P.plane_bytes);
-                            ptx::tma_load_5d(smem_a + (size_t)slot * P.plane_bytes, &maps.x, &a_full[slot], 0, z, y0, x0 + p, nb);
-                        }
-                        __syncwarp();
-                        if (++slot == P.slots) { slot = 0; par ^= 1u; }
-                    }
-                }
-            }
-        }
-    } else if (warp == 2) {
-        // ---------------------------------------------------------------- weight producer: one tap (8 KB) per TMA
-        {
-            const bool leader = ptx::elect_one();
-            int stage = 0; uint32_t par = 0;
-            for (int tile = blockIdx.x; tile < P.total_tiles; tile += gridDim.x) {
-                for (int ph = 0; ph < P.n_phases; ++ph)
-                    for (int dxi = 0; dxi < P.ndx; ++dxi)
-                        for (int dyi = 0; dyi < P.ndy; ++dyi) {
-                            ptx::mbar_wait(&b_empty[stage], par ^ 1u);
-                            if (leader) {
-                                ptx::mbar_expect_tx(&b_full[stage], kSlabBBytes);
-                                ptx::tma_load_3d(smem_b + stage * kSlabBBytes, &maps.w, &b_full[stage], 0, 0, (int)P.widx[ph][dxi][dyi]);
-                            }
-                            __syncwarp();
-                            if (++stage == kSlabBStages) { stage = 0; par ^= 1u; }
-                        }
-            }
-        }
-    } else if (warp == 1) {
-        // ---------------------------------------------------------------- MMA issuer
-        // The whole warp walks the (warp-uniform) loops and waits; one elected lane issues tcgen05.mma / commit.  Keeping
-        // the control flow converged lets ptxas hold the descriptors in uniform registers: at N = 64 an MMA lasts only
-        // 48 clk, so the issue path (not the tensor pipe) is what limits this kernel if every MMA needs a waterfall loop.
         const bool leader = ptx::elect_one();
-        const uint32_t sa0 = ptx::smem_u32(smem_a), sb0 = ptx::smem_u32(smem_b);
-        int a_slot = 0; uint32_t a_par = 0;          // ring position of plane 0 of the current phase
-        int b_stage = 0; uint32_t b_par = 0;
-        int buf = 0; uint32_t buf_par = 0;
-        for (int tile = blockIdx.x; tile < P.total_tiles; tile += gridDim.x) {
-            ptx::mbar_wait(&tempty[buf], buf_par ^ 1u);
-            ptx::tc_fence_after();
-            const uint32_t d_base = tmem_base + (uint32_t)(buf * kSlabAcc * 64);
-            uint32_t accumulate = 0;
-            for (int ph = 0; ph < P.n_phases; ++ph) {
-                int waited = 0;
-                for (int dxi = 0; dxi < P.ndx; ++dxi) {
-                    while (waited <= dxi + kSlabAcc - 1) {          // planes become visible in ring order
-                        int s = a_slot + waited; uint32_t pr = a_par;
-                        if (s >= P.slots) { s -= P.slots; pr ^= 1u; }
-                        ptx::mbar_wait(&a_full[s], pr);
-                        ++waited;
-                    }
-                    ptx::tc_fence_after();
-                    uint64_t plane_desc[kSlabAcc];
-#pragma unroll
-                    for (int a = 0; a < kSlabAcc; ++a) {
-                        int s = a_slot + dxi + a;
-                        if (s >= P.slots) s -= P.slots;
-                        plane_desc[a] = ptx::make_desc_sw128(sa0 + (uint32_t)(s * P.plane_bytes));
-                    }
-                    for (int dyi = 0; dyi < P.ndy; ++dyi) {
-                        const uint64_t yoff = (uint64_t)P.dyrel[dyi] * 64u;          // dy atoms of 1024 B, in the >>4 address field
-                        ptx::mbar_wait(&b_full[b_stage], b_par);
-                        ptx::tc_fence_after();
-                        const uint64_t db = ptx::make_desc_sw128(sb0 + (uint32_t)(b_stage * kSlabBBytes));
-                        if (leader) {
-#pragma unroll
-                            for (int a = 0; a < kSlabAcc; ++a) {
-                                const uint64_t da = plane_desc[a] + yoff;
-#pragma unroll
-                                for (int k = 0; k < 4; ++k)
-                                    ptx::umma_bf16(d_base + (uint32_t)(a * 64), da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), kIdesc,
-                                                   (accumulate | (uint32_t)k) ? 1u : 0u);
-                            }
-                            ptx::umma_commit(&b_empty[b_stage]);
-                        }
-                        __syncwarp();
-                        accumulate = 1u;
-                        if (++b_stage == kSlabBStages) { b_stage = 0; b_par ^= 1u; }
-                    }
-                    // plane p is last read by (dx index min(p, ndx-1)): release what this dx index finished with
-                    const int p_lo = dxi, p_hi = (dxi == P.ndx - 1) ? P.planes - 1 : dxi;
-                    for (int p = p_lo; p <= p_hi; ++p) {
-                        int s = a_slot + p;
-                        if (s >= P.slots) s -= P.slots;
-                        if (leader) ptx::umma_commit(&a_empty[s]);
-                    }
-                    __syncwarp();
-                }
-                a_slot += P.planes;
-                if (a_slot >= P.slots) { a_slot -= P.slots; a_par ^= 1u; }
-            }
-            if (leader) ptx::umma_commit(&tfull[buf]);
-            __syncwarp();
-            if (++buf == 2) { buf = 0; buf_par ^= 1u; }
-        }
-    } else {
-        // ---------------------------------------------------------------- epilogue (warps 3..6)
-        const int q = warp & 3;                          // TMEM lane quarter this warp may access
-        const int row = q * 32 + lane;                   // accumulator row = (y, z) inside the tile, z fastest
-        const int yi = row >> 3, zi = row & 7;
-        int buf = 0; uint32_t buf_par = 0;
+        int slot = 0; uint32_t par = 0;
         for (int tile = blockIdx.x; tile < P.total_tiles; tile += gridDim.x) {
             int t = tile;
             const int tiz = t % P.tz; t /= P.tz;
             const int tiy = t % P.ty; t /= P.ty;
             const int tix = t % P.tx; const int nb = t / P.tx;
-            const int gy = tiy * kSlabTileY + yi, gz = tiz * kSlabTileZ + zi;
-            const bool valid_yz = gy < P.yo && gz < P.zo;
-            ptx::mbar_wait(&tfull[buf], buf_par);
-            ptx::tc_fence_after();
-            const uint32_t t_base = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * kSlabAcc * 64);
-#pragma unroll 1
-            for (int a = 0; a < kSlabAcc; ++a) {
-                uint32_t r0[32], r1[32];
-                ptx::tmem_ld_32x32(t_base + (uint32_t)(a * 64), r0);
-                ptx::tmem_ld_32x32(t_base + (uint32_t)(a * 64 + 32), r1);
-                ptx::tmem_ld_wait();
-                const int gx = tix * kSlabAcc + a;
-                if (valid_yz && gx < P.xo) {
-                    __nv_bfloat16* o = P.y + ((((size_t)nb * P.xo + gx) * P.yo + gy) * P.zo + gz) * P.ldy;
-#pragma unroll
-                    for (int h = 0; h < 4; ++h) {                       // 16 channels = 32 bytes per step
-                        const int chh = h * 16;
-                        if (chh >= P.cout) break;
-                        uint4 pk[2];
-#pragma unroll
-                        for (int gg = 0; gg < 2; ++gg) {
-                            const int g = h * 2 + gg, ch = g * 8;
-                            const uint32_t* r = (g < 4) ? (r0 + g * 8) : (r1 + (g - 4) * 8);
-                            float v[8];
-                            if (ch < P.cout) {
-                                const float4 s0 = __ldg(reinterpret_cast<const float4*>(P.shift + ch));
-                                const float4 s1 = __ldg(reinterpret_cast<const float4*>(P.shift + ch + 4));
-                                v[0] = __uint_as_float(r[0]) + s0.x; v[1] = __uint_as_float(r[1]) + s0.y; v[2] = __uint_as_float(r[2]) + s0.z;
-                                v[3] = __uint_as_float(r[3]) + s0.w; v[4] = __uint_as_float(r[4]) + s1.x; v[5] = __uint_as_float(r[5]) + s1.y;
-                                v[6] = __uint_as_float(r[6]) + s1.z; v[7] = __uint_as_float(r[7]) + s1.w;
-                            } else {
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) v[i] = 0.0f;
-                            }
-                            if (P.relu == 1) {
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) v[i] = fmaxf(v[i], 0.0f);
-                            } else if (P.relu == 2) {
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) v[i] = 0.5f * v[i] * (1.0f + erff(v[i] * 0.70710678118654752f));
-                            }
-                            pk[gg] = make_uint4(pack_act2(v[0], v[1], P.fp16), pack_act2(v[2], v[3], P.fp16), pack_act2(v[4], v[5], P.fp16), pack_act2(v[6], v[7], P.fp16));
-                        }
-                        const bool both = chh + 16 <= P.cout;
-                        if (both && P.wide_y) ptx::st_global_v8(o + chh, pk[0], pk[1]);
-                        else { *reinterpret_cast<uint4*>(o + chh) = pk[0]; if (both) *reinterpret_cast<uint4*>(o + chh + 8) = pk[1]; }
+            const int x0 = tix * kSlabAcc + P.dx0, y0 = tiy * kSlabTileY + P.dy0, z0 = tiz * kSlabTileZ;
+            for (int ph = 0; ph < P.n_phases; ++ph) {
+                const int z = z0 + P.dz[ph];
+                for (int p = 0; p < P.planes; ++p) {
+                    ptx::mbar_wait(&a_empty[slot], par ^ 1u);
+                    if (leader) {
+                        ptx::mbar_expect_tx(&a_full[slot], (uint32_t)P.plane_bytes);
+                        ptx::tma_load_5d(smem_a + (size_t)slot * P.plane_bytes, &maps.x, &a_full[slot], 0, z, y0, x0 + p, nb);
                     }
+                    __syncwarp();
+                    if (++slot == P.slots) { slot = 0; par ^= 1u; }
                 }
             }
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&tempty[buf]);
-            if (++buf == 2) { buf = 0; buf_par ^= 1u; }
         }
+        return;
+    }
+    if (warp == kSlabConsumers / 32 + 1) {
+        // ---------------------------------------------------------------- weight producer: one tap (8 KB) per TMA
+        const bool leader = ptx::elect_one();
+        int stage = 0; uint32_t par = 0;
+        for (int tile = blockIdx.x; tile < P.total_tiles; tile += gridDim.x) {
+            for (int ph = 0; ph < P.n_phases; ++ph)
+                for (int dxi = 0; dxi < P.ndx; ++dxi)
+                    for (int dyi = 0; dyi < P.ndy; ++dyi) {
+                        ptx::mbar_wait(&b_empty[stage], par ^ 1u);
+                        if (leader) {
+                            ptx::mbar_expect_tx(&b_full[stage], kSlabBBytes);
+                            ptx::tma_load_3d(smem_b + stage * kSlabBBytes, &maps.w, &b_full[stage], 0, 0, (int)P.widx[ph][dxi][dyi]);
+                        }
+                        __syncwarp();
+                        if (++stage == kSlabBStages) { stage = 0; par ^= 1u; }
+                    }
+        }
+        return;
     }
 
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) { ptx::tc_fence_after(); ptx::tmem_dealloc(tmem_base, 512); }
+    // -------------------------------------------------------------------- consumers: MMA + epilogue
+    const int t = threadIdx.x & 127, wg = threadIdx.x >> 7;
+    const uint32_t sa0 = ptx::smem_u32(smem_a) + (uint32_t)(wg * 8192), sb0 = ptx::smem_u32(smem_b);     // rows 64 wg .. 64 wg + 63
+    int a_slot = 0; uint32_t a_par = 0;          // ring position of plane 0 of the current phase
+    int b_stage = 0; uint32_t b_par = 0;
+    float acc[kSlabAcc][32];
+    for (int tile = blockIdx.x; tile < P.total_tiles; tile += gridDim.x) {
+        uint32_t accumulate = 0;
+#pragma unroll
+        for (int a = 0; a < kSlabAcc; ++a) ptx::reg_fence(acc[a]);
+        for (int ph = 0; ph < P.n_phases; ++ph) {
+            int waited = 0;
+            for (int dxi = 0; dxi < P.ndx; ++dxi) {
+                while (waited <= dxi + kSlabAcc - 1) {          // planes become visible in ring order
+                    int s = a_slot + waited; uint32_t pr = a_par;
+                    if (s >= P.slots) { s -= P.slots; pr ^= 1u; }
+                    ptx::mbar_wait(&a_full[s], pr);
+                    ++waited;
+                }
+                uint64_t plane_desc[kSlabAcc];
+#pragma unroll
+                for (int a = 0; a < kSlabAcc; ++a) {
+                    int s = a_slot + dxi + a;
+                    if (s >= P.slots) s -= P.slots;
+                    plane_desc[a] = ptx::make_desc_sw128(sa0 + (uint32_t)(s * P.plane_bytes));
+                }
+                for (int dyi = 0; dyi < P.ndy; ++dyi) {
+                    const uint64_t yoff = (uint64_t)P.dyrel[dyi] * 64u;          // dy atoms of 1024 B, in the >>4 address field
+                    ptx::mbar_wait(&b_full[b_stage], b_par);
+                    const uint64_t db = ptx::make_desc_sw128(sb0 + (uint32_t)(b_stage * kSlabBBytes));
+                    auto issue = [&](auto f16) {
+                        ptx::wgmma_fence();
+#pragma unroll
+                        for (int a = 0; a < kSlabAcc; ++a) {
+                            const uint64_t da = plane_desc[a] + yoff;
+#pragma unroll
+                            for (int k = 0; k < 4; ++k)
+                                ptx::Wgmma<64, decltype(f16)::value>::template ss<0, 0>(acc[a], da + (uint64_t)(2 * k), db + (uint64_t)(2 * k),
+                                                                                         (accumulate | (uint32_t)k) ? 1u : 0u);
+                        }
+                        ptx::wgmma_commit();
+                    };
+                    if (P.fp16) issue(std::true_type{}); else issue(std::false_type{});
+                    ptx::wgmma_wait<0>();
+                    if (t == 0) ptx::mbar_arrive(&b_empty[b_stage]);
+                    accumulate = 1u;
+                    if (++b_stage == kSlabBStages) { b_stage = 0; b_par ^= 1u; }
+                }
+                // plane p is last read by (dx index min(p, ndx-1)): release what this dx index finished with
+                const int p_lo = dxi, p_hi = (dxi == P.ndx - 1) ? P.planes - 1 : dxi;
+                for (int p = p_lo; p <= p_hi; ++p) {
+                    int s = a_slot + p;
+                    if (s >= P.slots) s -= P.slots;
+                    if (t == 0) ptx::mbar_arrive(&a_empty[s]);
+                }
+            }
+            a_slot += P.planes;
+            if (a_slot >= P.slots) { a_slot -= P.slots; a_par ^= 1u; }
+        }
+#pragma unroll
+        for (int a = 0; a < kSlabAcc; ++a) ptx::reg_fence(acc[a]);
+
+        // ---- epilogue: accumulator row = (y, z) inside the tile, z fastest
+        int tt = tile;
+        const int tiz = tt % P.tz; tt /= P.tz;
+        const int tiy = tt % P.ty; tt /= P.ty;
+        const int tix = tt % P.tx; const int nb = tt / P.tx;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = wg * 64 + ptx::frag_row(t, h);
+            const int gy = tiy * kSlabTileY + (row >> 3), gz = tiz * kSlabTileZ + (row & 7);
+            if (gy >= P.yo || gz >= P.zo) continue;
+#pragma unroll
+            for (int a = 0; a < kSlabAcc; ++a) {
+                const int gx = tix * kSlabAcc + a;
+                if (gx >= P.xo) continue;
+                __nv_bfloat16* o = P.y + ((((size_t)nb * P.xo + gx) * P.yo + gy) * P.zo + gz) * P.ldy;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const int ch = ptx::frag_col(t, j);
+                    if (ch >= P.cout) continue;
+                    const float2 s = __ldg(reinterpret_cast<const float2*>(P.shift + ch));
+                    float v0 = acc[a][4 * j + 2 * h] + s.x, v1 = acc[a][4 * j + 2 * h + 1] + s.y;
+                    if (P.relu == 1) { v0 = fmaxf(v0, 0.0f); v1 = fmaxf(v1, 0.0f); }
+                    else if (P.relu == 2) { v0 = 0.5f * v0 * (1.0f + erff(v0 * 0.70710678118654752f)); v1 = 0.5f * v1 * (1.0f + erff(v1 * 0.70710678118654752f)); }
+                    *reinterpret_cast<uint32_t*>(o + ch) = pack_act2(v0, v1, P.fp16);
+                }
+            }
+        }
+    }
 }
 
 // ------------------------------------------------------------------------------------------------ host
@@ -337,7 +279,6 @@ int conv3d_slab_launch(const nrpn_conv_desc* d, cudaStream_t st) {
     P.total_tiles = S.n * P.tx * P.ty * P.tz;
     P.fp16 = d->act_fp16 ? 1 : 0;
     P.cout = d->cout; P.relu = d->relu; P.ldy = S.ldy; P.shift = d->shift; P.y = reinterpret_cast<__nv_bfloat16*>(S.y);
-    P.wide_y = (((size_t)S.ldy * 2) % 32 == 0 && reinterpret_cast<uintptr_t>(S.y) % 32 == 0) ? 1 : 0;
 
     SlabMaps maps;
     {   // activations (C, Z, Y, X, N): one box = one x-plane of the slab, {64 ch, 8 z, Ys y}

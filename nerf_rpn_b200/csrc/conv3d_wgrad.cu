@@ -1,4 +1,4 @@
-// Weight gradient of a stride-1 'same' 3-D convolution on tcgen05 (training, SURVEY.md 8(a) a18):
+// Weight gradient of a stride-1 'same' 3-D convolution on wgmma (training, SURVEY.md 8(a) a18):
 //     dW[tap][co][ci] = sum over voxels v   dY[v][co] * X[v + tap_offset][ci]
 // The contraction runs over VOXELS, for which channels-last activations (a voxel's channels are contiguous) are MN-major operands.
 // Two operand paths, selected by nrpn_wgrad_desc.operand_layout:
@@ -8,21 +8,23 @@
 //     kernel so that K-major descriptors can be used: the (y, z) plane is addressed as ONE flattened axis of Y * z_pitch elements, a TMA box
 //     {64 flattened voxels, 1 x, channels, 1} lands as `channels` rows of exactly 128 bytes; TMA needs 16-byte aligned inner coordinates, so a y shift
 //     is the flattened offset dy * z_pitch (z_pitch % 8 == 0) and a z shift of -1 / +1 reads a z-SHIFTED COPY of X^T written by the transpose kernel.
-// In both: D (128 x N_T, fp32 in TMEM) += A * B^T with A = dY brick (128 output channels x 64 voxels), B = X brick shifted by the tap (N_T input
+// In both: D (128 x N_T, fp32 in registers of two warpgroups) += A * B^T with A = dY brick (128 output channels x 64 voxels), B = X brick shifted by the tap (N_T input
 // channels x 64 voxels).  Work item = (tap or tap group, Cout slice(s), Cin slice, K-split); every item streams its share of the voxel bricks of all
 // pyramid levels that share the weights (the RPN head on P2..P5) and writes fp32 partial tiles; a second kernel sums them in a fixed order
 // (bit-reproducible) into dW (taps, Cout, Cin) or nn.Conv3d.weight's own (Cout, Cin, taps) order.
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 #include "common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 #include "conv_internal.cuh"
 
 namespace nrpn {
 
 constexpr int kWgStages = 4;
 constexpr int kWgABytes = 128 * 128;            // 128 output channels x 64 voxels x 2 B
-constexpr int kWgThreads = 192;
+constexpr int kWgConsumers = 256;               // two warpgroups: output channels 0-63 / 64-127 of the slice
+constexpr int kWgThreads = kWgConsumers + 32;   // + the TMA producer warp
 
 struct WgLevelDev { int n, X, chunks, zp, brick_begin; };      // chunks = ceil(Y * zp / 64) K-blocks per x-plane
 
@@ -35,41 +37,48 @@ struct WgDev {
 
 struct WgMaps { CUtensorMap dy[NRPN_CONV_MAX_LEVELS]; CUtensorMap x[NRPN_CONV_MAX_LEVELS][3]; };      // x[level][dz + 1]: z-shifted copies
 
+// Stores the consumer warpgroup's rows of an accumulator (128 x NT, columns >= n_t are padding) as one fp32 partial tile.
+template <int NT>
+__device__ __forceinline__ void store_partial(float* tile, int n_t, int wg, int t, const float (&acc)[NT / 2], bool empty) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float* out = tile + (size_t)(wg * 64 + ptx::frag_row(t, h)) * n_t;
+#pragma unroll
+        for (int j = 0; j < NT / 8; ++j) {
+            const int col = ptx::frag_col(t, j);
+            if (col < n_t)
+                *reinterpret_cast<float2*>(out + col) = empty ? make_float2(0.f, 0.f) : make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
+    }
+}
+
+template <int NT>
 __global__ void __launch_bounds__(kWgThreads, 1) conv3d_wgrad_kernel(const __grid_constant__ WgMaps maps, const WgDev P) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int b_bytes = P.n_t * 128;
-    const int stage_bytes = kWgABytes + b_bytes;
+    constexpr int stage_bytes = kWgABytes + NT * 128;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWgStages * stage_bytes);
     uint64_t* full_bar = bars;
     uint64_t* empty_bar = bars + kWgStages;
-    uint64_t* tfull_bar = bars + 2 * kWgStages;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kWgStages + 1);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kWgStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-        ptx::mbar_init(tfull_bar, 1);
+        for (int s = 0; s < kWgStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 2); }
         ptx::fence_barrier_init();
         for (int l = 0; l < P.n_levels; ++l) { ptx::prefetch_tmap(&maps.dy[l]); for (int k = 0; k < 3; ++k) ptx::prefetch_tmap(&maps.x[l][k]); }
     }
-    if (warp == 1) { ptx::tmem_alloc(tmem_slot, 256); ptx::tmem_relinquish(); }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t idesc = P.fp16 ? ptx::make_idesc_f16(128, P.n_t) : ptx::make_idesc_bf16(128, P.n_t);
     const int items = P.n_taps * P.m_tiles * P.n_tiles * P.splits;
-    uint32_t tphase = 0;
-    int stage_p = 0, stage_c = 0; uint32_t phase_p = 0, phase_c = 0;          // producer / consumer ring positions (persist over items)
+    const uint32_t load_bytes = (uint32_t)(kWgABytes + P.n_t * 128);
 
-    for (int item = blockIdx.x; item < items; item += gridDim.x) {
-        const int split = item % P.splits;
-        const int nt = (item / P.splits) % P.n_tiles;
-        const int mt = (item / (P.splits * P.n_tiles)) % P.m_tiles;
-        const int tap = item / (P.splits * P.n_tiles * P.m_tiles);
-        const int b0 = (int)(((long)P.total_bricks * split) / P.splits), b1 = (int)(((long)P.total_bricks * (split + 1)) / P.splits);
-        if (warp == 0) {
-            const bool leader = ptx::elect_one();
+    if (warp == kWgConsumers / 32) {
+        const bool leader = ptx::elect_one();
+        int stage = 0; uint32_t phase = 0;
+        for (int item = blockIdx.x; item < items; item += gridDim.x) {
+            const int split = item % P.splits;
+            const int nt = (item / P.splits) % P.n_tiles;
+            const int mt = (item / (P.splits * P.n_tiles)) % P.m_tiles;
+            const int tap = item / (P.splits * P.n_tiles * P.m_tiles);
+            const int b0 = (int)(((long)P.total_bricks * split) / P.splits), b1 = (int)(((long)P.total_bricks * (split + 1)) / P.splits);
             const int dx = P.tap[tap][0], dy = P.tap[tap][1], dz = P.tap[tap][2];
             for (int b = b0; b < b1; ++b) {
                 int l = 0;
@@ -80,59 +89,51 @@ __global__ void __launch_bounds__(kWgThreads, 1) conv3d_wgrad_kernel(const __gri
                 const int ck = t % L.chunks; t /= L.chunks;
                 const int x0 = t % L.X; const int nb = t / L.X;
                 const int f0 = ck * 64;                                      // position on the flattened (y, z-with-pad) axis
-                ptx::mbar_wait(&empty_bar[stage_p], phase_p ^ 1u);
+                ptx::mbar_wait(&empty_bar[stage], phase ^ 1u);
                 if (leader) {
-                    uint8_t* sa = smem + stage_p * stage_bytes;
-                    ptx::mbar_expect_tx(&full_bar[stage_p], (uint32_t)stage_bytes);
-                    ptx::tma_load_4d(sa, &maps.dy[l], &full_bar[stage_p], f0, x0, mt * 128, nb);
-                    ptx::tma_load_4d(sa + kWgABytes, &maps.x[l][dz + 1], &full_bar[stage_p], f0 + dy * L.zp, x0 + dx, nt * P.n_t, nb);   // z shift lives in the copy
+                    uint8_t* sa = smem + stage * stage_bytes;
+                    ptx::mbar_expect_tx(&full_bar[stage], load_bytes);
+                    ptx::tma_load_4d(sa, &maps.dy[l], &full_bar[stage], f0, x0, mt * 128, nb);
+                    ptx::tma_load_4d(sa + kWgABytes, &maps.x[l][dz + 1], &full_bar[stage], f0 + dy * L.zp, x0 + dx, nt * P.n_t, nb);   // z shift lives in the copy
                 }
                 __syncwarp();
-                if (++stage_p == kWgStages) { stage_p = 0; phase_p ^= 1u; }
+                if (++stage == kWgStages) { stage = 0; phase ^= 1u; }
             }
-        } else if (warp == 1) {
-            const bool leader = ptx::elect_one();
-            for (int b = b0; b < b1; ++b) {
-                ptx::mbar_wait(&full_bar[stage_c], phase_c);
-                ptx::tc_fence_after();
-                const uint32_t sa = ptx::smem_u32(smem + stage_c * stage_bytes);
-                const uint64_t da = ptx::make_desc_sw128(sa), db = ptx::make_desc_sw128(sa + kWgABytes);
-                if (leader) {
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        ptx::umma_bf16(tmem, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, ((b - b0) | k) ? 1u : 0u);
-                    ptx::umma_commit(&empty_bar[stage_c]);
-                }
-                __syncwarp();
-                if (++stage_c == kWgStages) { stage_c = 0; phase_c ^= 1u; }
-            }
-            if (leader) ptx::umma_commit(tfull_bar);
-            __syncwarp();
-        } else {
-            // epilogue warps 2..5: row = output channel of the slice, columns = input channels
-            const int q = warp & 3, row = q * 32 + lane;
-            float* out = P.partial + (((((size_t)tap * P.m_tiles + mt) * P.n_tiles + nt) * P.splits + split) * 128 + row) * P.n_t;
-            ptx::mbar_wait(tfull_bar, tphase);
-            ptx::tc_fence_after();
-            const bool empty = (b1 <= b0);                               // nothing accumulated: the TMEM contents are stale
-            for (int c = 0; c < P.n_t; c += 32) {
-                uint32_t r[32];
-                ptx::tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)c, r);
-                ptx::tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    *reinterpret_cast<float4*>(out + c + j) = empty ? make_float4(0.f, 0.f, 0.f, 0.f)
-                        : make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-            }
-            ptx::tc_fence_before();
         }
-        tphase ^= 1u;
-        __syncthreads();            // the accumulator is drained before the next item's first MMA overwrites it
-        ptx::tc_fence_after();
+        return;
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) { ptx::tc_fence_after(); ptx::tmem_dealloc(tmem, 256); }
+
+    // consumers: rows = output channels of the slice, columns = input channels
+    const int t = threadIdx.x & 127, wg = threadIdx.x >> 7;
+    int stage = 0; uint32_t phase = 0;
+    float acc[NT / 2];
+    for (int item = blockIdx.x; item < items; item += gridDim.x) {
+        const int split = item % P.splits;
+        const int nt = (item / P.splits) % P.n_tiles;
+        const int mt = (item / (P.splits * P.n_tiles)) % P.m_tiles;
+        const int tap = item / (P.splits * P.n_tiles * P.m_tiles);
+        const int b0 = (int)(((long)P.total_bricks * split) / P.splits), b1 = (int)(((long)P.total_bricks * (split + 1)) / P.splits);
+        ptx::reg_fence(acc);
+        for (int b = b0; b < b1; ++b) {
+            ptx::mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa = ptx::smem_u32(smem + stage * stage_bytes);
+            const uint64_t da = ptx::make_desc_sw128(sa + (uint32_t)(wg * (kWgABytes / 2))), db = ptx::make_desc_sw128(sa + kWgABytes);
+            auto issue = [&](auto f16) {
+                ptx::wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+                    ptx::Wgmma<NT, decltype(f16)::value>::template ss<0, 0>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), ((b - b0) | k) ? 1u : 0u);
+                ptx::wgmma_commit();
+            };
+            if (P.fp16) issue(std::true_type{}); else issue(std::false_type{});
+            ptx::wgmma_wait<0>();
+            if (t == 0) ptx::mbar_arrive(&empty_bar[stage]);
+            if (++stage == kWgStages) { stage = 0; phase ^= 1u; }
+        }
+        ptx::reg_fence(acc);
+        float* tile = P.partial + ((((size_t)tap * P.m_tiles + mt) * P.n_tiles + nt) * P.splits + split) * 128 * P.n_t;
+        store_partial<NT>(tile, P.n_t, wg, t, acc, b1 <= b0);         // nothing accumulated: zeros
+    }
 }
 
 // dW[tap][co][ci] = sum over splits (fixed order) of the partial tiles
@@ -153,19 +154,18 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ partial, int n_tap
     }
 }
 
-// ------------------------------------------------------------------------------------------------ channels-last operands (MN-major UMMA)
+// ------------------------------------------------------------------------------------------------ channels-last operands (MN-major wgmma)
 // The same contraction with BOTH operands read where they live: channels-last (N, X, Y, Z, ld) tensors.  A TMA box {64 channels, bz, by, bx} of
-// 64 voxels lands in shared memory as 64 rows of 128 bytes (128B swizzle) -- which IS the canonical MN-major operand layout of tcgen05.mma
-// (cute::UMMA make_umma_desc<Major::MN>, SWIZZLE_128B: ((8,n),(8,k)) x 16 bytes : ((1,LBO),(8,SBO)) -- 64 channels contiguous per voxel row, 8 rows
-// per 1024-byte swizzle atom, SBO = 1024 bytes between groups of 8 voxels, LBO = the distance between two 64-channel boxes).  The instruction
-// descriptor's a_major / b_major bits (15, 16) select it.  No transposed copies, no zero-filled staging buffers: the tap offset is a plain
-// coordinate shift of the X box and TMA's out-of-bounds zero fill is the convolution padding.
+// 64 voxels lands in shared memory as 64 rows of 128 bytes (128B swizzle) -- which IS the canonical MN-major operand layout of wgmma
+// (SWIZZLE_128B: 64 channels contiguous per voxel row, 8 rows per 1024-byte swizzle atom, SBO = 1024 bytes between groups of 8 voxels,
+// LBO = the distance between two 64-channel boxes), selected by the instruction's transpose flags.  No transposed copies, no zero-filled
+// staging buffers: the tap offset is a plain coordinate shift of the X box and TMA's out-of-bounds zero fill is the convolution padding.
 //   A = dY box pair  (128 output channels  x 64 voxels),  B = X boxes (n_t input channels x 64 voxels, shifted by the tap)
 struct WgLevelCl { int n, nxb, nyb, nzb, bx, by, bz, brick_begin; };
 struct WgDevCl {
     int n_levels, n_taps, cin, cout, n_t, m_tiles, n_tiles, splits, total_bricks, fp16, b_boxes;
-    int m_pair, m_items, stages;           // Cout slices per work item (1 or 2: two TMEM accumulators share one X tile), items along Cout, ring depth
-    int t_group, n_groups, acc_stride;     // taps per work item (their accumulators share one dY tile), tap groups, TMEM columns between accumulators
+    int m_pair, m_items, stages;           // Cout slices per work item (1 or 2: two accumulators share one X tile), items along Cout, ring depth
+    int t_group, n_groups;                 // taps per work item (their accumulators share one dY tile), tap groups
     signed char tap[NRPN_CONV_MAX_TAPS][4];
     WgLevelCl lv[NRPN_CONV_MAX_LEVELS];
     float* partial;
@@ -173,15 +173,14 @@ struct WgDevCl {
 struct WgMapsCl { CUtensorMap dy[NRPN_CONV_MAX_LEVELS]; CUtensorMap x[NRPN_CONV_MAX_LEVELS]; };
 constexpr int kWgBox = 64 * 128;               // one {64 channels x 64 voxels} box, 16-bit
 constexpr int kWgMaxStages = 4;
+constexpr int kWgAccRegs = 128;                // accumulator registers per consumer thread: m_pair * t_group * NT / 2 <= this
 
-__device__ __forceinline__ uint64_t make_desc_mn_sw128(uint32_t smem_addr) {   // LBO = 8192 B (next 64-channel box), SBO = 1024 B (next 8 voxels)
-    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)(kWgBox >> 4) << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-
-// With Cout >= 256 one work item computes TWO 128-channel slices of Cout against the same X tile (accumulators in TMEM columns [0, n_t) and
-// [256, 256 + n_t)): the kernel is bound by the shared-memory fill rate out of L2 (48 KB per four MMAs at N = 256: 11.7 TB/s in the head layer),
-// and sharing X cuts that to 32 KB.
+// NT = 64 * b_boxes input channels per accumulator (columns >= n_t are TMA zero fill), NACC >= m_pair * t_group accumulators per work item
+// (accumulator m * t_group + i = Cout slice m of the pair x tap i of the group).  With Cout >= 256 two 128-channel slices of Cout share the
+// same X tile and a tap group shares one dY tile: the kernel is bound by the shared-memory fill rate out of L2, and sharing cuts it.
+template <int NT, int NACC>
 __global__ void __launch_bounds__(kWgThreads, 1) conv3d_wgrad_cl_kernel(const __grid_constant__ WgMapsCl maps, const WgDevCl P) {
+    static_assert(NT * NACC / 2 <= kWgAccRegs, "accumulator registers");
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int a_boxes = 2 * P.m_pair;
@@ -190,36 +189,25 @@ __global__ void __launch_bounds__(kWgThreads, 1) conv3d_wgrad_cl_kernel(const __
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + stages * stage_bytes);
     uint64_t* full_bar = bars;
     uint64_t* empty_bar = bars + kWgMaxStages;
-    uint64_t* tfull_bar = bars + 2 * kWgMaxStages;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kWgMaxStages + 1);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint32_t tmem_cols = 32;
-    while ((int)tmem_cols < P.m_pair * P.t_group * P.acc_stride) tmem_cols <<= 1;
+    const int warp = threadIdx.x >> 5;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < stages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-        ptx::mbar_init(tfull_bar, 1);
+        for (int s = 0; s < stages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 2); }
         ptx::fence_barrier_init();
         for (int l = 0; l < P.n_levels; ++l) { ptx::prefetch_tmap(&maps.dy[l]); ptx::prefetch_tmap(&maps.x[l]); }
     }
-    if (warp == 1) { ptx::tmem_alloc(tmem_slot, tmem_cols); ptx::tmem_relinquish(); }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t idesc = (P.fp16 ? ptx::make_idesc_f16(128, P.n_t) : ptx::make_idesc_bf16(128, P.n_t)) | (1u << 15) | (1u << 16);   // MN-major A and B
     const int items = P.n_groups * P.m_items * P.n_tiles * P.splits;
-    uint32_t tphase = 0;
-    int stage_p = 0, stage_c = 0; uint32_t phase_p = 0, phase_c = 0;
 
-    for (int item = blockIdx.x; item < items; item += gridDim.x) {
-        const int split = item % P.splits;
-        const int nt = (item / P.splits) % P.n_tiles;
-        const int mi = (item / (P.splits * P.n_tiles)) % P.m_items;
-        const int tap0 = (item / (P.splits * P.n_tiles * P.m_items)) * P.t_group;
-        const int ntap = P.n_taps - tap0 < P.t_group ? P.n_taps - tap0 : P.t_group;        // taps of this item: tap0 .. tap0 + ntap - 1
-        const int b0 = (int)(((long)P.total_bricks * split) / P.splits), b1 = (int)(((long)P.total_bricks * (split + 1)) / P.splits);
-        if (warp == 0) {
-            const bool leader = ptx::elect_one();
+    if (warp == kWgConsumers / 32) {
+        const bool leader = ptx::elect_one();
+        int stage = 0; uint32_t phase = 0;
+        for (int item = blockIdx.x; item < items; item += gridDim.x) {
+            const int split = item % P.splits;
+            const int nt = (item / P.splits) % P.n_tiles;
+            const int mi = (item / (P.splits * P.n_tiles)) % P.m_items;
+            const int tap0 = (item / (P.splits * P.n_tiles * P.m_items)) * P.t_group;
+            const int ntap = P.n_taps - tap0 < P.t_group ? P.n_taps - tap0 : P.t_group;        // taps of this item: tap0 .. tap0 + ntap - 1
+            const int b0 = (int)(((long)P.total_bricks * split) / P.splits), b1 = (int)(((long)P.total_bricks * (split + 1)) / P.splits);
             for (int b = b0; b < b1; ++b) {
                 int l = 0;
 #pragma unroll
@@ -230,75 +218,73 @@ __global__ void __launch_bounds__(kWgThreads, 1) conv3d_wgrad_cl_kernel(const __
                 const int yb = t % L.nyb; t /= L.nyb;
                 const int xb = t % L.nxb; const int nb = t / L.nxb;
                 const int z0 = zb * L.bz, y0 = yb * L.by, x0 = xb * L.bx;
-                ptx::mbar_wait(&empty_bar[stage_p], phase_p ^ 1u);
+                ptx::mbar_wait(&empty_bar[stage], phase ^ 1u);
                 if (leader) {
-                    uint8_t* sa = smem + stage_p * stage_bytes;
-                    ptx::mbar_expect_tx(&full_bar[stage_p], (uint32_t)((a_boxes + ntap * P.b_boxes) * kWgBox));
+                    uint8_t* sa = smem + stage * stage_bytes;
+                    ptx::mbar_expect_tx(&full_bar[stage], (uint32_t)((a_boxes + ntap * P.b_boxes) * kWgBox));
                     for (int j = 0; j < a_boxes; ++j)          // Cout slice (mi * m_pair + j / 2), 64-channel half j % 2 (beyond Cout: zero-filled)
-                        ptx::tma_load_5d(sa + j * kWgBox, &maps.dy[l], &full_bar[stage_p], (mi * P.m_pair) * 128 + 64 * j, z0, y0, x0, nb);
+                        ptx::tma_load_5d(sa + j * kWgBox, &maps.dy[l], &full_bar[stage], (mi * P.m_pair) * 128 + 64 * j, z0, y0, x0, nb);
                     for (int ti = 0; ti < ntap; ++ti) {        // one X tile per tap of the group: the tap is a coordinate shift
                         const int dx = P.tap[tap0 + ti][0], dy = P.tap[tap0 + ti][1], dz = P.tap[tap0 + ti][2];
                         for (int j = 0; j < P.b_boxes; ++j)
-                            ptx::tma_load_5d(sa + (a_boxes + ti * P.b_boxes + j) * kWgBox, &maps.x[l], &full_bar[stage_p], nt * P.n_t + 64 * j, z0 + dz, y0 + dy,
+                            ptx::tma_load_5d(sa + (a_boxes + ti * P.b_boxes + j) * kWgBox, &maps.x[l], &full_bar[stage], nt * P.n_t + 64 * j, z0 + dz, y0 + dy,
                                              x0 + dx, nb);
                     }
                 }
                 __syncwarp();
-                if (++stage_p == stages) { stage_p = 0; phase_p ^= 1u; }
+                if (++stage == stages) { stage = 0; phase ^= 1u; }
             }
-        } else if (warp == 1) {
-            const bool leader = ptx::elect_one();
-            for (int b = b0; b < b1; ++b) {
-                ptx::mbar_wait(&full_bar[stage_c], phase_c);
-                ptx::tc_fence_after();
-                const uint32_t sa = ptx::smem_u32(smem + stage_c * stage_bytes);
-                if (leader) {
-                    for (int ti = 0; ti < ntap; ++ti) {
-                        const uint64_t db = make_desc_mn_sw128(sa + (a_boxes + ti * P.b_boxes) * kWgBox);
-                        for (int mp = 0; mp < P.m_pair; ++mp) {
-                            const uint64_t da = make_desc_mn_sw128(sa + mp * 2 * kWgBox);
-                            const uint32_t acc = tmem + (uint32_t)((mp * P.t_group + ti) * P.acc_stride);
-#pragma unroll
-                            for (int k = 0; k < 4; ++k)      // 16 voxels per MMA = two 1024-byte atoms further along K
-                                ptx::umma_bf16(acc, da + (uint64_t)(128 * k), db + (uint64_t)(128 * k), idesc, ((b - b0) | k) ? 1u : 0u);
-                        }
-                    }
-                    ptx::umma_commit(&empty_bar[stage_c]);
-                }
-                __syncwarp();
-                if (++stage_c == stages) { stage_c = 0; phase_c ^= 1u; }
-            }
-            if (leader) ptx::umma_commit(tfull_bar);
-            __syncwarp();
-        } else {
-            const int q = warp & 3, row = q * 32 + lane;
-            ptx::mbar_wait(tfull_bar, tphase);
-            ptx::tc_fence_after();
-            const bool empty = (b1 <= b0);
-            for (int am = 0; am < P.m_pair * ntap; ++am) {
-                const int mp = am / ntap, ti = am - mp * ntap;
-                const int mt = mi * P.m_pair + mp, tap = tap0 + ti;
-                if (mt >= P.m_tiles) break;
-                float* out = P.partial + (((((size_t)tap * P.m_tiles + mt) * P.n_tiles + nt) * P.splits + split) * 128 + row) * P.n_t;
-                for (int c = 0; c < P.n_t; c += 32) {
-                    uint32_t r[32];
-                    ptx::tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)((mp * P.t_group + ti) * P.acc_stride + c), r);
-                    ptx::tmem_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4)
-                        *reinterpret_cast<float4*>(out + c + j) = empty ? make_float4(0.f, 0.f, 0.f, 0.f)
-                            : make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-                }
-            }
-            ptx::tc_fence_before();
         }
-        tphase ^= 1u;
-        __syncthreads();
-        ptx::tc_fence_after();
+        return;
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) { ptx::tc_fence_after(); ptx::tmem_dealloc(tmem, tmem_cols); }
+
+    const int t = threadIdx.x & 127, wg = threadIdx.x >> 7;       // warpgroup wg: output channels 64 wg .. 64 wg + 63 of each slice
+    int stage = 0; uint32_t phase = 0;
+    float acc[NACC][NT / 2];
+    for (int item = blockIdx.x; item < items; item += gridDim.x) {
+        const int split = item % P.splits;
+        const int nt = (item / P.splits) % P.n_tiles;
+        const int mi = (item / (P.splits * P.n_tiles)) % P.m_items;
+        const int tap0 = (item / (P.splits * P.n_tiles * P.m_items)) * P.t_group;
+        const int ntap = P.n_taps - tap0 < P.t_group ? P.n_taps - tap0 : P.t_group;
+        const int b0 = (int)(((long)P.total_bricks * split) / P.splits), b1 = (int)(((long)P.total_bricks * (split + 1)) / P.splits);
+#pragma unroll
+        for (int am = 0; am < NACC; ++am) ptx::reg_fence(acc[am]);
+        for (int b = b0; b < b1; ++b) {
+            ptx::mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa = ptx::smem_u32(smem + stage * stage_bytes);
+            auto issue = [&](auto f16) {
+                ptx::wgmma_fence();
+#pragma unroll
+                for (int am = 0; am < NACC; ++am) {
+                    // NACC == m_pair * t_group, so mp < m_pair always.  In a last tap group with ntap < t_group the surplus accumulators
+                    // repeat tap ntap - 1 and are never stored: every MMA is issued, no branch around them (a divergent-looking path
+                    // around wgmma makes ptxas serialise the whole chain)
+                    const int mp = am / P.t_group, ti = min(am - mp * P.t_group, ntap - 1);
+                    const uint64_t da = ptx::make_desc_mn_sw128(sa + (uint32_t)((2 * mp + wg) * kWgBox), kWgBox);
+                    const uint64_t db = ptx::make_desc_mn_sw128(sa + (uint32_t)((a_boxes + ti * P.b_boxes) * kWgBox), kWgBox);
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)      // 16 voxels per MMA = two 1024-byte atoms further along K
+                        ptx::Wgmma<NT, decltype(f16)::value>::template ss<1, 1>(acc[am], da + (uint64_t)(128 * k), db + (uint64_t)(128 * k),
+                                                                                 ((b - b0) | k) ? 1u : 0u);
+                }
+                ptx::wgmma_commit();
+            };
+            if (P.fp16) issue(std::true_type{}); else issue(std::false_type{});
+            ptx::wgmma_wait<0>();
+            if (t == 0) ptx::mbar_arrive(&empty_bar[stage]);
+            if (++stage == stages) { stage = 0; phase ^= 1u; }
+        }
+#pragma unroll
+        for (int am = 0; am < NACC; ++am) {
+            ptx::reg_fence(acc[am]);
+            const int mp = am / P.t_group, ti = am - mp * P.t_group;
+            const int mt = mi * P.m_pair + mp, tap = tap0 + ti;
+            if (mp >= P.m_pair || ti >= ntap || mt >= P.m_tiles) continue;
+            float* tile = P.partial + ((((size_t)tap * P.m_tiles + mt) * P.n_tiles + nt) * P.splits + split) * 128 * P.n_t;
+            store_partial<NT>(tile, P.n_t, wg, t, acc[am], b1 <= b0);
+        }
+    }
 }
 
 // channels-last (N, X*Y*Z, ld) -> planar (N, C, X*Y, Zp) with Zp = z pitch >= Z (a multiple of 8 so that every TMA stride is a
@@ -324,6 +310,31 @@ __global__ void __launch_bounds__(256) cl_to_planar_kernel(const uint16_t* __res
             if (zo >= 0 && zo < Zp) dst[(size_t)(c0 + c) * plane + (size_t)(vv / Z) * Zp + zo] = tile[v][c];
         }
     }
+}
+
+template <int NT, int NACC>
+int launch_wgrad_cl(const WgMapsCl& maps, const WgDevCl& P, int grid, int smem, cudaStream_t st) {
+    static int smem_set = 0;
+    if (smem > smem_set) {
+        NRPN_CUDA_TRY(cudaFuncSetAttribute(conv3d_wgrad_cl_kernel<NT, NACC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        smem_set = smem;
+    }
+    conv3d_wgrad_cl_kernel<NT, NACC><<<grid, kWgThreads, smem, st>>>(maps, P);
+    NRPN_LAUNCH_CHECK();
+    return NRPN_OK;
+}
+
+template <int NT>
+int launch_wgrad_planar(const WgMaps& maps, const WgDev& P, int grid, cudaStream_t st) {
+    constexpr int smem = kWgStages * (kWgABytes + NT * 128) + 1024 + 256;
+    static bool attr_set = false;
+    if (!attr_set) {
+        NRPN_CUDA_TRY(cudaFuncSetAttribute(conv3d_wgrad_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        attr_set = true;
+    }
+    conv3d_wgrad_kernel<NT><<<grid, kWgThreads, smem, st>>>(maps, P);
+    NRPN_LAUNCH_CHECK();
+    return NRPN_OK;
 }
 
 }  // namespace nrpn
@@ -377,8 +388,8 @@ static int wgrad_plan(const nrpn_wgrad_desc* d, WgDev& P) {
 }
 
 // K-splits of a wgrad launch: the work items (taps x Cout slices x Cin slices x splits) run on a persistent grid of one CTA per SM, so the split count
-// is chosen for the fullest last wave (3^3 256->256: 54 base items; 2 splits = 108 items filled 73 % of 148 SMs, 8 splits = 432 items fill 97 % of
-// three waves), smallest count on ties, and at least 8 voxel bricks per split.
+// is chosen for the fullest last wave (3^3 256->256 on 132 SMs: 54 base items; 2 splits = 108 items fill 82 % of one wave, 7 splits = 378 items
+// fill 95 % of three waves), smallest count on ties, and at least 8 voxel bricks per split.
 static int wgrad_pick_splits(int base, int bricks) {
     const int sms = num_sms();
     int best = 1; double best_util = 0.0;
@@ -411,17 +422,15 @@ static int wgrad_plan_cl(const nrpn_wgrad_desc* d, WgDevCl& P) {
     P.n_t = d->cin > 256 ? 256 : d->cin; P.n_tiles = d->cin / P.n_t; P.m_tiles = ceil_div(d->cout, 128);
     P.b_boxes = ceil_div(P.n_t, 64);
     static const bool pair_off = [] { const char* e = getenv("NRPN_WGRAD_MPAIR"); return e && e[0] == '0'; }();
-    P.m_pair = (P.m_tiles >= 2 && !pair_off) ? 2 : 1;
+    P.m_pair = (P.m_tiles >= 2 && !pair_off && 2 * P.b_boxes * 64 / 2 <= kWgAccRegs) ? 2 : 1;
     P.m_items = ceil_div(P.m_tiles, P.m_pair);
     {
         // taps per work item: their accumulators share one dY tile (the fill rate out of L2 bounds this kernel: 24 KB per four MMAs at N = 64 with one
-        // tap, 12 KB with four); as many as TMEM (512 columns) and a ring of >= 3 stages allow, at most 4
+        // tap, 12 KB with four); as many as the accumulator registers (kWgAccRegs per thread) and a ring of >= 3 stages allow, at most 4
         static const bool group_off = [] { const char* e = getenv("NRPN_WGRAD_TAPGROUP"); return e && e[0] == '0'; }();
-        P.acc_stride = 32;
-        while (P.acc_stride < P.n_t) P.acc_stride <<= 1;
         P.t_group = 1;
         for (int t = 2; t <= 4 && !group_off; t <<= 1) {
-            if (t > d->n_taps || P.m_pair * t * P.acc_stride > 512) break;
+            if (t > d->n_taps || P.m_pair * t * P.b_boxes * 64 / 2 > kWgAccRegs) break;
             if ((227 * 1024 - 2048) / ((2 * P.m_pair + t * P.b_boxes) * kWgBox) < 3) break;
             P.t_group = t;
         }
@@ -485,15 +494,18 @@ static int wgrad_run_cl(const nrpn_wgrad_desc* d, cudaStream_t st) {
     for (int l = d->n_levels; l < NRPN_CONV_MAX_LEVELS; ++l) { maps.dy[l] = maps.dy[0]; maps.x[l] = maps.x[0]; }
     P.partial = reinterpret_cast<float*>(align_up((size_t)d->workspace, 256));
     const int smem = P.stages * (2 * P.m_pair + P.t_group * P.b_boxes) * kWgBox + 1024 + 256;
-    static int smem_set = 0;
-    if (smem > smem_set) {
-        NRPN_CUDA_TRY(cudaFuncSetAttribute(conv3d_wgrad_cl_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        smem_set = smem;
-    }
     const int items = P.n_groups * P.m_items * P.n_tiles * P.splits;
     const int grid = items < num_sms() ? items : num_sms();
-    conv3d_wgrad_cl_kernel<<<grid, kWgThreads, smem, st>>>(maps, P);
-    NRPN_LAUNCH_CHECK();
+    const int nacc = P.m_pair * P.t_group;
+    int rc;
+    switch (P.b_boxes) {
+        case 1: rc = nacc == 1 ? launch_wgrad_cl<64, 1>(maps, P, grid, smem, st) : nacc == 2 ? launch_wgrad_cl<64, 2>(maps, P, grid, smem, st)
+                                                                                          : launch_wgrad_cl<64, 4>(maps, P, grid, smem, st); break;
+        case 2: rc = nacc == 1 ? launch_wgrad_cl<128, 1>(maps, P, grid, smem, st) : launch_wgrad_cl<128, 2>(maps, P, grid, smem, st); break;
+        case 3: rc = launch_wgrad_cl<192, 1>(maps, P, grid, smem, st); break;
+        default: rc = launch_wgrad_cl<256, 1>(maps, P, grid, smem, st); break;
+    }
+    if (rc) return rc;
     const size_t total = (size_t)P.n_taps * P.cout * P.cin;
     size_t blocks = ceil_div(total, (size_t)256);
     if (blocks > (size_t)num_sms() * 8) blocks = (size_t)num_sms() * 8;
@@ -554,17 +566,15 @@ int nrpn_conv3d_wgrad(const nrpn_wgrad_desc* d, nrpn_stream_t stream) {
     }
     for (int l = d->n_levels; l < NRPN_CONV_MAX_LEVELS; ++l) { maps.dy[l] = maps.dy[0]; for (int k = 0; k < 3; ++k) maps.x[l][k] = maps.x[0][k]; }
     P.partial = reinterpret_cast<float*>(align_up((size_t)d->workspace, 256));
-    const int smem = kWgStages * (kWgABytes + P.n_t * 128) + 1024 + 256;
-    static int smem_set = 0;
-    if (smem > smem_set) {
-        NRPN_CUDA_TRY(cudaFuncSetAttribute(conv3d_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        smem_set = smem;
-    }
     const int items = P.n_taps * P.m_tiles * P.n_tiles * P.splits;
     const int grid = items < num_sms() ? items : num_sms();
     cudaStream_t st = (cudaStream_t)stream;
-    conv3d_wgrad_kernel<<<grid, kWgThreads, smem, st>>>(maps, P);
-    NRPN_LAUNCH_CHECK();
+    {
+        const int nt_pad = ceil_div(P.n_t, 64) * 64;       // MMA width: columns past n_t are never stored
+        const int rc = nt_pad == 64 ? launch_wgrad_planar<64>(maps, P, grid, st) : nt_pad == 128 ? launch_wgrad_planar<128>(maps, P, grid, st)
+                     : nt_pad == 192 ? launch_wgrad_planar<192>(maps, P, grid, st) : launch_wgrad_planar<256>(maps, P, grid, st);
+        if (rc) return rc;
+    }
     const size_t total = (size_t)P.n_taps * P.cout * P.cin;
     size_t blocks = ceil_div(total, (size_t)256);
     if (blocks > (size_t)num_sms() * 8) blocks = (size_t)num_sms() * 8;

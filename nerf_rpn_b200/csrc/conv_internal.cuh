@@ -27,11 +27,9 @@ inline EncodeTiledFn get_encode() {
 }
 
 // Launch with programmatic stream serialization (the kernel must call ptx::pdl_wait() before reading its inputs): the
-// prologue of layer i+1 (barrier init, TMEM allocation, tensor-map prefetch) overlaps the tail of layer i, also inside a
-// captured CUDA graph.  NRPN_PDL=0 falls back to ordinary stream-ordered launches.
-// Measured [B200]: it helps the latency-bound launches (config 1, 32^3 VGG: 1.92 -> 1.83 ms per scene) and costs up to 5 % on
-// the 4-scene ResNet step whose layers run tens of tiles per CTA, so it is applied only to launches of at most 2 tiles per SM
-// slot (`small`); NRPN_PDL=2 forces it on for every launch.
+// prologue of layer i+1 (barrier init, tensor-map prefetch) overlaps the tail of layer i, also inside a captured CUDA graph.
+// NRPN_PDL=0 falls back to ordinary stream-ordered launches.  It is applied only to latency-bound launches of at most 2 tiles
+// per SM slot (`small`); NRPN_PDL=2 forces it on for every launch.
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool small, Args&&... args) {
     static const int mode = [] { const char* e = getenv("NRPN_PDL"); return e ? (e[0] - '0') : 1; }();

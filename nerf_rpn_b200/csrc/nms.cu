@@ -1087,7 +1087,7 @@ static int nms_run_cells(const float* boxes, int box_dim, const float* scores, c
     cl_state_init_kernel<<<ceil_div(n, 256), 256, 0, st>>>(w.sgroup, n, ignore_group, c.state, c.adj_cnt);
     NRPN_LAUNCH_CHECK();
 
-    static const int pair_grid = [] { int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); return 2 * sms; }();
+    static const int pair_grid = [] { int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); return 2 * sms; }();
     PairArgs pa;
     pa.prep = w.prep; pa.box_dim = box_dim; pa.thr = thr; pa.thr_m = thr_m; pa.grid = w.grid;
     pa.qstart = c.B.start; pa.qrecs = c.B.recs; pa.item_start = c.B.item_start; pa.items = c.B.items; pa.work = c.meta;

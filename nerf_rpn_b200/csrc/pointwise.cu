@@ -297,7 +297,7 @@ const char* nrpn_status_string(int status) {
         case NRPN_ERR_UNSUPPORTED: return "unsupported shape";
         case NRPN_ERR_WORKSPACE: return "workspace too small";
         case NRPN_ERR_CUDA: return "CUDA error";
-        case NRPN_ERR_NO_DEVICE: return "no sm_100 device / driver entry point";
+        case NRPN_ERR_NO_DEVICE: return "no sm_90 device / driver entry point";
         default: return "unknown status";
     }
 }

@@ -1,5 +1,5 @@
 // Swin-3D support kernels (SwinTransformer_FPN, nerf_rpn/model/feature_extractor.py:382-789). The GEMMs of the transformer
-// (qkv, proj, MLP, patch merging, patch embedding) run on the tcgen05 implicit-GEMM kernel as 1x1x1 convolutions over
+// (qkv, proj, MLP, patch merging, patch embedding) run on the wgmma implicit-GEMM kernel as 1x1x1 convolutions over
 // channels-last token grids; this file holds what is left around them:
 //   patch_embed_pack      fp32 NCDHW grid -> (X/4, Y/4, Z/4, 256) bf16 patch rows    (Conv3d k4 s4 as a GEMM, :731-733)
 //   layernorm             per-token LayerNorm over C channels                        (:621,634,736)
@@ -8,7 +8,7 @@
 // Activations are (N, H, W, D, ld) bf16 with C real channels and ld >= C (ld a multiple of 64; channels [C, ld) stay zero).
 #include <cstdlib>
 #include "common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 
 namespace nrpn {
 
@@ -178,192 +178,157 @@ __global__ void __launch_bounds__(64) window_attention_kernel(AttnDev P) {
     }
 }
 
-// ---------------------------------------------------------------------------------------------- window attention on tcgen05
-// Two 64-token windows of the same head are stacked into ONE M = 128 problem: S = Q K^T is a 128 x 128 tcgen05.mma whose two
-// diagonal 64 x 64 blocks are the windows' score matrices (the off-diagonal blocks are never read); softmax runs from TMEM
-// (thread r <-> query row r: scale, relative-position bias, -100 region mask, exp); the un-normalised probabilities go back to
-// shared memory as bf16 with the other window's block zeroed, and O = P V is a second MMA (M 128, N 32, K 128) against V^T.
-// The 1/sum normalisation is applied to the fp32 accumulator.  Operands are written to shared memory by the threads
-// themselves (a token's q/k/v are 64 contiguous bytes each) in the 128B-swizzled K-major layout; V is transposed on the way.
-constexpr int kAttnThreads = 128;
-constexpr int kAttnSmem = 16384 /*Q*/ + 16384 /*K*/ + 2 * 4096 /*V^T*/ + 2 * 16384 /*P*/ + 1024 /*align*/ + 2048 /*table, regions, barriers*/;
+// ---------------------------------------------------------------------------------------------- window attention on wgmma
+// One warpgroup per (64-token window, head): S = Q K^T is an m64n64k32 wgmma into registers; softmax runs on the accumulator
+// fragments (a row's 64 scores are spread over the 4 threads of a quad: scale, relative-position bias, -100 region mask, exp,
+// max and sum through quad shuffles); the un-normalised probabilities go to shared memory as 16-bit values and O = P V is a
+// second wgmma (M 64, N 32, K 64) against V^T.  The 1/sum normalisation is applied to the fp32 accumulator.  Operands are
+// written to shared memory by the threads themselves (a token's q/k/v are 64 contiguous bytes each) in the 128B-swizzled
+// K-major layout; V is transposed on the way.  Two warpgroups per CTA work on two windows of the same head independently.
+constexpr int kAttnThreads = 256;
+constexpr int kAttnWgBytes = 8192 /*Q*/ + 8192 /*K*/ + 4096 /*V^T*/ + 8192 /*P*/;
+constexpr int kAttnSmem = 2 * kAttnWgBytes + 1024 /*align*/ + 1408 /*table*/ + 512 /*regions*/;
 
 __device__ __forceinline__ uint32_t attn_sw(int row, int chunk) { return (uint32_t)(row * 128 + ((chunk ^ (row & 7)) << 4)); }
 
-__global__ void __launch_bounds__(kAttnThreads) window_attention_tc_kernel(AttnDev P, int n_windows) {
+struct AttnTok { bool real; size_t tok; int ph, pw, pd; };
+
+__device__ __forceinline__ AttnTok attn_tok(const AttnDev& P, int w, int tw) {
+    AttnTok a;
+    const int wd = w % P.nwd; w /= P.nwd;
+    const int ww = w % P.nww; w /= P.nww;
+    const int wh = w % P.nwh; const int b = w / P.nwh;
+    a.ph = wh * 4 + (tw >> 4); a.pw = ww * 4 + ((tw >> 2) & 3); a.pd = wd * 4 + (tw & 3);   // position in the padded, shifted grid
+    const int sh_ = (a.ph + P.sh) % P.PH, sw_ = (a.pw + P.sw) % P.PW, sd_ = (a.pd + P.sd) % P.PD;
+    a.real = sh_ < P.H && sw_ < P.W && sd_ < P.D;
+    a.tok = (((size_t)b * P.H + sh_) * P.W + sw_) * P.D + sd_;
+    return a;
+}
+
+template <bool F16>
+__device__ __forceinline__ void attn_mma_s(float (&s)[32], uint64_t dq, uint64_t dk) {
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 2; ++k)                                   // head_dim 32 = two K-steps of 16
+        ptx::Wgmma<64, F16>::template ss<0, 0>(s, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), k ? 1u : 0u);
+    ptx::wgmma_commit();
+}
+template <bool F16>
+__device__ __forceinline__ void attn_mma_o(float (&o)[16], uint64_t dp, uint64_t dv) {
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)                                   // 64 keys = four K-steps of 16
+        ptx::Wgmma<32, F16>::template ss<0, 0>(o, dp + (uint64_t)(2 * k), dv + (uint64_t)(2 * k), k ? 1u : 0u);
+    ptx::wgmma_commit();
+}
+
+__global__ void __launch_bounds__(kAttnThreads, 2) window_attention_tc_kernel(AttnDev P, int n_windows) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* Qs = smem;
-    uint8_t* Ks = smem + 16384;
-    uint8_t* Vt = smem + 32768;                 // [2 tiles][32 rows (d)][64 tokens]
-    uint8_t* Ps = smem + 40960;                 // [2 tiles (key halves)][128 rows][64 keys]
-    float* tbl = reinterpret_cast<float*>(smem + 73728);          // 343 relative-position biases of this head
-    int* region = reinterpret_cast<int*>(smem + 73728 + 1408);    // 128
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 73728 + 1408 + 512);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
+    const int t = threadIdx.x & 127, wg = threadIdx.x >> 7;
+    uint8_t* Qs = smem + wg * kAttnWgBytes;
+    uint8_t* Ks = Qs + 8192;
+    uint8_t* Vt = Qs + 16384;                   // [32 rows (d)][64 tokens]
+    uint8_t* Ps = Qs + 20480;                   // [64 rows (queries)][64 keys]
+    float* tbl = reinterpret_cast<float*>(smem + 2 * kAttnWgBytes);          // 343 relative-position biases of this head
+    int* region = reinterpret_cast<int*>(smem + 2 * kAttnWgBytes + 1408) + wg * 64;
     const int head = blockIdx.y;
-    const int t = threadIdx.x, warp = t >> 5;
     const int hc = head * 32;
-    for (int i = t; i < 343; i += kAttnThreads) tbl[i] = P.table[i * P.heads + head];
-    if (t == 0) { ptx::mbar_init(&bars[0], 1); ptx::mbar_init(&bars[1], 1); ptx::fence_barrier_init(); }
-    if (warp == 0) { ptx::tmem_alloc(tmem_slot, 128); ptx::tmem_relinquish(); }
-    ptx::tc_fence_before();
+    for (int i = threadIdx.x; i < 343; i += kAttnThreads) tbl[i] = P.table[i * P.heads + head];
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     const bool shifted = (P.sh + P.sw + P.sd) > 0;
-    const int half = t >> 6, tw = t & 63;                          // stacked window (0/1), token inside it
-    const int ti = tw >> 4, tj = (tw >> 2) & 3, tk = tw & 3;
-    const uint32_t kIdescS = P.fp16 ? ptx::make_idesc_f16(128, 128) : ptx::make_idesc_bf16(128, 128);
-    const uint32_t kIdescO = P.fp16 ? ptx::make_idesc_f16(128, 32) : ptx::make_idesc_bf16(128, 32);
-    uint32_t phase = 0;
+    const uint64_t dq = ptx::make_desc_sw128(ptx::smem_u32(Qs)), dk = ptx::make_desc_sw128(ptx::smem_u32(Ks));
+    const uint64_t dv = ptx::make_desc_sw128(ptx::smem_u32(Vt)), dp = ptx::make_desc_sw128(ptx::smem_u32(Ps));
     for (int pair = blockIdx.x; pair * 2 < n_windows; pair += gridDim.x) {
-        int w = pair * 2 + half;
-        const bool have = w < n_windows;
-        const int wd = w % P.nwd; w /= P.nwd;
-        const int ww = w % P.nww; w /= P.nww;
-        const int wh = w % P.nwh; const int b = w / P.nwh;
-        const int ph = wh * 4 + ti, pw = ww * 4 + tj, pd = wd * 4 + tk;   // position in the padded, shifted grid
-        const int sh_ = (ph + P.sh) % P.PH, sw_ = (pw + P.sw) % P.PW, sd_ = (pd + P.sd) % P.PD;
-        const bool real = have && sh_ < P.H && sw_ < P.W && sd_ < P.D;
-        const size_t tok = have ? ((((size_t)b * P.H + sh_) * P.W + sw_) * P.D + sd_) : 0;
-        {   // ---- stage q, k (row t of the K-major tiles) and v (column t of V^T)
-            uint4 qv[4], kv[4], vv[4];
-            if (real) {
-                const __nv_bfloat16* row = P.qkv + tok * P.ld_qkv;
+        const int w = pair * 2 + wg;
+        if (w >= n_windows) break;
+        {   // ---- stage: threads 0-63 write q and k of token t (rows of the K-major tiles), threads 64-127 v (column of V^T)
+            const int tw = t & 63;
+            const AttnTok a = attn_tok(P, w, tw);
+            const __nv_bfloat16* row = P.qkv + a.tok * P.ld_qkv;
+            auto load = [&](int off, int i) -> uint4 {           // 8 channels of q / k / v; padding tokens carry the qkv bias
+                if (a.real) return __ldg(reinterpret_cast<const uint4*>(row + off + hc) + i);
+                uint32_t u[4];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) u[k] = pack_act2(P.qkv_bias[off + hc + i * 8 + 2 * k], P.qkv_bias[off + hc + i * 8 + 2 * k + 1], P.fp16);
+                return make_uint4(u[0], u[1], u[2], u[3]);
+            };
+            if (t < 64) {
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
-                    qv[i] = __ldg(reinterpret_cast<const uint4*>(row + hc) + i);
-                    kv[i] = __ldg(reinterpret_cast<const uint4*>(row + P.C + hc) + i);
-                    vv[i] = __ldg(reinterpret_cast<const uint4*>(row + 2 * P.C + hc) + i);
+                    *reinterpret_cast<uint4*>(Qs + attn_sw(tw, i)) = load(0, i);
+                    *reinterpret_cast<uint4*>(Ks + attn_sw(tw, i)) = load(P.C, i);
                 }
             } else {
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
-                    uint32_t a[4], c[4], e[4];
+                    const uint4 vv = load(2 * P.C, i);
+                    const __nv_bfloat16* e = reinterpret_cast<const __nv_bfloat16*>(&vv);
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        const int d = i * 8 + u * 2;
-                        a[u] = have ? pack_act2(P.qkv_bias[hc + d], P.qkv_bias[hc + d + 1], P.fp16) : 0u;
-                        c[u] = have ? pack_act2(P.qkv_bias[P.C + hc + d], P.qkv_bias[P.C + hc + d + 1], P.fp16) : 0u;
-                        e[u] = have ? pack_act2(P.qkv_bias[2 * P.C + hc + d], P.qkv_bias[2 * P.C + hc + d + 1], P.fp16) : 0u;
-                    }
-                    qv[i] = make_uint4(a[0], a[1], a[2], a[3]); kv[i] = make_uint4(c[0], c[1], c[2], c[3]); vv[i] = make_uint4(e[0], e[1], e[2], e[3]);
+                    for (int u = 0; u < 8; ++u) *reinterpret_cast<__nv_bfloat16*>(Vt + attn_sw(i * 8 + u, tw >> 3) + (tw & 7) * 2) = e[u];
                 }
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                *reinterpret_cast<uint4*>(Qs + attn_sw(t, i)) = qv[i];
-                *reinterpret_cast<uint4*>(Ks + attn_sw(t, i)) = kv[i];
-            }
-            uint8_t* vt = Vt + half * 4096;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const __nv_bfloat16* e = reinterpret_cast<const __nv_bfloat16*>(&vv[i]);
-#pragma unroll
-                for (int u = 0; u < 8; ++u) {
-                    const int d = i * 8 + u;
-                    *reinterpret_cast<__nv_bfloat16*>(vt + attn_sw(d, tw >> 3) + (tw & 7) * 2) = e[u];
-                }
-            }
-            auto reg1 = [](int p, int Pext, int s) { return s == 0 ? 2 : (p < Pext - 4 ? 0 : (p < Pext - s ? 1 : 2)); };
-            region[t] = shifted ? (reg1(ph, P.PH, P.sh) * 9 + reg1(pw, P.PW, P.sw) * 3 + reg1(pd, P.PD, P.sd)) : 0;
-        }
-        ptx::fence_proxy_async();
-        ptx::tc_fence_before();
-        __syncthreads();
-        if (warp == 0) {
-            ptx::tc_fence_after();
-            if (ptx::elect_one()) {
-                const uint64_t da = ptx::make_desc_sw128(ptx::smem_u32(Qs)), db = ptx::make_desc_sw128(ptx::smem_u32(Ks));
-#pragma unroll
-                for (int k = 0; k < 2; ++k)                                   // head_dim 32 = two K-steps of 16
-                    ptx::umma_bf16(tmem, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), kIdescS, k ? 1u : 0u);
-                ptx::umma_commit(&bars[0]);
-            }
-            __syncwarp();
-        }
-        ptx::mbar_wait(&bars[0], phase);
-        ptx::tc_fence_after();
-        // ---- softmax of row t over its own window's 64 keys
-        float sc[64];
-        {
-            uint32_t r0[32], r1[32];
-            const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)(half * 64);
-            ptx::tmem_ld_32x32(taddr, r0);
-            ptx::tmem_ld_32x32(taddr + 32, r1);
-            ptx::tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) { sc[j] = __uint_as_float(r0[j]); sc[32 + j] = __uint_as_float(r1[j]); }
-        }
-        const int myreg = region[t];
-        float mx = -INFINITY;
-#pragma unroll
-        for (int j = 0; j < 64; ++j) {
-            const int ji = j >> 4, jj = (j >> 2) & 3, jk = j & 3;
-            float a = sc[j] * 0.17677669529663687f + tbl[(ti - ji + 3) * 49 + (tj - jj + 3) * 7 + (tk - jk + 3)];
-            if (shifted && region[half * 64 + j] != myreg) a += -100.0f;
-            sc[j] = a; mx = fmaxf(mx, a);
-        }
-        float sum = 0.f;
-        {
-            uint8_t* mine = Ps + half * 16384;
-            uint8_t* other = Ps + (1 - half) * 16384;
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                float e[8];
-#pragma unroll
-                for (int u = 0; u < 8; ++u) { e[u] = __expf(sc[c * 8 + u] - mx); sum += e[u]; }
-                uint32_t pk[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) pk[u] = pack_act2(e[2 * u], e[2 * u + 1], P.fp16);
-                *reinterpret_cast<uint4*>(mine + attn_sw(t, c)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                *reinterpret_cast<uint4*>(other + attn_sw(t, c)) = make_uint4(0u, 0u, 0u, 0u);
+                auto reg1 = [](int p, int Pext, int s) { return s == 0 ? 2 : (p < Pext - 4 ? 0 : (p < Pext - s ? 1 : 2)); };
+                region[tw] = shifted ? (reg1(a.ph, P.PH, P.sh) * 9 + reg1(a.pw, P.PW, P.sw) * 3 + reg1(a.pd, P.PD, P.sd)) : 0;
             }
         }
         ptx::fence_proxy_async();
-        ptx::tc_fence_before();
-        __syncthreads();                                   // every S row has been read: its TMEM columns may be overwritten by O
-        if (warp == 0) {
-            ptx::tc_fence_after();
-            if (ptx::elect_one()) {
+        ptx::named_barrier(1 + wg, 128);
+        float s[32];
+        ptx::reg_fence(s);
+        if (P.fp16) attn_mma_s<true>(s, dq, dk); else attn_mma_s<false>(s, dq, dk);
+        ptx::wgmma_wait<0>();
+        ptx::reg_fence(s);
+        // ---- softmax of rows q0 = frag_row(t, 0) and q0 + 8 over the window's 64 keys (this thread: 16 keys of each)
+        float sum[2];
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const uint64_t da = ptx::make_desc_sw128(ptx::smem_u32(Ps + h * 16384));
-                    const uint64_t db = ptx::make_desc_sw128(ptx::smem_u32(Vt + h * 4096));
+        for (int h = 0; h < 2; ++h) {
+            const int q = ptx::frag_row(t, h);
+            const int ti = q >> 4, tj = (q >> 2) & 3, tk = q & 3;
+            const int myreg = region[q];
+            float mx = -INFINITY;
 #pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        ptx::umma_bf16(tmem, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), kIdescO, (h | k) ? 1u : 0u);
+            for (int j = 0; j < 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int c = ptx::frag_col(t, j) + e;
+                    const int ji = c >> 4, jj = (c >> 2) & 3, jk = c & 3;
+                    float a = s[4 * j + 2 * h + e] * 0.17677669529663687f + tbl[(ti - ji + 3) * 49 + (tj - jj + 3) * 7 + (tk - jk + 3)];
+                    if (shifted && region[c] != myreg) a += -100.0f;
+                    s[4 * j + 2 * h + e] = a; mx = fmaxf(mx, a);
                 }
-                ptx::umma_commit(&bars[1]);
-            }
-            __syncwarp();
-        }
-        ptx::mbar_wait(&bars[1], phase);
-        ptx::tc_fence_after();
-        {
-            uint32_t o[32];
-            ptx::tmem_ld_32x32(tmem + ((uint32_t)(warp * 32) << 16), o);
-            ptx::tmem_ld_wait();
-            if (real) {
-                const float inv = 1.0f / sum;
-                __nv_bfloat16* orow = P.out + tok * P.ld_out + hc;
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            float sm = 0.f;
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    uint32_t pk[4];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u)
-                        pk[u] = pack_act2(__uint_as_float(o[i * 8 + 2 * u]) * inv, __uint_as_float(o[i * 8 + 2 * u + 1]) * inv, P.fp16);
-                    *(reinterpret_cast<uint4*>(orow) + i) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                }
+            for (int j = 0; j < 8; ++j) {
+                const float e0 = __expf(s[4 * j + 2 * h] - mx), e1 = __expf(s[4 * j + 2 * h + 1] - mx);
+                sm += e0; sm += e1;
+                *reinterpret_cast<uint32_t*>(Ps + attn_sw(q, j) + (t & 3) * 4) = pack_act2(e0, e1, P.fp16);
             }
+            sm += __shfl_xor_sync(0xffffffffu, sm, 1);
+            sm += __shfl_xor_sync(0xffffffffu, sm, 2);
+            sum[h] = sm;
         }
-        ptx::tc_fence_before();
-        __syncthreads();                                   // O has been read, the operand tiles may be rewritten
-        ptx::tc_fence_after();
-        phase ^= 1u;
+        ptx::fence_proxy_async();
+        ptx::named_barrier(1 + wg, 128);
+        float o[16];
+        ptx::reg_fence(o);
+        if (P.fp16) attn_mma_o<true>(o, dp, dv); else attn_mma_o<false>(o, dp, dv);
+        ptx::wgmma_wait<0>();
+        ptx::reg_fence(o);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int q = ptx::frag_row(t, h);
+            const AttnTok a = attn_tok(P, w, q);
+            if (!a.real) continue;
+            const float inv = 1.0f / sum[h];
+            __nv_bfloat16* orow = P.out + a.tok * P.ld_out + hc;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                *reinterpret_cast<uint32_t*>(orow + ptx::frag_col(t, j)) = pack_act2(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv, P.fp16);
+        }
+        ptx::named_barrier(1 + wg, 128);                   // the operand tiles and regions may be rewritten
     }
-    if (warp == 0) ptx::tmem_dealloc(tmem, 128);
 }
 
 static inline unsigned grid_for(size_t total, int block) {
@@ -420,7 +385,7 @@ int nrpn_window_attention(const void* qkv, int ld_qkv, void* out, int ld_out, co
     P.nwh = P.PH / 4; P.nww = P.PW / 4; P.nwd = P.PD / 4;
     const long windows = (long)n * P.nwh * P.nww * P.nwd;
     if (windows > 0x7fffffffL || heads > 65535) return NRPN_ERR_UNSUPPORTED;
-    // tcgen05 path: needs 16-byte aligned 64-byte q/k/v segments; NRPN_ATTN_TC=0 selects the CUDA-core kernel (A/B testing)
+    // tensor-core path: needs 16-byte aligned 64-byte q/k/v segments; NRPN_ATTN_TC=0 selects the CUDA-core kernel (A/B testing)
     const char* e = getenv("NRPN_ATTN_TC");
     const bool tc = !(e && e[0] == '0') && ld_qkv % 8 == 0 && ld_out % 8 == 0 && c % 8 == 0 &&
                     reinterpret_cast<uintptr_t>(qkv) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0;
@@ -431,7 +396,7 @@ int nrpn_window_attention(const void* qkv, int ld_qkv, void* out, int ld_out, co
             attr_set = true;
         }
         const long pairs = (windows + 1) / 2;
-        long gx = (long)num_sms() * 3 / heads;              // ~3 resident CTAs per SM in total, each looping over window pairs
+        long gx = (long)num_sms() * 2 / heads;              // 2 resident CTAs per SM in total, each looping over window pairs
         if (gx < 1) gx = 1;
         if (gx > pairs) gx = pairs;
         window_attention_tc_kernel<<<dim3((unsigned)gx, heads), kAttnThreads, kAttnSmem, (cudaStream_t)stream>>>(P, (int)windows);

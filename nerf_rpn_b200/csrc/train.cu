@@ -1,4 +1,4 @@
-// Training-step kernels around the three tcgen05 GEMMs (fprop, dgrad = fprop on mirrored weights, wgrad): everything of
+// Training-step kernels around the three wgmma GEMMs (fprop, dgrad = fprop on mirrored weights, wgrad): everything of
 // `loss.backward(); optimizer.step()` for the anchor RPN (SURVEY.md 8(a) a18, config 4) that is not a convolution.
 //   BatchNorm3d in TRAIN mode  (feature_extractor.py:38-43,48-68 under model.train()): batch statistics, normalise (+ residual)
 //                               (+ ReLU), running-stat update; backward = two per-channel reductions + one pointwise pass

@@ -109,7 +109,7 @@ class RPNInferenceEngine:
         L = {}
         kinds = {"ResNet_FPN_256": "resnet", "VGG_FPN": "vgg", "SwinTransformer_FPN": "swin"}
         if type(bb).__name__ not in kinds:
-            raise NotImplementedError(f"nerf_rpn_b200: backbone {type(bb).__name__} is not implemented by the B200 engine "
+            raise NotImplementedError(f"nerf_rpn_b200: backbone {type(bb).__name__} is not implemented by the CUDA engine "
                                       "(ResNet_FPN_256, VGG_FPN, SwinTransformer_FPN are)")
         self.kind = kinds[type(bb).__name__]
         if self.kind == "resnet":          # the layer plan below is the configuration run_rpn.py:276 builds; anything else would run silently wrong
@@ -148,7 +148,7 @@ class RPNInferenceEngine:
         self._plans.clear()
 
     def _pack_swin(self, L, device):
-        """SwinTransformer_FPN (feature_extractor.py:689-789). Every Linear becomes a 1x1x1 conv of the tcgen05 kernel; widths
+        """SwinTransformer_FPN (feature_extractor.py:689-789). Every Linear becomes a 1x1x1 conv of the wgmma kernel; widths
         that are not multiples of 64 (96 at stage 0) live in rows padded with zero channels."""
         bb = self.backbone
         f32 = lambda t: t.detach().float().to(device).contiguous()
@@ -278,7 +278,7 @@ class RPNInferenceEngine:
         if self.backbone.training or (self.head is not None and self.head.training):
             raise NotImplementedError(
                 "nerf_rpn_b200: training-mode forward (BatchNorm batch statistics, RPN losses, gradients) is not "
-                "implemented by the B200 engine yet; call .eval() (inference) -- there is no PyTorch fallback")
+                "implemented by the CUDA engine yet; call .eval() (inference) -- there is no PyTorch fallback")
 
     def forward_device(self, grids: torch.Tensor, valid_dims: Optional[Sequence[Sequence[int]]] = None):
         """grids: (N,4,X,Y,Z) fp32 CUDA.  Returns the plan whose output buffers hold the results (no host sync)."""
@@ -729,8 +729,7 @@ class _Plan:
         runs on the current stream, the others on branch streams forked from / joined to it -- eagerly, or as parallel branches of the
         captured side-stream graph -- so the chain's critical path is one scene long, not n."""
         fs = self._post[par]
-        # MEASURED on the B200 (profiles/r02_bench_post_parallel_ab.txt, 4 scenes per step): branches 215.7 scenes/s vs one chain 224.2 / 224.9 --
-        # the chain is off the critical path already (high-priority side stream) and four concurrent chains only take SM slots from the
+        # The chain is off the critical path already (high-priority side stream) and four concurrent chains only take SM slots from the
         # convolutions; the serial chain is the default, NRPN_POST_PARALLEL=1 selects the branches.
         if len(fs) == 1 or os.environ.get("NRPN_POST_PARALLEL", "0") != "1":
             for f in fs:

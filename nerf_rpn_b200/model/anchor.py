@@ -1,7 +1,7 @@
 """Anchor generator and RPN head. Mirrors nerf_rpn/model/anchor.py:
   AnchorGenerator3D   anchor.py:14-174
   RPNHead             anchor.py:177-213
-In the B200 engine anchors are never materialised (2.43 M x 6 floats per scene in the reference): the decode
+In the CUDA engine anchors are never materialised (2.43 M x 6 floats per scene in the reference): the decode
 kernel rebuilds the anchor of a selected candidate from its flat index.  AnchorGenerator3D therefore only has to
 produce the per-level cell anchors in the reference's order -- which comes from iterating a Python set of
 permutations (anchor.py:40-46,57-60) and is reproduced by evaluating the same expression.

@@ -2,7 +2,7 @@
 FCOSOverNeRF :287-386) and fcos/inference.py:11-46 (FCOSPostProcessor's hyper-parameters): same class names, constructor
 arguments, attribute / parameter names (state_dict keys `fcos_module.head.{cls_tower,bbox_tower}.{i}.*`, `cls_logits.*`,
 `bbox_pred.*`, `centerness.*`, `scales.{i}.scale`) and creation / init order, so seeds and checkpoints line up.
-Inference (`--norm_reg_targets --centerness_on_reg`, the flags of test_fcos.sh) runs on the fused B200 engine.  The training LOSS
+Inference (`--norm_reg_targets --centerness_on_reg`, the flags of test_fcos.sh) runs on the fused CUDA engine.  The training LOSS
 (fcos/loss.py) is built (`FCOSModule.loss_evaluator`, model/fcos/loss.py: two kernels + one autograd node over the head outputs);
 the backward pass of the FCOS towers (GroupNorm) and a captured FCOS training step are not, so `FCOSOverNeRF.forward` still raises
 in training mode."""

@@ -143,7 +143,7 @@ class _FCOSLoss(torch.autograd.Function):
 
 
 class FCOSLossComputation(object):
-    """This class computes the FCOS losses (3-D, binary objectness) on the B200 kernels; see the module docstring."""
+    """This class computes the FCOS losses (3-D, binary objectness) on the CUDA kernels; see the module docstring."""
 
     def __init__(self, fpn_strides, center_sampling_radius, iou_loss_type, norm_reg_targets, world_size, use_obb, use_additional_l1_loss,
                  proj2d_loss_weight=0.0):

@@ -4,7 +4,7 @@
 The modules own ordinary nn.Conv3d / nn.BatchNorm3d parameters, created in the reference's order so that
 torch.manual_seed(s) reproduces the reference's initial weights and state_dict keys are identical
 (conv1.weight, bn1.*, layers.{s}.{b}.conv{1,2,3}.weight, ..., smooths.{i}.*, latlayers.{i}.*; SURVEY.md section 5).
-forward() never calls those nn modules: it runs the pre-packed tcgen05 engine (nerf_rpn_b200/engine.py).
+forward() never calls those nn modules: it runs the pre-packed wgmma engine (nerf_rpn_b200/engine.py).
 VGG_FPN (config 1) and SwinTransformer_FPN (config 3) follow below on the same engine.
 """
 from typing import List
@@ -31,7 +31,7 @@ class Bottleneck(nn.Module):
         self.stride = stride
 
     def forward(self, x):
-        """(N, inplanes, W, L, H) fp32 CUDA -> (N, 4*planes, w, l, h): feature_extractor.py:48-68 on the tcgen05 kernels (eval mode).
+        """(N, inplanes, W, L, H) fp32 CUDA -> (N, 4*planes, w, l, h): feature_extractor.py:48-68 on the wgmma kernels (eval mode).
         Inside ResNet_FPN_256 the same layers run as part of the captured engine; this is the stand-alone entry point."""
         from ._eager import bottleneck_forward
         return bottleneck_forward(self, x, getattr(self, "precision", None))
@@ -44,7 +44,7 @@ class ResNet_FPN_256(EngineHolder, nn.Module):
         super().__init__()
         self.precision = _resolve_precision(precision)
         if input_dim != 4 or not is_max_pool or block is not Bottleneck:
-            raise NotImplementedError("the B200 engine implements the configuration run_rpn.py builds: "
+            raise NotImplementedError("the CUDA engine implements the configuration run_rpn.py builds: "
                                       "ResNet_FPN_256(Bottleneck, [3,4,6,3], input_dim=4, is_max_pool=True)")
         self.in_planes = 64
         self.out_channels = 256
@@ -96,7 +96,7 @@ class ResNet_FPN_256(EngineHolder, nn.Module):
 def _not_built(name):
     class _Missing(nn.Module):
         def __init__(self, *a, **k):
-            raise NotImplementedError(f"nerf_rpn_b200: backbone {name} is not implemented by the B200 engine (built: ResNet_FPN_256, VGG_FPN, "
+            raise NotImplementedError(f"nerf_rpn_b200: backbone {name} is not implemented by the CUDA engine (built: ResNet_FPN_256, VGG_FPN, "
                                       "SwinTransformer_FPN -- the backbones of BASELINE.json's configurations; the name is importable because "
                                       "run_rpn.py:18-20 imports it)")
     _Missing.__name__ = name
@@ -124,7 +124,7 @@ class VGG_FPN(EngineHolder, nn.Module):
         super().__init__()
         self.precision = _resolve_precision(precision)
         if conv_at_start or in_channels != 4 or not cfg.endswith("F"):
-            raise NotImplementedError("the B200 engine implements VGG_FPN(cfg in {AF,DF,EF}, 4, batch_norm, input_size)")
+            raise NotImplementedError("the CUDA engine implements VGG_FPN(cfg in {AF,DF,EF}, 4, batch_norm, input_size)")
         from .fpn import FPN
         self.out_channels = 256
         self.layers = self.make_layers(vgg_cfgs[cfg], in_channels, batch_norm, input_size)
@@ -243,7 +243,7 @@ class SwinTransformer_FPN(EngineHolder, nn.Module):
         from functools import partial
         from .fpn import FPN
         if list(patch_size) != [4, 4, 4] or list(window_size) != [4, 4, 4] or input_dim != 4 or not expand_dim or dropout or attention_dropout:
-            raise NotImplementedError("the B200 engine implements patch 4^3 / window 4^3 / 4 input channels (run_rpn.py:286-292)")
+            raise NotImplementedError("the CUDA engine implements patch 4^3 / window 4^3 / 4 input channels (run_rpn.py:286-292)")
         norm_layer = norm_layer or partial(nn.LayerNorm, eps=1e-5)
         block = block or SwinTransformerBlock
         downsample_layer = downsample_layer or PatchMerging

@@ -124,7 +124,7 @@ class NeRFRegionProposalNetwork(nn.Module):
 
     # ------------------------------------------------------------------------------------------------ training
     def train_engine(self, **kw):
-        """The B200 training engine bound to this model (nerf_rpn_b200/train.py).  Created on first use; keyword arguments (precision,
+        """The CUDA training engine bound to this model (nerf_rpn_b200/train.py).  Created on first use; keyword arguments (precision,
         lr, weight_decay, clip_grad_norm, reg_loss_weight, process_group ...) configure a NEW engine."""
         from ..train import RPNTrainEngine
         if self._train_engine is None or kw:
@@ -134,7 +134,7 @@ class NeRFRegionProposalNetwork(nn.Module):
     def _forward_train(self, meshes, targets):
         """Training-mode forward as the reference defines it (nerf_rpn.py:166-217 + rpn.py:514-534): returns losses that carry a
         grad_fn, so the UNMODIFIED loop of run_rpn.py:384-395 (`loss.backward(); clip_grad_norm_; optimizer.step()`) and a DDP
-        wrapper drive the B200 forward / backward kernels: torch.autograd only sees ONE node whose backward runs the engine's launch
+        wrapper drive the CUDA forward / backward kernels: torch.autograd only sees ONE node whose backward runs the engine's launch
         list and hands every parameter its gradient."""
         if targets is None:
             raise ValueError("targets should not be None")

@@ -202,7 +202,7 @@ def conv3d_variant(levels, w, shift, cin, cout, taps, stride=1, relu=False, out_
 def conv3d_fprop(levels: Sequence[ConvLevelArgs], w: torch.Tensor, shift: torch.Tensor, cin: int, cout: int,
                  taps: Sequence[Sequence[int]], stride: int = 1, relu: bool = False, out_fp32: bool = False,
                  workspace: Optional[torch.Tensor] = None):
-    """One persistent tcgen05 implicit-GEMM launch over 1..4 levels sharing (w, shift).  `workspace`: optional uint8
+    """One persistent wgmma implicit-GEMM launch over 1..4 levels sharing (w, shift).  `workspace`: optional uint8
     tensor that was zero-filled once (split-K scratch, left zero-filled by every launch)."""
     d = _conv_desc(levels, w, shift, cin, cout, taps, stride, relu, out_fp32)
     if workspace is not None:
@@ -240,7 +240,7 @@ def to_planar(x: torch.Tensor, z_shift: int = 0) -> torch.Tensor:
 
 def conv3d_wgrad(dys: Sequence[torch.Tensor], xs: Sequence[torch.Tensor], taps: Sequence[Sequence[int]], operands: str = "channels_last") -> torch.Tensor:
     """dW (taps, Cout, Cin) fp32 of a stride-1 'same' conv from channels-last 16-bit dY (N,X,Y,Z,Cout) and X (N,X,Y,Z,Cin), one pair per
-    pyramid level that shares the weights.  operands="channels_last": the tensors are read where they live (MN-major tcgen05 operands);
+    pyramid level that shares the weights.  operands="channels_last": the tensors are read where they live (MN-major wgmma operands);
     "planar": through transposed, z-shifted staging copies (tap z offsets in {-1, 0, +1}) -- the earlier path, kept for comparison."""
     if operands == "channels_last":
         return _conv3d_wgrad_cl(dys, xs, taps)

@@ -1,4 +1,4 @@
-"""Weight pre-packing for the tcgen05 implicit-GEMM convolution (host-side, runs once per checkpoint).
+"""Weight pre-packing for the wgmma implicit-GEMM convolution (host-side, runs once per checkpoint).
 
 Reference layouts: nn.Conv3d.weight is (Cout, Cin, kx, ky, kz) fp32 over an NCDHW (N,C,W,L,H) input
 (feature_extractor.py:36-43,163,178,184; anchor.py:190-198).  The kernel wants one K-major (Cout x Cin) bf16
@@ -131,7 +131,7 @@ def pack_stem_s1_weight(w: torch.Tensor, scale: Optional[torch.Tensor] = None, d
 
 def pack_conv_weight_dgrad(w: torch.Tensor, dtype=torch.bfloat16):
     """Data-gradient weights of a stride-1 'same' Conv3d: dL/dx = conv(dL/dy, W') with W'[ci, co, a, b, c] = W[co, ci, k-1-a, k-1-b, k-1-c]
-    (taps mirrored, matrices transposed), so the backward-data pass of every stride-1 layer runs on the SAME tcgen05 implicit-GEMM
+    (taps mirrored, matrices transposed), so the backward-data pass of every stride-1 layer runs on the SAME wgmma implicit-GEMM
     kernel as the forward pass (row a18: first building block of the training path; weight gradients need a voxel-major GEMM and
     are not built).  Returns (packed (taps, CinPad, CoutPad... as the kernel's (taps, N, K)), taps)."""
     wt = w.detach().float().permute(1, 0, 2, 3, 4).flip(2, 3, 4).contiguous()

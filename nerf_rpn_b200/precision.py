@@ -1,5 +1,5 @@
-"""Numeric modes of the B200 engine (DESIGN.md section 4).  Every mode multiplies 16-bit operands on tcgen05 (`kind::f16`, same
-tensor rate) and accumulates in fp32 in TMEM; they differ in what the 16 bits are:
+"""Numeric modes of the CUDA engine (DESIGN.md section 4).  Every mode multiplies 16-bit operands on wgmma (same tensor rate
+for fp16 and bf16) and accumulates in fp32 registers; they differ in what the 16 bits are:
 
   "bf16"     bf16 activations and weights.  8-bit significand: feature maps ~8e-3 (norm-wise) off the fp32 reference.  Cannot
              overflow on unnormalised activations.  BASELINE.json config 2 names this dtype; kept as a labelled bench line.

@@ -1,4 +1,4 @@
-"""Training step of the anchor RPN on the B200 kernels (SURVEY.md 8(a) a18, BASELINE config 4).
+"""Training step of the anchor RPN on the CUDA kernels (SURVEY.md 8(a) a18, BASELINE config 4).
 
 Mirrors what `losses = model(rgbsigma, boxes); loss.backward(); clip_grad_norm_; optimizer.step()` computes in the reference
   NeRFRegionProposalNetwork.forward (train)   nerf_rpn/model/nerf_rpn.py:166-217
@@ -6,8 +6,8 @@ Mirrors what `losses = model(rgbsigma, boxes); loss.backward(); clip_grad_norm_;
   RegionProposalNetwork.forward (train)       nerf_rpn/model/rpn.py:514-534  (assign targets, sample 256, BCE + smooth-L1)
   Trainer.train_epoch                         nerf_rpn/run_rpn.py:372-412    (AdamW, clip_grad_norm_ 0.1, DDP gradient all-reduce)
 as a fixed list of libnerf_rpn_b200 launches:
-  forward   conv (tcgen05 implicit GEMM, raw output) -> batch statistics -> normalise (+ residual) + ReLU, FPN / head as in inference
-  backward  per conv: wgrad (tcgen05, voxel-major contraction, written straight into the flat fp32 gradient bucket in nn.Conv3d's own
+  forward   conv (wgmma implicit GEMM, raw output) -> batch statistics -> normalise (+ residual) + ReLU, FPN / head as in inference
+  backward  per conv: wgrad (wgmma, voxel-major contraction, written straight into the flat fp32 gradient bucket in nn.Conv3d's own
             layout) and dgrad (the forward kernel on mirrored / transposed weights, branch gradients added in its epilogue);
             BatchNorm / ReLU / max-pool / up-sampling backward are bandwidth kernels (csrc/train.cu)
   update    the flat gradient bucket is all-reduced over NCCL in chunks, each launched as soon as the backward pass has produced it

@@ -35,7 +35,7 @@
 
 /* Arithmetic mode (orc_set_mode), mirrors NRPN_IOU_MODE of csrc/box_iou.cuh:
  *   0 (default)  the conventions above == the reference's CPU build on the golden vectors;
- *   bit 0        operation ORDER of the reference's torch-CUDA build, measured on the B200 by tools/ref_gpu_probe.py against the
+ *   bit 0        operation ORDER of the reference's torch-CUDA build, measured on the GPU by tools/ref_gpu_probe.py against the
  *                unmodified reference: box2corners_th's bmm = fma(y4, r1, x4*r0); torch.sum over the 24 masked vertices = four
  *                interleaved accumulators ((a0+a1)+a2)+a3; torch.sum over the 8 shoelace terms = (t0+t4 + t2+t6) + (t1+t5 + t3+t7);
  *   bit 1        sin / cos through float sinf / cosf (the CUDA build calls CUDA's; a CPU libm can only approximate that, so

@@ -8,10 +8,10 @@ The reference (lyclyc52/NeRF_RPN) is a script directory (no setup.py / pyproject
   1. copy /root/reference/nerf_rpn (Python sources, 660 KB) to oracle/_ref/nerf_rpn -- oracle/_ref/ is git-ignored
      (history stays free of reference sources) but NOT gpurun-ignored, so the copy ships with the snapshot;
   2. build the reference's ONE native op on the hot path, `sort_vertices` (model/rotated_iou/cuda_op/sort_vert.cpp,
-     sort_vert_kernel.cu -- K1 of SURVEY.md 2.2) with its own setup.py, unmodified, TORCH_CUDA_ARCH_LIST=10.0, inside
+     sort_vert_kernel.cu -- K1 of SURVEY.md 2.2) with its own setup.py, unmodified, TORCH_CUDA_ARCH_LIST=9.0, inside
      the copy (the reference tree is read-only).
 
-On the B200 box this gives the true GPU oracle (the reference's torch-CUDA IoU chain + K1 + Python NMS + cuDNN convs)
+On the GPU machine this gives the true GPU oracle (the reference's torch-CUDA IoU chain + K1 + Python NMS + cuDNN convs)
 and the incumbent whose scenes/s bench.py reports next to ours.  `python oracle/build_ref.py` or build_ref() from
 __graft_entry__.build(); a no-op when /root/reference is absent (the GPU box uses the staged files).
 """
@@ -52,7 +52,7 @@ def build_ref(force: bool = False, verbose: bool = True):
         os.makedirs(os.path.dirname(REF_DST), exist_ok=True)
         shutil.copytree(REF_SRC, REF_DST, ignore=shutil.ignore_patterns("__pycache__", "*.pyc"), dirs_exist_ok=True)
     if k1_path() is None:
-        env = dict(os.environ, TORCH_CUDA_ARCH_LIST="10.0", MAX_JOBS="4")
+        env = dict(os.environ, TORCH_CUDA_ARCH_LIST="9.0", MAX_JOBS="4")
         log = os.path.join(HERE, "_ref", "k1_build.log")
         with open(log, "w") as f:
             rc = subprocess.call([sys.executable, "setup.py", "build_ext", "--inplace"], cwd=CUDA_OP, env=env, stdout=f, stderr=subprocess.STDOUT)

@@ -1,6 +1,6 @@
-"""Timing of the INCUMBENT: the unmodified reference (oracle/_ref) on the same B200 -- cuDNN fp32 / TF32 convolutions, ATen
+"""Timing of the INCUMBENT: the unmodified reference (oracle/_ref) on the same GPU -- cuDNN fp32 / TF32 convolutions, ATen
 pointwise kernels, the Python NMS loop and its own K1 extension (SURVEY.md 8(d): "also report the reference GPU path on the same
-B200 since that is the real incumbent").  TEST / BENCH INFRASTRUCTURE: only bench.py's `reference_gpu` leg and tools/ call this.
+H100 since that is the real incumbent").  TEST / BENCH INFRASTRUCTURE: only bench.py's `reference_gpu` leg and tools/ call this.
 
 Method = the reference's own benchmark() (run_rpn.py:594-617): eval mode, warm-up forwards, then `reps` forwards of
 `model([grid])` each bracketed by CUDA events + synchronize, mean / std in ms.  The reference uses 10 + 300 repetitions on a

@@ -4,7 +4,7 @@ Only tests/, __graft_entry__.smoke() and bench.py's reference/incumbent legs may
 (nerf_rpn_b200/) never does.
 
 `load()` imports the reference's own modules (`model.*`, `eval`, `datasets`) from the staged copy with its real native op
-`sort_vertices` (K1, built by its own setup.py for sm_100) when a GPU is present, and returns them in a namespace.  The
+`sort_vertices` (K1, built by its own setup.py for sm_90) when a GPU is present, and returns them in a namespace.  The
 reference imports by bare module name (`from model.utils import ...`, run_rpn.py:14-22), so the staged directory is put on
 sys.path for the duration of the import and the bare names are removed from sys.modules afterwards: the loaded classes keep
 working (they hold their module objects) and nothing leaks into later imports (e.g. dropin/model.py in the same process).

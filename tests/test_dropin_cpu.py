@@ -1,6 +1,6 @@
 """CPU: the drop-in shims make the reference's UNMODIFIED driver resolve `model.*` to this package and construct its model
-through our module mirror with the reference's own constructor calls (run_rpn.py:171-216, 274-292). Skipped on boxes without
-/root/reference (the GPU box)."""
+through our module mirror with the reference's own constructor calls (run_rpn.py:171-216, 274-292).  The reference is the copy that
+__graft_entry__.build() stages under oracle/_ref; skipped where it has not been staged."""
 import os
 import subprocess
 import sys
@@ -9,10 +9,10 @@ import textwrap
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference/nerf_rpn"
+REF = os.path.join(ROOT, "oracle", "_ref", "nerf_rpn")
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present")
+@pytest.mark.skipif(not os.path.isdir(REF), reason="oracle/_ref not staged")
 @pytest.mark.parametrize("backbone", ["resnet", "vgg_EF", "swin_s"])
 def test_reference_driver_builds_our_modules(backbone, tmp_path):
     code = textwrap.dedent(f"""
@@ -42,7 +42,7 @@ def test_reference_driver_builds_our_modules(backbone, tmp_path):
     assert "OK" in r.stdout
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present")
+@pytest.mark.skipif(not os.path.isdir(REF), reason="oracle/_ref not staged")
 def test_reference_fcos_driver_builds_our_modules(tmp_path):
     code = textwrap.dedent(f"""
         import sys, types

@@ -193,7 +193,7 @@ def test_config1_vgg19_fpn_small_grid(golden_dir, precision):
 
 @pytest.mark.parametrize("name,rot", [("rpn_small_aabb", False), ("rpn_small_obb", True)])
 def test_fp16_activation_mode_reaches_the_north_star_tolerance(golden_dir, name, rot):
-    """precision='fp16' (IEEE half activations / weights, same tcgen05 rate, fp32 accumulation): feature maps against the
+    """precision='fp16' (IEEE half activations / weights, same tensor-core rate, fp32 accumulation): feature maps against the
     reference's fp32 golden. bf16 storage cannot get below ~7e-3 (8-bit significand); fp16 is expected around 1e-3."""
     g = np.load(os.path.join(golden_dir, name + ".npz"))
     model, ag = build(rot, g)

@@ -1,5 +1,5 @@
 """GPU: the CUDA path against the UNMODIFIED reference RUN ON THE SAME GPU (oracle/_ref, staged by oracle/build_ref.py):
-its real native op K1 (`sort_vertices`, built by its own setup.py for sm_100), its torch-CUDA IoU chain and Python NMS loop, its
+its real native op K1 (`sort_vertices`, built by its own setup.py for sm_90), its torch-CUDA IoU chain and Python NMS loop, its
 fp32 cuDNN network, and its unmodified driver run_rpn.py launched on top of the drop-in shims.
 
 Skipped (with the reason) when oracle/_ref is not staged -- it is created by __graft_entry__.build() in the build container and
@@ -56,7 +56,7 @@ def test_sort_vertices_bit_identical_to_reference_kernel():
     v = (v - v.mean(dim=2, keepdim=True)).contiguous()
     m = torch.rand(8, 1024, 24, generator=g2) > 0.8
     # a polygon with more than 8 valid vertices makes the reference write PAST its 9 output slots into the next polygon's first slot
-    # (:103-106: observed on the B200 as 3 % of rows with a foreign first index): keep every polygon at <= 8 so the comparison is defined
+    # (:103-106: observed on the GPU as 3 % of rows with a foreign first index): keep every polygon at <= 8 so the comparison is defined
     over = m.int().sum(-1) > 8
     m[over] = False
     m = m.cuda()
@@ -289,7 +289,7 @@ def _run_driver(via, args, tmp, timeout=1500):
 
 def test_unmodified_run_rpn_eval_through_dropin_matches_reference_run(tmp_path):
     """`run_rpn.py --mode eval` (the reference's file, byte for byte) over 4 scenes with planted OBBs: once on the reference's own
-    modules (cuDNN + Python NMS + K1) and once through dropin/run.py on the B200 engine, same checkpoint.  Both must finish and write
+    modules (cuDNN + Python NMS + K1) and once through dropin/run.py on this package's engine, same checkpoint.  Both must finish and write
     eval.json; recall@0.25 from the two runs within 0.5 pt... on 48 boxes that is a zero-box difference at top-2500, one box elsewhere."""
     tmp = str(tmp_path)
     csv = _write_scenes(tmp, 4, (64, 96, 80))
@@ -313,7 +313,7 @@ def test_unmodified_run_rpn_eval_through_dropin_matches_reference_run(tmp_path):
 
 def test_unmodified_run_rpn_benchmark_through_dropin(tmp_path):
     """`run_rpn.py --mode benchmark` (run_rpn.py:594-617: randn(4,200,200,130), 10 warm-up + 300 timed forwards, CUDA events) runs
-    unchanged on the B200 engine and prints its own timing line."""
+    unchanged on this package's engine and prints its own timing line."""
     r, dt = _run_driver("b200", ["--mode", "benchmark", "--dataset_name", "general", "--backbone_type", "resnet"], str(tmp_path))
     assert r.returncode == 0, r.stderr[-3000:]
     line = [l for l in r.stdout.splitlines() if "Average inference time" in l]

@@ -304,7 +304,7 @@ def test_training_step_full_size_config4_vs_reference_autograd():
 def _training_step_parity(layers, rotated, precision, dims, n_gt):
     """One training step at 64x96x80 with 12 planted boxes against the UNMODIFIED reference (oracle/_ref: its modules in train mode, its own
     compute_loss, torch autograd, clip_grad_norm_, torch.optim.AdamW) on this GPU, same seed-0 weights, same sampled anchors.
-    What "parity" can mean here was MEASURED (tools/debug_train.py, profiles/r02_debug_train.log): with BatchNorm on batch statistics and the
+    What "parity" can mean here was MEASURED (tools/debug_train.py): with BatchNorm on batch statistics and the
     reference's init, this network is so ill-conditioned that the reference ITSELF under torch.autocast lands 9-14 % (fp16) / 41-58 % (bf16)
     away from its fp32 feature maps and at gradient cosine 0.63 / 0.11 -- 16-bit rounding, amplified by ~55 normalisations.  The engine is
     therefore held to the mixed-precision reference: every error metric against fp32 must be no worse than the reference's own autocast run

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Target for `ncu --nvtx --nvtx-include "target/"`: one full-size scene (eager), then the kernels we want captured,
-each inside the NVTX range "target": the RPN-head conv layer (tcgen05 implicit GEMM over P2..P5), the stem conv,
+each inside the NVTX range "target": the RPN-head conv layer (wgmma implicit GEMM over P2..P5), the stem conv,
 pack_stem_input, maxpool and the whole post-processing (top-k, decode, NMS)."""
 import os
 import sys

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""BASELINE config 5: oriented 3-D IoU + NMS throughput sweep, 1k .. 1M proposals per scene, 1 x B200.
+"""BASELINE config 5: oriented 3-D IoU + NMS throughput sweep, 1k .. 1M proposals per scene, 1 x H100.
 Inputs per SURVEY.md 8(d): centres U[0,256)^3*(1,1,0.625), sizes U[4,48], theta U[-pi/2,pi/2), scores U[0,1), seed 0,
 threshold 0.3, 1 and 4 level groups; cull mode 0 (exact-zero culls only: provably the reference's keep set) and 3 (+ geometric ratio culls).  Algorithmic bytes: 32 B per input box + 8 B per kept index."""
 import json

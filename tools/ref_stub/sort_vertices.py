@@ -24,7 +24,7 @@ def _cmp(x1, y1, x2, y2):
     decided |= c
     with np.errstate(all="ignore"):
         # nvcc contracts `x1*x1 + y1*y1` (sort_vert_kernel.cu:25) into fma(x1, x1, y1*y1): SASS of the reference's own build, and
-        # bit-for-bit agreement with that binary on the B200 (tests/test_gpu_reference.py)
+        # bit-for-bit agreement with that binary on the GPU (tests/test_gpu_reference.py)
         n1 = ((x1.astype(np.float64) * x1 + (y1 * y1).astype(np.float64)).astype(np.float32).astype(np.float64) + EPS).astype(np.float32)
         n2 = ((x2.astype(np.float64) * x2 + (y2 * y2).astype(np.float64)).astype(np.float32).astype(np.float64) + EPS).astype(np.float32)
         d = (np.abs(x1) * x1 / n1 - np.abs(x2) * x2 / n2).astype(np.float32).astype(np.float64)
