@@ -245,7 +245,8 @@ int nrpn_layernorm(const void *in, int ld_in, void *out, int ld_out, long tokens
 int nrpn_patch_merge_ln(const void *in, int ld_in, int n, int h, int w, int d, int c, void *out, const float *gamma,
                         const float *beta, float eps, int act_fp16, nrpn_stream_t stream);
 /* 4x4x4 (shifted) window multi-head attention, head_dim 32: qkv (N,h,w,d, 3c) -> out (N,h,w,d, ld_out). shift in {0, 2};
- * table = (343, heads) relative position bias table; qkv_bias (3c) stands in for zero-padded tokens. */
+ * table = (343, heads) relative position bias table; qkv_bias (3c) stands in for zero-padded tokens.
+ * qkv and out are 16-byte aligned and ld_qkv, ld_out are multiples of 8 (rows of whole 16-byte chunks); NRPN_ERR_INVALID otherwise. */
 int nrpn_window_attention(const void *qkv, int ld_qkv, void *out, int ld_out, const float *qkv_bias, const float *table, int n,
                           int h, int w, int d, int c, int heads, int shift, int act_fp16, nrpn_stream_t stream);
 
@@ -306,16 +307,13 @@ int nrpn_assign_targets(const float *anchors, int n_anchors, const float *gt, in
 
 /* ------------------------------------------------------------------------------------------------ weight gradient
  * dW[tap][co][ci] = sum_v dY[v][co] * X[v + tap_off][ci] of a stride-1 convolution (training, SURVEY.md 8(a) a18) on wgmma.
- * operand_layout 1 (what the training engine uses): both operands are read channels-last where they live (MN-major wgmma operands).
- * operand_layout 0: both operands in PLANAR layout (N, C, X, Y, z_pitch), 16-bit (nrpn_transpose_to_planar converts a channels-last tensor);
- * levels that share the weights (RPN head on P2..P5) accumulate into the same dW.  dw: fp32 (taps, cout, cin), overwritten.
- * cout % 128 == 0; cin % 32 == 0, cin <= 256; tap z offsets in {-1, 0, +1}.  Deterministic (fixed-order reduction of the K-split partial tiles). */
+ * Both operands are read channels-last where they live (MN-major wgmma operands); levels that share the weights (RPN head on
+ * P2..P5) accumulate into the same dW.  dw: fp32 in dw_layout's order, overwritten unless accumulate is set.
+ * cout % 8 == 0; cin % 32 == 0 with cin <= 256, or cin % 256 == 0; ld_dy / ld_x multiples of 8; any tap offsets.
+ * Deterministic (fixed-order reduction of the K-split partial tiles). */
 typedef struct {
-    const void *dy_planar;   /* (N, cout, X, Y, z_pitch) bf16 / fp16 */
-    const void *x_planar[3]; /* (N, cin,  X, Y, z_pitch): copies shifted along z, [k][z] = x[z + (k - 1)], zero outside; NULL if no tap has dz = k - 1 */
     int32_t n, x, y, z;
-    int32_t z_pitch;         /* >= z + 1, multiple of 8; positions without a source MUST be zero (pre-zeroed buffers) */
-    /* operand_layout == 1: the operands where they live, channels-last 16-bit (N, X, Y, Z, ld); no copies, no staging buffers */
+    /* the operands where they live, channels-last 16-bit (N, X, Y, Z, ld); no copies, no staging buffers */
     const void *dy_cl;       /* (N, x, y, z, ld_dy >= cout) */
     const void *x_cl;        /* (N, xx, xy, xz, ld_x >= cin): the layer input, same grid as dY unless xx / xy / xz say otherwise */
     int32_t ld_dy, ld_x;     /* row pitches in elements, multiples of 8 */
@@ -333,15 +331,10 @@ typedef struct {
     int32_t act_fp16;
     int32_t dw_layout;       /* 0: dw is (taps, Cout, Cin); 1: dw is (Cout, Cin, taps) = nn.Conv3d.weight's own memory order */
     int32_t accumulate;      /* 1: dw += result (a weight shared by several launches) */
-    int32_t operand_layout;  /* 0: planar copies (dy_planar / x_planar); 1: channels-last tensors (dy_cl / x_cl) read through MN-major descriptors */
 } nrpn_wgrad_desc;
 
 size_t nrpn_conv3d_wgrad_workspace_bytes(const nrpn_wgrad_desc *desc /*host*/);
 int nrpn_conv3d_wgrad(const nrpn_wgrad_desc *desc /*host*/, nrpn_stream_t stream);
-/* channels-last (N, X, Y, Z, ld >= c) 16-bit -> planar (N, c, X, Y, z_pitch >= Z); columns [Z, z_pitch) are left untouched
- * (pre-zero the buffer once) */
-int nrpn_transpose_to_planar(const void *in_cl, int n, int x, int y, int z, int c, int ld, void *out_planar, int z_pitch,
-                             int z_shift /* out[z'] = in[z' + z_shift] */, nrpn_stream_t stream);
 
 /* Pointwise pieces of a conv + bias + ReLU layer's backward pass (training building blocks):
  * db[c] = sum over rows of dY[row][c] (fixed-order two-stage reduction, bit-reproducible); dY *= (act > 0) in place. */

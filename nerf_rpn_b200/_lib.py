@@ -46,8 +46,7 @@ class RpnDesc(ctypes.Structure):
 
 
 class WgradLevel(ctypes.Structure):
-    _fields_ = [("dy_planar", ctypes.c_void_p), ("x_planar", ctypes.c_void_p * 3), ("n", ctypes.c_int32), ("x", ctypes.c_int32),
-                ("y", ctypes.c_int32), ("z", ctypes.c_int32), ("z_pitch", ctypes.c_int32),
+    _fields_ = [("n", ctypes.c_int32), ("x", ctypes.c_int32), ("y", ctypes.c_int32), ("z", ctypes.c_int32),
                 ("dy_cl", ctypes.c_void_p), ("x_cl", ctypes.c_void_p), ("ld_dy", ctypes.c_int32), ("ld_x", ctypes.c_int32),
                 ("xx", ctypes.c_int32), ("xy", ctypes.c_int32), ("xz", ctypes.c_int32)]
 
@@ -56,7 +55,7 @@ class WgradDesc(ctypes.Structure):
     _fields_ = [("cin", ctypes.c_int32), ("cout", ctypes.c_int32), ("n_taps", ctypes.c_int32),
                 ("tap_off", (ctypes.c_int8 * 3) * MAX_TAPS), ("n_levels", ctypes.c_int32), ("level", WgradLevel * MAX_LEVELS),
                 ("dw", ctypes.c_void_p), ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_size_t),
-                ("act_fp16", ctypes.c_int32), ("dw_layout", ctypes.c_int32), ("accumulate", ctypes.c_int32), ("operand_layout", ctypes.c_int32)]
+                ("act_fp16", ctypes.c_int32), ("dw_layout", ctypes.c_int32), ("accumulate", ctypes.c_int32)]
 
 
 class GnLevel(ctypes.Structure):
@@ -115,8 +114,6 @@ _SIGNATURES = {
     "nrpn_conv3d_fprop": (ctypes.c_int, [ctypes.POINTER(ConvDesc), c_stream]),
     "nrpn_conv3d_wgrad_workspace_bytes": (ctypes.c_size_t, [ctypes.POINTER(WgradDesc)]),
     "nrpn_conv3d_wgrad": (ctypes.c_int, [ctypes.POINTER(WgradDesc), c_stream]),
-    "nrpn_transpose_to_planar": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                                ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, c_stream]),
     "nrpn_bias_grad_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int]),
     "nrpn_bias_grad": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_long, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, ctypes.c_void_p,
                                       ctypes.c_size_t, c_stream]),

@@ -1,18 +1,16 @@
 // Weight gradient of a stride-1 'same' 3-D convolution on wgmma (training, SURVEY.md 8(a) a18):
 //     dW[tap][co][ci] = sum over voxels v   dY[v][co] * X[v + tap_offset][ci]
-// The contraction runs over VOXELS, for which channels-last activations (a voxel's channels are contiguous) are MN-major operands.
-// Two operand paths, selected by nrpn_wgrad_desc.operand_layout:
-//   1 (what the training engine uses, conv3d_wgrad_cl_kernel below): both tensors are read where they live through MN-major shared-memory
-//     descriptors; a tap is a coordinate shift of the X box, TMA's zero fill is the padding; work items share tiles across Cout slices / taps.
-//   0 (round 1, conv3d_wgrad_kernel, kept for A/B runs): the tensors are first transposed to a planar (N, C, X, Y, z_pitch) layout by a bandwidth
-//     kernel so that K-major descriptors can be used: the (y, z) plane is addressed as ONE flattened axis of Y * z_pitch elements, a TMA box
-//     {64 flattened voxels, 1 x, channels, 1} lands as `channels` rows of exactly 128 bytes; TMA needs 16-byte aligned inner coordinates, so a y shift
-//     is the flattened offset dy * z_pitch (z_pitch % 8 == 0) and a z shift of -1 / +1 reads a z-SHIFTED COPY of X^T written by the transpose kernel.
-// In both: D (128 x N_T, fp32 in registers of two warpgroups) += A * B^T with A = dY brick (128 output channels x 64 voxels), B = X brick shifted by the tap (N_T input
-// channels x 64 voxels).  Work item = (tap or tap group, Cout slice(s), Cin slice, K-split); every item streams its share of the voxel bricks of all
-// pyramid levels that share the weights (the RPN head on P2..P5) and writes fp32 partial tiles; a second kernel sums them in a fixed order
+// The contraction runs over VOXELS, for which channels-last activations (a voxel's channels are contiguous) are MN-major operands:
+// both tensors are read where they live, channels-last (N, X, Y, Z, ld), through MN-major shared-memory descriptors.  A TMA box
+// {64 channels, bz, by, bx} of 64 voxels lands in shared memory as 64 rows of 128 bytes (128B swizzle) -- which IS the canonical MN-major
+// operand layout of wgmma (SWIZZLE_128B: 64 channels contiguous per voxel row, 8 rows per 1024-byte swizzle atom, SBO = 1024 bytes between
+// groups of 8 voxels, LBO = the distance between two 64-channel boxes), selected by the instruction's transpose flags.  No transposed copies,
+// no zero-filled staging buffers: the tap offset is a plain coordinate shift of the X box and TMA's out-of-bounds zero fill is the convolution
+// padding.
+// D (128 x NT, fp32 in registers of two warpgroups) += A * B^T with A = dY box pair (128 output channels x 64 voxels), B = X boxes shifted by the tap
+// (n_t input channels x 64 voxels).  Work item = (tap group, Cout slice(s), Cin slice, K-split); every item streams its share of the voxel bricks
+// of all pyramid levels that share the weights (the RPN head on P2..P5) and writes fp32 partial tiles; a second kernel sums them in a fixed order
 // (bit-reproducible) into dW (taps, Cout, Cin) or nn.Conv3d.weight's own (Cout, Cin, taps) order.
-#include <cstdlib>
 #include <cstring>
 #include <type_traits>
 #include "common.cuh"
@@ -21,21 +19,8 @@
 
 namespace nrpn {
 
-constexpr int kWgStages = 4;
-constexpr int kWgABytes = 128 * 128;            // 128 output channels x 64 voxels x 2 B
 constexpr int kWgConsumers = 256;               // two warpgroups: output channels 0-63 / 64-127 of the slice
 constexpr int kWgThreads = kWgConsumers + 32;   // + the TMA producer warp
-
-struct WgLevelDev { int n, X, chunks, zp, brick_begin; };      // chunks = ceil(Y * zp / 64) K-blocks per x-plane
-
-struct WgDev {
-    int n_levels, n_taps, cin, cout, n_t, m_tiles, n_tiles, splits, total_bricks, fp16, dw_layout, accumulate;
-    signed char tap[NRPN_CONV_MAX_TAPS][4];
-    WgLevelDev lv[NRPN_CONV_MAX_LEVELS];
-    float* partial;                            // [tap][m_tile][n_tile][split][128][n_t]
-};
-
-struct WgMaps { CUtensorMap dy[NRPN_CONV_MAX_LEVELS]; CUtensorMap x[NRPN_CONV_MAX_LEVELS][3]; };      // x[level][dz + 1]: z-shifted copies
 
 // Stores the consumer warpgroup's rows of an accumulator (128 x NT, columns >= n_t are padding) as one fp32 partial tile.
 template <int NT>
@@ -49,90 +34,6 @@ __device__ __forceinline__ void store_partial(float* tile, int n_t, int wg, int 
             if (col < n_t)
                 *reinterpret_cast<float2*>(out + col) = empty ? make_float2(0.f, 0.f) : make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
-    }
-}
-
-template <int NT>
-__global__ void __launch_bounds__(kWgThreads, 1) conv3d_wgrad_kernel(const __grid_constant__ WgMaps maps, const WgDev P) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    constexpr int stage_bytes = kWgABytes + NT * 128;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWgStages * stage_bytes);
-    uint64_t* full_bar = bars;
-    uint64_t* empty_bar = bars + kWgStages;
-    const int warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kWgStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 2); }
-        ptx::fence_barrier_init();
-        for (int l = 0; l < P.n_levels; ++l) { ptx::prefetch_tmap(&maps.dy[l]); for (int k = 0; k < 3; ++k) ptx::prefetch_tmap(&maps.x[l][k]); }
-    }
-    __syncthreads();
-    const int items = P.n_taps * P.m_tiles * P.n_tiles * P.splits;
-    const uint32_t load_bytes = (uint32_t)(kWgABytes + P.n_t * 128);
-
-    if (warp == kWgConsumers / 32) {
-        const bool leader = ptx::elect_one();
-        int stage = 0; uint32_t phase = 0;
-        for (int item = blockIdx.x; item < items; item += gridDim.x) {
-            const int split = item % P.splits;
-            const int nt = (item / P.splits) % P.n_tiles;
-            const int mt = (item / (P.splits * P.n_tiles)) % P.m_tiles;
-            const int tap = item / (P.splits * P.n_tiles * P.m_tiles);
-            const int b0 = (int)(((long)P.total_bricks * split) / P.splits), b1 = (int)(((long)P.total_bricks * (split + 1)) / P.splits);
-            const int dx = P.tap[tap][0], dy = P.tap[tap][1], dz = P.tap[tap][2];
-            for (int b = b0; b < b1; ++b) {
-                int l = 0;
-#pragma unroll
-                for (int i = 1; i < NRPN_CONV_MAX_LEVELS; ++i) if (i < P.n_levels && b >= P.lv[i].brick_begin) l = i;
-                const WgLevelDev& L = P.lv[l];
-                int t = b - L.brick_begin;
-                const int ck = t % L.chunks; t /= L.chunks;
-                const int x0 = t % L.X; const int nb = t / L.X;
-                const int f0 = ck * 64;                                      // position on the flattened (y, z-with-pad) axis
-                ptx::mbar_wait(&empty_bar[stage], phase ^ 1u);
-                if (leader) {
-                    uint8_t* sa = smem + stage * stage_bytes;
-                    ptx::mbar_expect_tx(&full_bar[stage], load_bytes);
-                    ptx::tma_load_4d(sa, &maps.dy[l], &full_bar[stage], f0, x0, mt * 128, nb);
-                    ptx::tma_load_4d(sa + kWgABytes, &maps.x[l][dz + 1], &full_bar[stage], f0 + dy * L.zp, x0 + dx, nt * P.n_t, nb);   // z shift lives in the copy
-                }
-                __syncwarp();
-                if (++stage == kWgStages) { stage = 0; phase ^= 1u; }
-            }
-        }
-        return;
-    }
-
-    // consumers: rows = output channels of the slice, columns = input channels
-    const int t = threadIdx.x & 127, wg = threadIdx.x >> 7;
-    int stage = 0; uint32_t phase = 0;
-    float acc[NT / 2];
-    for (int item = blockIdx.x; item < items; item += gridDim.x) {
-        const int split = item % P.splits;
-        const int nt = (item / P.splits) % P.n_tiles;
-        const int mt = (item / (P.splits * P.n_tiles)) % P.m_tiles;
-        const int tap = item / (P.splits * P.n_tiles * P.m_tiles);
-        const int b0 = (int)(((long)P.total_bricks * split) / P.splits), b1 = (int)(((long)P.total_bricks * (split + 1)) / P.splits);
-        ptx::reg_fence(acc);
-        for (int b = b0; b < b1; ++b) {
-            ptx::mbar_wait(&full_bar[stage], phase);
-            const uint32_t sa = ptx::smem_u32(smem + stage * stage_bytes);
-            const uint64_t da = ptx::make_desc_sw128(sa + (uint32_t)(wg * (kWgABytes / 2))), db = ptx::make_desc_sw128(sa + kWgABytes);
-            auto issue = [&](auto f16) {
-                ptx::wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    ptx::Wgmma<NT, decltype(f16)::value>::template ss<0, 0>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), ((b - b0) | k) ? 1u : 0u);
-                ptx::wgmma_commit();
-            };
-            if (P.fp16) issue(std::true_type{}); else issue(std::false_type{});
-            ptx::wgmma_wait<0>();
-            if (t == 0) ptx::mbar_arrive(&empty_bar[stage]);
-            if (++stage == kWgStages) { stage = 0; phase ^= 1u; }
-        }
-        ptx::reg_fence(acc);
-        float* tile = P.partial + ((((size_t)tap * P.m_tiles + mt) * P.n_tiles + nt) * P.splits + split) * 128 * P.n_t;
-        store_partial<NT>(tile, P.n_t, wg, t, acc, b1 <= b0);         // nothing accumulated: zeros
     }
 }
 
@@ -154,23 +55,16 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ partial, int n_tap
     }
 }
 
-// ------------------------------------------------------------------------------------------------ channels-last operands (MN-major wgmma)
-// The same contraction with BOTH operands read where they live: channels-last (N, X, Y, Z, ld) tensors.  A TMA box {64 channels, bz, by, bx} of
-// 64 voxels lands in shared memory as 64 rows of 128 bytes (128B swizzle) -- which IS the canonical MN-major operand layout of wgmma
-// (SWIZZLE_128B: 64 channels contiguous per voxel row, 8 rows per 1024-byte swizzle atom, SBO = 1024 bytes between groups of 8 voxels,
-// LBO = the distance between two 64-channel boxes), selected by the instruction's transpose flags.  No transposed copies, no zero-filled
-// staging buffers: the tap offset is a plain coordinate shift of the X box and TMA's out-of-bounds zero fill is the convolution padding.
-//   A = dY box pair  (128 output channels  x 64 voxels),  B = X boxes (n_t input channels x 64 voxels, shifted by the tap)
-struct WgLevelCl { int n, nxb, nyb, nzb, bx, by, bz, brick_begin; };
-struct WgDevCl {
+struct WgLevel { int n, nxb, nyb, nzb, bx, by, bz, brick_begin; };
+struct WgDev {
     int n_levels, n_taps, cin, cout, n_t, m_tiles, n_tiles, splits, total_bricks, fp16, b_boxes;
     int m_pair, m_items, stages;           // Cout slices per work item (1 or 2: two accumulators share one X tile), items along Cout, ring depth
     int t_group, n_groups;                 // taps per work item (their accumulators share one dY tile), tap groups
     signed char tap[NRPN_CONV_MAX_TAPS][4];
-    WgLevelCl lv[NRPN_CONV_MAX_LEVELS];
-    float* partial;
+    WgLevel lv[NRPN_CONV_MAX_LEVELS];
+    float* partial;                        // [tap][m_tile][n_tile][split][128][n_t]
 };
-struct WgMapsCl { CUtensorMap dy[NRPN_CONV_MAX_LEVELS]; CUtensorMap x[NRPN_CONV_MAX_LEVELS]; };
+struct WgMaps { CUtensorMap dy[NRPN_CONV_MAX_LEVELS]; CUtensorMap x[NRPN_CONV_MAX_LEVELS]; };
 constexpr int kWgBox = 64 * 128;               // one {64 channels x 64 voxels} box, 16-bit
 constexpr int kWgMaxStages = 4;
 constexpr int kWgAccRegs = 128;                // accumulator registers per consumer thread: m_pair * t_group * NT / 2 <= this
@@ -179,7 +73,7 @@ constexpr int kWgAccRegs = 128;                // accumulator registers per cons
 // (accumulator m * t_group + i = Cout slice m of the pair x tap i of the group).  With Cout >= 256 two 128-channel slices of Cout share the
 // same X tile and a tap group shares one dY tile: the kernel is bound by the shared-memory fill rate out of L2, and sharing cuts it.
 template <int NT, int NACC>
-__global__ void __launch_bounds__(kWgThreads, 1) conv3d_wgrad_cl_kernel(const __grid_constant__ WgMapsCl maps, const WgDevCl P) {
+__global__ void __launch_bounds__(kWgThreads, 1) conv3d_wgrad_cl_kernel(const __grid_constant__ WgMaps maps, const WgDev P) {
     static_assert(NT * NACC / 2 <= kWgAccRegs, "accumulator registers");
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -212,7 +106,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) conv3d_wgrad_cl_kernel(const __
                 int l = 0;
 #pragma unroll
                 for (int i = 1; i < NRPN_CONV_MAX_LEVELS; ++i) if (i < P.n_levels && b >= P.lv[i].brick_begin) l = i;
-                const WgLevelCl& L = P.lv[l];
+                const WgLevel& L = P.lv[l];
                 int t = b - L.brick_begin;
                 const int zb = t % L.nzb; t /= L.nzb;
                 const int yb = t % L.nyb; t /= L.nyb;
@@ -287,33 +181,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) conv3d_wgrad_cl_kernel(const __
     }
 }
 
-// channels-last (N, X*Y*Z, ld) -> planar (N, C, X*Y, Zp) with Zp = z pitch >= Z (a multiple of 8 so that every TMA stride is a
-// multiple of 16 bytes; the pad is never read: the tensor maps carry the logical Z), 16-bit elements, 64 x 64 tiles through smem
-__global__ void __launch_bounds__(256) cl_to_planar_kernel(const uint16_t* __restrict__ in, int ld, int C, long V, int Z, int Zp,
-                                                           int z_shift, uint16_t* __restrict__ out) {
-    __shared__ uint16_t tile[64][66];
-    const long v0 = (long)blockIdx.x * 64;
-    const int c0 = blockIdx.y * 64, nb = blockIdx.z;
-    const uint16_t* src = in + (size_t)nb * V * ld;
-    const size_t plane = (size_t)(V / Z) * Zp;
-    uint16_t* dst = out + (size_t)nb * C * plane;
-    for (int i = threadIdx.x; i < 64 * 64; i += 256) {
-        const int v = i >> 6, c = i & 63;
-        tile[v][c] = (v0 + v < V && c0 + c < C) ? src[(size_t)(v0 + v) * ld + c0 + c] : (uint16_t)0;
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < 64 * 64; i += 256) {
-        const int c = i >> 6, v = i & 63;
-        if (v0 + v < V && c0 + c < C) {
-            const long vv = v0 + v;
-            const int zo = (int)(vv % Z) - z_shift;          // out[z'] = in[z' + z_shift]: a z-shifted copy keeps TMA coordinates 16-byte aligned
-            if (zo >= 0 && zo < Zp) dst[(size_t)(c0 + c) * plane + (size_t)(vv / Z) * Zp + zo] = tile[v][c];
-        }
-    }
-}
-
 template <int NT, int NACC>
-int launch_wgrad_cl(const WgMapsCl& maps, const WgDevCl& P, int grid, int smem, cudaStream_t st) {
+int launch_wgrad(const WgMaps& maps, const WgDev& P, int grid, int smem, cudaStream_t st) {
     static int smem_set = 0;
     if (smem > smem_set) {
         NRPN_CUDA_TRY(cudaFuncSetAttribute(conv3d_wgrad_cl_kernel<NT, NACC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -324,68 +193,12 @@ int launch_wgrad_cl(const WgMapsCl& maps, const WgDevCl& P, int grid, int smem, 
     return NRPN_OK;
 }
 
-template <int NT>
-int launch_wgrad_planar(const WgMaps& maps, const WgDev& P, int grid, cudaStream_t st) {
-    constexpr int smem = kWgStages * (kWgABytes + NT * 128) + 1024 + 256;
-    static bool attr_set = false;
-    if (!attr_set) {
-        NRPN_CUDA_TRY(cudaFuncSetAttribute(conv3d_wgrad_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        attr_set = true;
-    }
-    conv3d_wgrad_kernel<NT><<<grid, kWgThreads, smem, st>>>(maps, P);
-    NRPN_LAUNCH_CHECK();
-    return NRPN_OK;
-}
-
 }  // namespace nrpn
 
 using namespace nrpn;
 
 extern "C" {
 #pragma GCC visibility push(default)
-
-int nrpn_transpose_to_planar(const void* in_cl, int n, int x, int y, int z, int c, int ld, void* out_planar, int z_pitch, int z_shift,
-                             nrpn_stream_t stream) {
-    if (!in_cl || !out_planar || n < 1 || x < 1 || y < 1 || z < 1 || c < 1 || ld < c || z_pitch < z) return NRPN_ERR_INVALID;
-    const long voxels = (long)x * y * z;
-    dim3 grid((unsigned)ceil_div(voxels, 64L), (unsigned)ceil_div(c, 64), (unsigned)n);
-    if (grid.y > 65535 || grid.z > 65535) return NRPN_ERR_UNSUPPORTED;
-    cl_to_planar_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const uint16_t*>(in_cl), ld, c, voxels, z, z_pitch, z_shift,
-                                                               reinterpret_cast<uint16_t*>(out_planar));
-    NRPN_LAUNCH_CHECK();
-    return NRPN_OK;
-}
-
-static int wgrad_plan(const nrpn_wgrad_desc* d, WgDev& P) {
-    if (!d || d->n_levels < 1 || d->n_levels > NRPN_CONV_MAX_LEVELS || d->n_taps < 1 || d->n_taps > NRPN_CONV_MAX_TAPS) return NRPN_ERR_INVALID;
-    // Cout: any multiple of 8 (a last slice narrower than 128 rows is zero-filled by TMA: the box exceeds the tensor's channel
-    // extent); Cin: a multiple of 32 up to 256, or a multiple of 256 (N tiles of 256 input channels)
-    if (d->cout < 8 || d->cout % 8 != 0 || d->cin < 32 || d->cin % 32 != 0 || (d->cin > 256 && d->cin % 256 != 0)) return NRPN_ERR_UNSUPPORTED;
-    memset(&P, 0, sizeof(P));
-    P.n_levels = d->n_levels; P.n_taps = d->n_taps; P.cin = d->cin; P.cout = d->cout;
-    P.n_t = d->cin > 256 ? 256 : d->cin; P.n_tiles = d->cin / P.n_t; P.m_tiles = ceil_div(d->cout, 128);
-    P.fp16 = d->act_fp16 ? 1 : 0; P.dw_layout = d->dw_layout ? 1 : 0; P.accumulate = d->accumulate ? 1 : 0;
-    for (int t = 0; t < d->n_taps; ++t) { P.tap[t][0] = d->tap_off[t][0]; P.tap[t][1] = d->tap_off[t][1]; P.tap[t][2] = d->tap_off[t][2]; P.tap[t][3] = 0; }
-    int max_dz = 1;
-    for (int t = 0; t < d->n_taps; ++t) { const int a = d->tap_off[t][2] < 0 ? -d->tap_off[t][2] : d->tap_off[t][2]; if (a > max_dz) max_dz = a; }
-    if (max_dz > 1) return NRPN_ERR_UNSUPPORTED;                       // z-shifted operand copies exist for dz in {-1, 0, +1}
-    int bricks = 0;
-    for (int l = 0; l < d->n_levels; ++l) {
-        const nrpn_wgrad_level& S = d->level[l];
-        if (S.n < 1 || S.x < 1 || S.y < 1 || S.z < 1 || S.z_pitch < S.z + max_dz || S.z_pitch % 8 != 0) return NRPN_ERR_INVALID;   // zero pad columns >= the largest z offset
-        WgLevelDev& L = P.lv[l];
-        L.n = S.n; L.X = S.x; L.zp = S.z_pitch; L.chunks = ceil_div(S.y * S.z_pitch, 64);
-        L.brick_begin = bricks;
-        bricks += S.n * S.x * L.chunks;
-    }
-    P.total_bricks = bricks;
-    const int base = d->n_taps * P.m_tiles * P.n_tiles;
-    int splits = num_sms() / base;                      // one wave of work items: (taps x Cout slices x splits) <= SMs
-    if (splits > bricks) splits = bricks;
-    if (splits < 1) splits = 1;
-    P.splits = splits;
-    return NRPN_OK;
-}
 
 // K-splits of a wgrad launch: the work items (taps x Cout slices x Cin slices x splits) run on a persistent grid of one CTA per SM, so the split count
 // is chosen for the fullest last wave (3^3 256->256 on 132 SMs: 54 base items; 2 splits = 108 items fill 82 % of one wave, 7 splits = 378 items
@@ -404,7 +217,6 @@ static int wgrad_pick_splits(int base, int bricks) {
     return best;
 }
 
-// ---- channels-last operands (desc->operand_layout == 1)
 static int pick_box(int extent, int cap) {           // power of two in [1, cap] with the least overhang over `extent`, the larger one on ties
     int best = 1; long waste = -1;
     for (int b = 1; b <= cap; b <<= 1) {
@@ -414,22 +226,20 @@ static int pick_box(int extent, int cap) {           // power of two in [1, cap]
     return best;
 }
 
-static int wgrad_plan_cl(const nrpn_wgrad_desc* d, WgDevCl& P) {
+static int wgrad_plan(const nrpn_wgrad_desc* d, WgDev& P) {
     if (!d || d->n_levels < 1 || d->n_levels > NRPN_CONV_MAX_LEVELS || d->n_taps < 1 || d->n_taps > NRPN_CONV_MAX_TAPS) return NRPN_ERR_INVALID;
     if (d->cout < 8 || d->cout % 8 != 0 || d->cin < 32 || d->cin % 32 != 0 || (d->cin > 256 && d->cin % 256 != 0)) return NRPN_ERR_UNSUPPORTED;
     memset(&P, 0, sizeof(P));
     P.n_levels = d->n_levels; P.n_taps = d->n_taps; P.cin = d->cin; P.cout = d->cout;
     P.n_t = d->cin > 256 ? 256 : d->cin; P.n_tiles = d->cin / P.n_t; P.m_tiles = ceil_div(d->cout, 128);
     P.b_boxes = ceil_div(P.n_t, 64);
-    static const bool pair_off = [] { const char* e = getenv("NRPN_WGRAD_MPAIR"); return e && e[0] == '0'; }();
-    P.m_pair = (P.m_tiles >= 2 && !pair_off && 2 * P.b_boxes * 64 / 2 <= kWgAccRegs) ? 2 : 1;
+    P.m_pair = (P.m_tiles >= 2 && 2 * P.b_boxes * 64 / 2 <= kWgAccRegs) ? 2 : 1;
     P.m_items = ceil_div(P.m_tiles, P.m_pair);
     {
         // taps per work item: their accumulators share one dY tile (the fill rate out of L2 bounds this kernel: 24 KB per four MMAs at N = 64 with one
         // tap, 12 KB with four); as many as the accumulator registers (kWgAccRegs per thread) and a ring of >= 3 stages allow, at most 4
-        static const bool group_off = [] { const char* e = getenv("NRPN_WGRAD_TAPGROUP"); return e && e[0] == '0'; }();
         P.t_group = 1;
-        for (int t = 2; t <= 4 && !group_off; t <<= 1) {
+        for (int t = 2; t <= 4; t <<= 1) {
             if (t > d->n_taps || P.m_pair * t * P.b_boxes * 64 / 2 > kWgAccRegs) break;
             if ((227 * 1024 - 2048) / ((2 * P.m_pair + t * P.b_boxes) * kWgBox) < 3) break;
             P.t_group = t;
@@ -447,7 +257,7 @@ static int wgrad_plan_cl(const nrpn_wgrad_desc* d, WgDevCl& P) {
         const nrpn_wgrad_level& S = d->level[l];
         if (S.n < 1 || S.x < 1 || S.y < 1 || S.z < 1 || !S.dy_cl || !S.x_cl || S.ld_dy < d->cout || S.ld_x < d->cin || S.ld_dy % 8 != 0 || S.ld_x % 8 != 0)
             return NRPN_ERR_INVALID;
-        WgLevelCl& L = P.lv[l];
+        WgLevel& L = P.lv[l];
         L.n = S.n;
         L.bz = pick_box(S.z, 64); L.by = pick_box(S.y, 64 / L.bz); L.bx = 64 / (L.bz * L.by);
         L.nzb = ceil_div(S.z, L.bz); L.nyb = ceil_div(S.y, L.by); L.nxb = ceil_div(S.x, L.bx);
@@ -460,16 +270,16 @@ static int wgrad_plan_cl(const nrpn_wgrad_desc* d, WgDevCl& P) {
     return NRPN_OK;
 }
 
-static int wgrad_run_cl(const nrpn_wgrad_desc* d, cudaStream_t st) {
-    WgDevCl P;
-    { const int rc = wgrad_plan_cl(d, P); if (rc) return rc; }
+static int wgrad_run(const nrpn_wgrad_desc* d, cudaStream_t st) {
+    WgDev P;
+    { const int rc = wgrad_plan(d, P); if (rc) return rc; }
     EncodeTiledFn encode = get_encode();
     if (!encode) return NRPN_ERR_NO_DEVICE;
-    WgMapsCl maps;
+    WgMaps maps;
     const CUtensorMapDataType dt = d->act_fp16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     for (int l = 0; l < d->n_levels; ++l) {
         const nrpn_wgrad_level& S = d->level[l];
-        const WgLevelCl& L = P.lv[l];
+        const WgLevel& L = P.lv[l];
         cuuint32_t one[5] = {1, 1, 1, 1, 1};
         cuuint32_t box[5] = {64, (cuuint32_t)L.bz, (cuuint32_t)L.by, (cuuint32_t)L.bx, 1};
         // dY: (cout, Z, Y, X, N) with the extents of the OUTPUT grid; X: the input grid (its own extents when they differ)
@@ -499,11 +309,11 @@ static int wgrad_run_cl(const nrpn_wgrad_desc* d, cudaStream_t st) {
     const int nacc = P.m_pair * P.t_group;
     int rc;
     switch (P.b_boxes) {
-        case 1: rc = nacc == 1 ? launch_wgrad_cl<64, 1>(maps, P, grid, smem, st) : nacc == 2 ? launch_wgrad_cl<64, 2>(maps, P, grid, smem, st)
-                                                                                          : launch_wgrad_cl<64, 4>(maps, P, grid, smem, st); break;
-        case 2: rc = nacc == 1 ? launch_wgrad_cl<128, 1>(maps, P, grid, smem, st) : launch_wgrad_cl<128, 2>(maps, P, grid, smem, st); break;
-        case 3: rc = launch_wgrad_cl<192, 1>(maps, P, grid, smem, st); break;
-        default: rc = launch_wgrad_cl<256, 1>(maps, P, grid, smem, st); break;
+        case 1: rc = nacc == 1 ? launch_wgrad<64, 1>(maps, P, grid, smem, st) : nacc == 2 ? launch_wgrad<64, 2>(maps, P, grid, smem, st)
+                                                                                          : launch_wgrad<64, 4>(maps, P, grid, smem, st); break;
+        case 2: rc = nacc == 1 ? launch_wgrad<128, 1>(maps, P, grid, smem, st) : launch_wgrad<128, 2>(maps, P, grid, smem, st); break;
+        case 3: rc = launch_wgrad<192, 1>(maps, P, grid, smem, st); break;
+        default: rc = launch_wgrad<256, 1>(maps, P, grid, smem, st); break;
     }
     if (rc) return rc;
     const size_t total = (size_t)P.n_taps * P.cout * P.cin;
@@ -516,71 +326,15 @@ static int wgrad_run_cl(const nrpn_wgrad_desc* d, cudaStream_t st) {
 }
 
 size_t nrpn_conv3d_wgrad_workspace_bytes(const nrpn_wgrad_desc* d) {
-    if (d && d->operand_layout == 1) {
-        WgDevCl P;
-        if (wgrad_plan_cl(d, P) != NRPN_OK) return 0;
-        return (size_t)P.n_taps * P.m_tiles * P.n_tiles * P.splits * 128 * P.n_t * sizeof(float) + 256;
-    }
     WgDev P;
     if (wgrad_plan(d, P) != NRPN_OK) return 0;
     return (size_t)P.n_taps * P.m_tiles * P.n_tiles * P.splits * 128 * P.n_t * sizeof(float) + 256;
 }
 
 int nrpn_conv3d_wgrad(const nrpn_wgrad_desc* d, nrpn_stream_t stream) {
-    if (d && d->operand_layout == 1) {
-        if (!d->dw || !d->workspace || d->workspace_bytes < nrpn_conv3d_wgrad_workspace_bytes(d)) return NRPN_ERR_WORKSPACE;
-        return wgrad_run_cl(d, (cudaStream_t)stream);
-    }
-    WgDev P;
-    { const int rc = wgrad_plan(d, P); if (rc) return rc; }
+    if (!d) return NRPN_ERR_INVALID;
     if (!d->dw || !d->workspace || d->workspace_bytes < nrpn_conv3d_wgrad_workspace_bytes(d)) return NRPN_ERR_WORKSPACE;
-    EncodeTiledFn encode = get_encode();
-    if (!encode) return NRPN_ERR_NO_DEVICE;
-    WgMaps maps;
-    for (int l = 0; l < d->n_levels; ++l) {
-        const nrpn_wgrad_level& S = d->level[l];
-        if (!S.dy_planar) return NRPN_ERR_INVALID;
-        for (int t = 0; t < d->n_taps; ++t) if (!S.x_planar[d->tap_off[t][2] + 1]) return NRPN_ERR_INVALID;
-        const cuuint64_t X = S.x, F = (cuuint64_t)S.y * S.z_pitch;            // flattened (y, z-with-pad) extent
-        cuuint32_t one[4] = {1, 1, 1, 1};
-        {
-            cuuint64_t gdim[4] = {F, X, (cuuint64_t)d->cout, (cuuint64_t)S.n};
-            cuuint64_t gstr[3] = {F * 2, X * F * 2, X * F * 2 * (cuuint64_t)d->cout};
-            cuuint32_t box[4] = {64, 1, 128, 1};
-            CUresult r = encode(&maps.dy[l], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(S.dy_planar), gdim, gstr, box, one,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (r != CUDA_SUCCESS) { g_last_cuda_error = (int)r; return NRPN_ERR_CUDA; }
-        }
-        for (int k = 0; k < 3; ++k) {
-            const void* src = S.x_planar[k] ? S.x_planar[k] : S.dy_planar;        // unused slots get any valid map
-            const cuuint64_t ch = S.x_planar[k] ? (cuuint64_t)d->cin : (cuuint64_t)d->cout;
-            cuuint64_t gdim[4] = {F, X, ch, (cuuint64_t)S.n};
-            cuuint64_t gstr[3] = {F * 2, X * F * 2, X * F * 2 * ch};
-            cuuint32_t box[4] = {64, 1, (cuuint32_t)(S.x_planar[k] ? P.n_t : 128), 1};
-            CUresult r = encode(&maps.x[l][k], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(src), gdim, gstr, box, one,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (r != CUDA_SUCCESS) { g_last_cuda_error = (int)r; return NRPN_ERR_CUDA; }
-        }
-    }
-    for (int l = d->n_levels; l < NRPN_CONV_MAX_LEVELS; ++l) { maps.dy[l] = maps.dy[0]; for (int k = 0; k < 3; ++k) maps.x[l][k] = maps.x[0][k]; }
-    P.partial = reinterpret_cast<float*>(align_up((size_t)d->workspace, 256));
-    const int items = P.n_taps * P.m_tiles * P.n_tiles * P.splits;
-    const int grid = items < num_sms() ? items : num_sms();
-    cudaStream_t st = (cudaStream_t)stream;
-    {
-        const int nt_pad = ceil_div(P.n_t, 64) * 64;       // MMA width: columns past n_t are never stored
-        const int rc = nt_pad == 64 ? launch_wgrad_planar<64>(maps, P, grid, st) : nt_pad == 128 ? launch_wgrad_planar<128>(maps, P, grid, st)
-                     : nt_pad == 192 ? launch_wgrad_planar<192>(maps, P, grid, st) : launch_wgrad_planar<256>(maps, P, grid, st);
-        if (rc) return rc;
-    }
-    const size_t total = (size_t)P.n_taps * P.cout * P.cin;
-    size_t blocks = ceil_div(total, (size_t)256);
-    if (blocks > (size_t)num_sms() * 8) blocks = (size_t)num_sms() * 8;
-    wgrad_reduce_kernel<<<(unsigned)blocks, 256, 0, st>>>(P.partial, P.n_taps, P.m_tiles, P.n_tiles, P.splits, P.n_t, P.cout, P.cin, d->dw, P.dw_layout, P.accumulate);
-    NRPN_LAUNCH_CHECK();
-    return NRPN_OK;
+    return wgrad_run(d, (cudaStream_t)stream);
 }
 
 #pragma GCC visibility pop

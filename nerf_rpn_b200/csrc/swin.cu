@@ -6,7 +6,6 @@
 //   patch_merge_ln        2x2x2 gather (zero pad on odd extents) + LayerNorm(8C)     (:661-685)
 //   window_attention      4^3 shifted-window multi-head attention, head_dim 32        (:382-497)
 // Activations are (N, H, W, D, ld) bf16 with C real channels and ld >= C (ld a multiple of 64; channels [C, ld) stay zero).
-#include <cstdlib>
 #include "common.cuh"
 #include "wgmma.cuh"
 
@@ -97,11 +96,10 @@ __global__ void __launch_bounds__(256) patch_merge_ln_kernel(const __nv_bfloat16
     for (int c = lane; c < C8; c += 32) store_act(y + c, (src(c) - mean) * rstd * gamma[c] + beta[c], fp16);
 }
 
-// ---------------------------------------------------------------------------------------------- window attention
-// One CTA (64 threads) per (window, head); thread t = query token t of the 4x4x4 window.  K and V of the window are staged
-// in shared memory as fp32; scores, softmax and the output row live in registers.  Window w of the zero-padded, cyclically
-// shifted grid: padded coordinate p -> source coordinate (p + shift) mod P; sources past the real extent are padding
-// tokens whose q/k/v equal the qkv bias (the reference pads AFTER norm1, so padded tokens enter the Linear as zeros).
+// ---------------------------------------------------------------------------------------------- window attention on wgmma
+// Window w of the zero-padded, cyclically shifted grid: padded coordinate p -> source coordinate (p + shift) mod P; sources past
+// the real extent are padding tokens whose q/k/v equal the qkv bias (the reference pads AFTER norm1, so padded tokens enter the
+// Linear as zeros).
 struct AttnDev {
     const __nv_bfloat16* qkv; int ld_qkv;      // (N,H,W,D, 3C): [q | k | v], each head-major (head*32 + d)
     __nv_bfloat16* out; int ld_out;            // (N,H,W,D, ld): heads concatenated
@@ -113,72 +111,6 @@ struct AttnDev {
     int fp16;                                  // 16-bit format of qkv / out: 0 bf16, 1 fp16
 };
 
-__global__ void __launch_bounds__(64) window_attention_kernel(AttnDev P) {
-    __shared__ float Ks[64][33];
-    __shared__ float Vs[64][33];
-    __shared__ int region[64];
-    const int head = blockIdx.y;
-    int w = blockIdx.x;
-    const int wd = w % P.nwd; w /= P.nwd;
-    const int ww = w % P.nww; w /= P.nww;
-    const int wh = w % P.nwh; const int b = w / P.nwh;
-    const int t = threadIdx.x;
-    const int ti = t >> 4, tj = (t >> 2) & 3, tk = t & 3;             // token order inside the window: (i*4 + j)*4 + k
-    const int ph = wh * 4 + ti, pw = ww * 4 + tj, pd = wd * 4 + tk;   // position in the padded, shifted grid
-    const int sh_ = (ph + P.sh) % P.PH, sw_ = (pw + P.sw) % P.PW, sd_ = (pd + P.sd) % P.PD;   // source position
-    const bool real = sh_ < P.H && sw_ < P.W && sd_ < P.D;
-    const size_t tok = (((size_t)b * P.H + sh_) * P.W + sw_) * P.D + sd_;
-    const __nv_bfloat16* row = P.qkv + tok * P.ld_qkv;
-    const int hc = head * 32;
-    float q[32];
-    const float scale = 0.17677669529663687f;                          // 32^-0.5
-#pragma unroll
-    for (int d = 0; d < 32; ++d) {
-        const float qv = real ? load_act(row + hc + d, P.fp16) : P.qkv_bias[hc + d];
-        const float kv = real ? load_act(row + P.C + hc + d, P.fp16) : P.qkv_bias[P.C + hc + d];
-        const float vv = real ? load_act(row + 2 * P.C + hc + d, P.fp16) : P.qkv_bias[2 * P.C + hc + d];
-        q[d] = qv * scale; Ks[t][d] = kv; Vs[t][d] = vv;
-    }
-    // shift-mask region of this token (ids as built by the reference: per axis 0 / 1 / 2, an unshifted axis contributes one id)
-    auto reg1 = [](int p, int Pext, int s) { return s == 0 ? 2 : (p < Pext - 4 ? 0 : (p < Pext - s ? 1 : 2)); };
-    const bool shifted = (P.sh + P.sw + P.sd) > 0;
-    region[t] = shifted ? (reg1(ph, P.PH, P.sh) * 9 + reg1(pw, P.PW, P.sw) * 3 + reg1(pd, P.PD, P.sd)) : 0;
-    __syncthreads();
-    const int myreg = region[t];
-    float sc[64];
-    float mx = -INFINITY;
-#pragma unroll
-    for (int j = 0; j < 64; ++j) {
-        float a = 0.f;
-#pragma unroll
-        for (int d = 0; d < 32; ++d) a += q[d] * Ks[j][d];
-        const int ji = j >> 4, jj = (j >> 2) & 3, jk = j & 3;
-        const int idx = (ti - ji + 3) * 49 + (tj - jj + 3) * 7 + (tk - jk + 3);
-        a += P.table[idx * P.heads + head];
-        if (shifted && region[j] != myreg) a += -100.0f;
-        sc[j] = a; mx = fmaxf(mx, a);
-    }
-    float sum = 0.f;
-#pragma unroll
-    for (int j = 0; j < 64; ++j) { sc[j] = __expf(sc[j] - mx); sum += sc[j]; }
-    const float inv = 1.0f / sum;
-    float o[32];
-#pragma unroll
-    for (int d = 0; d < 32; ++d) o[d] = 0.f;
-#pragma unroll
-    for (int j = 0; j < 64; ++j) {
-        const float p = sc[j] * inv;
-#pragma unroll
-        for (int d = 0; d < 32; ++d) o[d] += p * Vs[j][d];
-    }
-    if (real) {
-        __nv_bfloat16* orow = P.out + tok * P.ld_out + hc;
-#pragma unroll
-        for (int d = 0; d < 32; d += 2) *reinterpret_cast<uint32_t*>(orow + d) = pack_act2(o[d], o[d + 1], P.fp16);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------- window attention on wgmma
 // One warpgroup per (64-token window, head): S = Q K^T is an m64n64k32 wgmma into registers; softmax runs on the accumulator
 // fragments (a row's 64 scores are spread over the 4 threads of a quad: scale, relative-position bias, -100 region mask, exp,
 // max and sum through quad shuffles); the un-normalised probabilities go to shared memory as 16-bit values and O = P V is a
@@ -376,6 +308,9 @@ int nrpn_window_attention(const void* qkv, int ld_qkv, void* out, int ld_out, co
                           int w, int d, int c, int heads, int shift, int act_fp16, nrpn_stream_t stream) {
     if (!qkv || !out || !qkv_bias || !table || n < 1 || h < 1 || w < 1 || d < 1 || heads < 1 || c != heads * 32) return NRPN_ERR_INVALID;
     if (ld_qkv < 3 * c || ld_out < c || (shift != 0 && shift != 2)) return NRPN_ERR_INVALID;
+    // q / k / v segments and output rows are read and written in 16-byte chunks
+    if (ld_qkv % 8 != 0 || ld_out % 8 != 0 || reinterpret_cast<uintptr_t>(qkv) % 16 != 0 || reinterpret_cast<uintptr_t>(out) % 16 != 0)
+        return NRPN_ERR_INVALID;
     AttnDev P;
     P.qkv = reinterpret_cast<const __nv_bfloat16*>(qkv); P.ld_qkv = ld_qkv; P.out = reinterpret_cast<__nv_bfloat16*>(out); P.ld_out = ld_out;
     P.fp16 = act_fp16 ? 1 : 0;
@@ -385,25 +320,16 @@ int nrpn_window_attention(const void* qkv, int ld_qkv, void* out, int ld_out, co
     P.nwh = P.PH / 4; P.nww = P.PW / 4; P.nwd = P.PD / 4;
     const long windows = (long)n * P.nwh * P.nww * P.nwd;
     if (windows > 0x7fffffffL || heads > 65535) return NRPN_ERR_UNSUPPORTED;
-    // tensor-core path: needs 16-byte aligned 64-byte q/k/v segments; NRPN_ATTN_TC=0 selects the CUDA-core kernel (A/B testing)
-    const char* e = getenv("NRPN_ATTN_TC");
-    const bool tc = !(e && e[0] == '0') && ld_qkv % 8 == 0 && ld_out % 8 == 0 && c % 8 == 0 &&
-                    reinterpret_cast<uintptr_t>(qkv) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0;
-    if (tc) {
-        static bool attr_set = false;
-        if (!attr_set) {
-            NRPN_CUDA_TRY(cudaFuncSetAttribute(window_attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
-            attr_set = true;
-        }
-        const long pairs = (windows + 1) / 2;
-        long gx = (long)num_sms() * 2 / heads;              // 2 resident CTAs per SM in total, each looping over window pairs
-        if (gx < 1) gx = 1;
-        if (gx > pairs) gx = pairs;
-        window_attention_tc_kernel<<<dim3((unsigned)gx, heads), kAttnThreads, kAttnSmem, (cudaStream_t)stream>>>(P, (int)windows);
-        NRPN_LAUNCH_CHECK();
-        return NRPN_OK;
+    static bool attr_set = false;
+    if (!attr_set) {
+        NRPN_CUDA_TRY(cudaFuncSetAttribute(window_attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
+        attr_set = true;
     }
-    window_attention_kernel<<<dim3((unsigned)windows, heads), 64, 0, (cudaStream_t)stream>>>(P);
+    const long pairs = (windows + 1) / 2;
+    long gx = (long)num_sms() * 2 / heads;              // 2 resident CTAs per SM in total, each looping over window pairs
+    if (gx < 1) gx = 1;
+    if (gx > pairs) gx = pairs;
+    window_attention_tc_kernel<<<dim3((unsigned)gx, heads), kAttnThreads, kAttnSmem, (cudaStream_t)stream>>>(P, (int)windows);
     NRPN_LAUNCH_CHECK();
     return NRPN_OK;
 }

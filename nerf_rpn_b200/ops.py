@@ -226,76 +226,33 @@ def is_channels_last_grid(grid: torch.Tensor) -> bool:
     return grid.dim() == 5 and not grid.is_contiguous() and grid.permute(0, 2, 3, 4, 1).is_contiguous()
 
 
-def to_planar(x: torch.Tensor, z_shift: int = 0) -> torch.Tensor:
-    """(N, X, Y, Z, ld) 16-bit channels-last -> planar (N, ld, X, Y, Z) VIEW of a zero-filled buffer whose z pitch is Z + 1 rounded up
-    to a multiple of 8; z_shift = s writes out[z'] = x[z' + s] (zero where the source falls outside): the operand layout of
-    conv3d_wgrad (TMA wants 16-byte aligned inner coordinates, so z offsets live in shifted copies)."""
-    _act16(x, "x")
-    n, X, Y, Z, c = x.shape
-    zp = (Z + 1 + 7) // 8 * 8
-    buf = torch.zeros((n, c, X, Y, zp), dtype=x.dtype, device=x.device)
-    check(lib().nrpn_transpose_to_planar(_ptr(x), n, X, Y, Z, c, c, _ptr(buf), zp, int(z_shift), _stream()), "transpose_to_planar")
-    return buf[..., :Z]
-
-
-def conv3d_wgrad(dys: Sequence[torch.Tensor], xs: Sequence[torch.Tensor], taps: Sequence[Sequence[int]], operands: str = "channels_last") -> torch.Tensor:
-    """dW (taps, Cout, Cin) fp32 of a stride-1 'same' conv from channels-last 16-bit dY (N,X,Y,Z,Cout) and X (N,X,Y,Z,Cin), one pair per
-    pyramid level that shares the weights.  operands="channels_last": the tensors are read where they live (MN-major wgmma operands);
-    "planar": through transposed, z-shifted staging copies (tap z offsets in {-1, 0, +1}) -- the earlier path, kept for comparison."""
-    if operands == "channels_last":
-        return _conv3d_wgrad_cl(dys, xs, taps)
+def wgrad_desc(dys: Sequence[torch.Tensor], xs: Sequence[torch.Tensor], taps: Sequence[Sequence[int]], cout: int, cin: int,
+               act_fp16: int) -> WgradDesc:
+    """nrpn_wgrad_desc of a stride-1 conv's weight gradient: taps and one level per channels-last 16-bit (dY (N,X,Y,Z,ld_dy), X (N,X',Y',Z',ld_x))
+    pair of the pyramid levels that share the weights.  The caller sets dw, workspace, dw_layout and accumulate."""
     d = WgradDesc()
-    d.cout, d.cin, d.n_taps = int(dys[0].shape[-1]), int(xs[0].shape[-1]), len(taps)
-    for t, off in enumerate(taps):
-        for k in range(3):
-            d.tap_off[t][k] = int(off[k])
-    dzs = sorted({int(off[2]) for off in taps})
-    if any(abs(z) > 1 for z in dzs):
-        raise ValueError("conv3d_wgrad: tap z offsets must be in {-1, 0, +1}")
-    d.n_levels = len(dys)
-    keep = []
-    for i, (dy, x) in enumerate(zip(dys, xs)):
-        f16 = _act16(dy, "dy")
-        if _act16(x, "x") != f16 or dy.shape[:4] != x.shape[:4]:
-            raise ValueError("conv3d_wgrad: dy and x must share dtype, batch and spatial extent (stride-1 'same' convolution)")
-        pdy = to_planar(dy)
-        keep.append(pdy)
-        lv = d.level[i]
-        lv.dy_planar = pdy.data_ptr()
-        for z in dzs:
-            px = to_planar(x, z)
-            keep.append(px)
-            lv.x_planar[z + 1] = px.data_ptr()
-        lv.n, lv.x, lv.y, lv.z = int(dy.shape[0]), int(dy.shape[1]), int(dy.shape[2]), int(dy.shape[3])
-        lv.z_pitch = int(pdy.stride(3))
-    d.act_fp16 = f16
-    dw = torch.empty((len(taps), d.cout, d.cin), dtype=torch.float32, device=dys[0].device)
-    need = lib().nrpn_conv3d_wgrad_workspace_bytes(ctypes.byref(d))
-    if need == 0:
-        raise ValueError("conv3d_wgrad: unsupported shape (cout % 128 == 0, cin % 32 == 0, cin <= 256)")
-    ws = _workspace(need, dys[0].device)
-    d.dw, d.workspace, d.workspace_bytes = dw.data_ptr(), ws.data_ptr(), ws.numel()
-    check(lib().nrpn_conv3d_wgrad(ctypes.byref(d), _stream()), "conv3d_wgrad")
-    return dw
-
-
-def _conv3d_wgrad_cl(dys, xs, taps):
-    d = WgradDesc()
-    d.cout, d.cin, d.n_taps = int(dys[0].shape[-1]), int(xs[0].shape[-1]), len(taps)
+    d.cout, d.cin, d.n_taps = int(cout), int(cin), len(taps)
     for t, off in enumerate(taps):
         for k in range(3):
             d.tap_off[t][k] = int(off[k])
     d.n_levels = len(dys)
     for i, (dy, x) in enumerate(zip(dys, xs)):
-        f16 = _act16(dy, "dy")
-        if _act16(x, "x") != f16 or dy.shape[0] != x.shape[0] or not (dy.is_contiguous() and x.is_contiguous()):
-            raise ValueError("conv3d_wgrad: dy and x must be contiguous (N,X,Y,Z,C) tensors of one dtype and batch")
         lv = d.level[i]
         lv.dy_cl, lv.x_cl, lv.ld_dy, lv.ld_x = dy.data_ptr(), x.data_ptr(), int(dy.shape[-1]), int(x.shape[-1])
         lv.n, lv.x, lv.y, lv.z = int(dy.shape[0]), int(dy.shape[1]), int(dy.shape[2]), int(dy.shape[3])
         lv.xx, lv.xy, lv.xz = int(x.shape[1]), int(x.shape[2]), int(x.shape[3])
-    d.act_fp16 = f16
-    d.operand_layout = 1
+    d.act_fp16 = int(act_fp16)
+    return d
+
+
+def conv3d_wgrad(dys: Sequence[torch.Tensor], xs: Sequence[torch.Tensor], taps: Sequence[Sequence[int]]) -> torch.Tensor:
+    """dW (taps, Cout, Cin) fp32 of a stride-1 'same' conv from channels-last 16-bit dY (N,X,Y,Z,Cout) and X (N,X,Y,Z,Cin), one pair per
+    pyramid level that shares the weights.  The tensors are read where they live (MN-major wgmma operands)."""
+    for dy, x in zip(dys, xs):
+        f16 = _act16(dy, "dy")
+        if _act16(x, "x") != f16 or dy.shape[0] != x.shape[0] or not (dy.is_contiguous() and x.is_contiguous()):
+            raise ValueError("conv3d_wgrad: dy and x must be contiguous (N,X,Y,Z,C) tensors of one dtype and batch")
+    d = wgrad_desc(dys, xs, taps, dys[0].shape[-1], xs[0].shape[-1], f16)
     dw = torch.empty((len(taps), d.cout, d.cin), dtype=torch.float32, device=dys[0].device)
     need = lib().nrpn_conv3d_wgrad_workspace_bytes(ctypes.byref(d))
     if need == 0:

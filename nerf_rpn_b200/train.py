@@ -26,11 +26,10 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import ops, packing
-from ._lib import RpnDesc, WgradDesc, check, lib
+from ._lib import RpnDesc, check, lib
 
 
 _TRAIN_GRAPH = os.environ.get("NRPN_TRAIN_GRAPH", "1") != "0"          # static launch lists of the training step replayed as CUDA graphs
-_WGRAD_PLANAR = os.environ.get("NRPN_WGRAD_PLANAR", "0") == "1"      # earlier wgrad operand path (transposed staging copies), for A/B runs
 
 
 
@@ -369,7 +368,7 @@ class _TrainPlan:
         def stem_bwd():
             check(L.nrpn_maxpool3d_k3s2_backward(_p(dp0), _p(self.pool_idx), n, d1[0], d1[1], d1[2], 64, _p(da0), self.f16, _stream()), "maxpool_backward")
             self._bn_bwd(eng.stem_bn, da0, a0, y0, dy0, None, True)
-            self._wgrad_stem(dy0, d1)
+            self._wgrad_stem(dy0)
         self.bwd.append(stem_bwd)
         self.bwd_lo.append(0)
 
@@ -472,7 +471,7 @@ class _TrainPlan:
         def head_bwd():
             h_last = level_views(hs[-1])
             # predictor: wgrad / bias grad into scratch (cls and bbox rows are separate parameters), dgrad -> dh4
-            self._wgrad(self.dpred_levels, h_last, fdims, [(0, 0, 0)], 128, 256, eng.pred_dw, layout=0)
+            self._wgrad(self.dpred_levels, h_last, [(0, 0, 0)], 128, 256, eng.pred_dw, layout=0)
             ws = self._workspace(L.nrpn_bias_grad_workspace_bytes(128))
             check(L.nrpn_bias_grad(_p(self.dpred), self.total_vox, 128, 128, self.f16, _p(eng.pred_db), _p(ws), ws.numel(), _stream()), "bias_grad")
             A, hd = eng.A, eng.head
@@ -483,7 +482,7 @@ class _TrainPlan:
                 layer = eng.hconv[k]
                 check(L.nrpn_relu_backward(_p(dhs[k]), _p(hs[k]), dhs[k].numel(), self.f16, _stream()), "relu_backward")
                 xin = feats if k == 0 else level_views(hs[k - 1])
-                self._wgrad(level_views(dhs[k]), xin, fdims, layer.taps, 256, 256, eng.grad_of(layer.weight), layout=1)
+                self._wgrad(level_views(dhs[k]), xin, layer.taps, 256, 256, eng.grad_of(layer.weight), layout=1)
                 ws = self._workspace(L.nrpn_bias_grad_workspace_bytes(256))
                 check(L.nrpn_bias_grad(_p(dhs[k]), self.total_vox, 256, 256, self.f16, _p(eng.grad_of(layer.bias)), _p(ws), ws.numel(), _stream()), "bias_grad")
                 dst = dfeats if k == 0 else level_views(dhs[k - 1])
@@ -542,41 +541,9 @@ class _TrainPlan:
         check(lib().nrpn_bn_backward(_p(dout), _p(act), _p(y), _p(dy), _p(dres), rows, bn.c, _p(bn.stats), _p(bn.m.weight.data), _p(sums), int(relu),
                                      self.f16, _p(ws), ws.numel(), _stream()), "bn_backward")
 
-    def _planar(self, name, x, zp, z_shift, z_logical=None):
-        """channels-last (n,X,Y,Z,C) -> planar (n,C,X,Y,zp) in a zero-filled scratch buffer."""
-        n, X, Y, Z, C = x.shape
-        buf = self._scratch_buf(name, n * C * X * Y * zp, x.dtype)
-        buf.zero_()
-        check(lib().nrpn_transpose_to_planar(_p(x), n, X, Y, Z, C, C, _p(buf), zp, int(z_shift), _stream()), "transpose_to_planar")
-        return buf
-
-    def _wgrad(self, dys, xs, dims_l, taps, cout, cin, dw, layout, z_extra=0, accumulate=False):
+    def _wgrad(self, dys, xs, taps, cout, cin, dw, layout, accumulate=False):
         """dW of a stride-1 'same' conv from per-level channels-last (dY, X) pairs, written to `dw` (fp32) in `layout`."""
-        d = WgradDesc()
-        d.cout, d.cin, d.n_taps = int(cout), int(cin), len(taps)
-        for t, off in enumerate(taps):
-            for k in range(3):
-                d.tap_off[t][k] = int(off[k])
-        dzs = sorted({int(off[2]) for off in taps})
-        d.n_levels = len(dys)
-        if not _WGRAD_PLANAR:                       # operands where they live: channels-last tensors through MN-major descriptors
-            for i, (dy, x) in enumerate(zip(dys, xs)):
-                lv = d.level[i]
-                lv.dy_cl, lv.x_cl, lv.ld_dy, lv.ld_x = dy.data_ptr(), x.data_ptr(), int(dy.shape[-1]), int(x.shape[-1])
-                lv.n, lv.x, lv.y, lv.z = int(dy.shape[0]), int(dy.shape[1]), int(dy.shape[2]), int(dy.shape[3])
-                lv.xx, lv.xy, lv.xz = int(x.shape[1]), int(x.shape[2]), int(x.shape[3])
-            d.operand_layout = 1
-        for i, (dy, x) in enumerate(zip(dys, xs) if _WGRAD_PLANAR else ()):
-            n, X, Y, Zx = x.shape[0], x.shape[1], x.shape[2], x.shape[3]
-            zl = max(Zx, dy.shape[3])
-            zp = _ru(zl + 1, 8)
-            pdy = self._planar(f"pdy{i}", dy, zp, 0)
-            lv = d.level[i]
-            lv.dy_planar = pdy.data_ptr()
-            for z in dzs:
-                lv.x_planar[z + 1] = self._planar(f"px{i}_{z}", x, zp, z).data_ptr()
-            lv.n, lv.x, lv.y, lv.z, lv.z_pitch = int(n), int(X), int(Y), int(zl), int(zp)
-        d.act_fp16 = self.f16
+        d = ops.wgrad_desc(dys, xs, taps, cout, cin, self.f16)
         d.dw_layout, d.accumulate = int(layout), int(bool(accumulate))
         need = lib().nrpn_conv3d_wgrad_workspace_bytes(ctypes.byref(d))
         if need == 0:
@@ -585,18 +552,18 @@ class _TrainPlan:
         d.dw, d.workspace, d.workspace_bytes = dw.data_ptr(), ws.data_ptr(), ws.numel()
         check(lib().nrpn_conv3d_wgrad(ctypes.byref(d), _stream()), "conv3d_wgrad")
 
-    def _wgrad_stem(self, dy0, d1):
+    def _wgrad_stem(self, dy0):
         eng = self.eng
         st = eng.stem
         dwp = self._scratch_buf("stem_dw", len(st.taps) * 64 * 64, torch.float32)
-        self._wgrad([dy0], [self.packed], [d1], st.taps, 64, 64, dwp, layout=0)
+        self._wgrad([dy0], [self.packed], st.taps, 64, 64, dwp, layout=0)
         g = eng.grad_of(st.weight)
         check(lib().nrpn_gather_pack(_p(dwp), _p(st.scatter_idx), g.numel(), None, _p(g), 1.0, self.f16, _stream()), "gather_pack(stem grad)")
 
     def _conv_bwd(self, layer: _TConv, x, xd, dy, od, dx, bias=False, dx_res=None, accumulate_dx=False):
         """wgrad (+ bias grad) of a stride-1 layer and its data gradient into dx (optionally + dx_res through the conv epilogue)."""
         eng, L, n = self.eng, lib(), self.n
-        self._wgrad([dy], [x], [od], layer.taps, layer.cout, layer.cin_real, eng.grad_of(layer.weight), layout=1)
+        self._wgrad([dy], [x], layer.taps, layer.cout, layer.cin_real, eng.grad_of(layer.weight), layout=1)
         if bias:
             ws = self._workspace(L.nrpn_bias_grad_workspace_bytes(layer.cout))
             rows = dy.numel() // layer.cout
@@ -631,7 +598,7 @@ class _TrainPlan:
             # dx accumulates: [lateral branch, already written by fpn_bwd for stage outputs] + skip / downsample branch + conv1 branch
             if e["ds"] is None:
                 # identity skip: dx = dgrad_c1(dy1) + g   (stride 1 always)
-                self._wgrad([dy1], [xs], [od], e["c1"].taps, planes, cin, eng.grad_of(e["c1"].weight), layout=1)
+                self._wgrad([dy1], [xs], e["c1"].taps, planes, cin, eng.grad_of(e["c1"].weight), layout=1)
                 tgt = dx if not add_lateral else self._scratch_buf("dx_tmp", dx.numel(), dt).view_as(dx)
                 args = [ops.ConvLevelArgs(dy1, tgt, n, od, od, cin, res=g, res_dims=od, ldr=outc)]
                 self._conv_call(e["c1"].bwd, e["c1"].bwd_shift, e["c1"].taps, e["c1"].bwd_cols, cin, args)
@@ -640,8 +607,8 @@ class _TrainPlan:
             else:
                 dyd = self._scratch_buf("dyd", yd.numel(), dt).view_as(yd)
                 self._bn_bwd(e["bnd"], g, None, yd, dyd, None, False)
-                self._wgrad([dy1], [xs], [od], e["c1"].taps, planes, cin, eng.grad_of(e["c1"].weight), layout=1)
-                self._wgrad([dyd], [xs], [od], e["ds"].taps, outc, cin, eng.grad_of(e["ds"].weight), layout=1)
+                self._wgrad([dy1], [xs], e["c1"].taps, planes, cin, eng.grad_of(e["c1"].weight), layout=1)
+                self._wgrad([dyd], [xs], e["ds"].taps, outc, cin, eng.grad_of(e["ds"].weight), layout=1)
                 t1 = self._scratch_buf("t1", n * od[0] * od[1] * od[2] * cin, dt).view(n, *od, cin)
                 args = [ops.ConvLevelArgs(dy1, t1, n, od, od, cin)]
                 self._conv_call(e["c1"].bwd, e["c1"].bwd_shift, e["c1"].taps, e["c1"].bwd_cols, cin, args)

@@ -43,15 +43,18 @@ int main(void) {
   printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\n", offsetof(nrpn_conv_desc, workspace), sizeof(nrpn_conv_level), sizeof(nrpn_conv_desc), offsetof(nrpn_conv_desc, stride),
          offsetof(nrpn_conv_desc, w), offsetof(nrpn_conv_desc, level), sizeof(nrpn_rpn_level), sizeof(nrpn_rpn_desc),
          offsetof(nrpn_rpn_desc, cell_anchors), offsetof(nrpn_rpn_desc, nms_thresh), offsetof(nrpn_rpn_desc, valid));
+  printf("%zu %zu %zu %zu %zu %zu\n", sizeof(nrpn_wgrad_level), sizeof(nrpn_wgrad_desc), offsetof(nrpn_wgrad_desc, level),
+         offsetof(nrpn_wgrad_desc, dw), offsetof(nrpn_wgrad_desc, workspace_bytes), offsetof(nrpn_wgrad_desc, accumulate));
   return 0; }'''
     with tempfile.TemporaryDirectory() as d:
         src, exe = os.path.join(d, "t.c"), os.path.join(d, "t")
         open(src, "w").write(code)
         subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), src, "-o", exe])
         vals = [int(v) for v in subprocess.check_output([exe]).split()]
-    C, R = _lib.ConvDesc, _lib.RpnDesc
+    C, R, W = _lib.ConvDesc, _lib.RpnDesc, _lib.WgradDesc
     mine = [C.workspace.offset, ctypes.sizeof(_lib.ConvLevel), ctypes.sizeof(C), C.stride.offset, C.w.offset, C.level.offset,
-            ctypes.sizeof(_lib.RpnLevel), ctypes.sizeof(R), R.cell_anchors.offset, R.nms_thresh.offset, R.valid.offset]
+            ctypes.sizeof(_lib.RpnLevel), ctypes.sizeof(R), R.cell_anchors.offset, R.nms_thresh.offset, R.valid.offset,
+            ctypes.sizeof(_lib.WgradLevel), ctypes.sizeof(W), W.level.offset, W.dw.offset, W.workspace_bytes.offset, W.accumulate.offset]
     assert mine == vals
 
 

@@ -79,6 +79,17 @@ def test_window_attention_kernel(dims, heads, shift):
     assert err < 3e-2 * max(1.0, ref.abs().max().item()), f"max abs err {err}"
 
 
+def test_window_attention_rejects_unaligned_rows():
+    """Rows are moved in 16-byte chunks: an output row pitch that is not a multiple of 8 elements is an invalid argument, refused
+    before anything is launched."""
+    from nerf_rpn_b200 import ops
+    heads, C = 3, 96
+    qkv = torch.zeros((1, 4, 4, 4, 3 * C), device="cuda", dtype=torch.bfloat16)
+    out = torch.zeros((1, 4, 4, 4, C + 4), device="cuda", dtype=torch.bfloat16)
+    with pytest.raises(RuntimeError, match="invalid argument"):
+        ops.window_attention(qkv, out, torch.zeros(3 * C, device="cuda"), torch.zeros((343, heads), device="cuda"), C, heads, 0)
+
+
 def _attn_ref_wide(xin, sd, heads, shift, C):
     """_window_attention with a 3C-wide input and identity qkv weight (so arbitrary q/k/v can be injected)."""
     import torch

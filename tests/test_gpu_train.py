@@ -149,7 +149,7 @@ def test_wgrad_general_shapes_vs_autograd(L, cout, cin, k):
     plan.eng = type("E", (), {"device": torch.device("cuda")})()
     plan._scratch, plan._ws, plan.f16, plan.n = {}, None, 0, 1
     dw = torch.full((cout, cin, k, k, k), float("nan"), device="cuda")
-    plan._wgrad([dy], [x], [dims], taps, cout, cin, dw, layout=1)
+    plan._wgrad([dy], [x], taps, cout, cin, dw, layout=1)
     torch.cuda.synchronize()
     w = torch.zeros(cout, cin, k, k, k, device="cuda", requires_grad=True)
     F.conv3d(x.float().permute(0, 4, 1, 2, 3), w, padding=k // 2).backward(dy.float().permute(0, 4, 1, 2, 3))

@@ -15,15 +15,13 @@ dys = [torch.randn((1, *d, 256), device="cuda", generator=g).to(torch.bfloat16) 
 taps = [(a - 1, b - 1, c - 1) for a in range(3) for b in range(3) for c in range(3)]
 vox = sum(d[0] * d[1] * d[2] for d in dims)
 fl = 2.0 * vox * 256 * 256 * 27
-for operands in ("channels_last", "planar"):
-    for _ in range(2):
-        dw = ops.conv3d_wgrad(dys, xs, taps, operands=operands)
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(5):
-        dw = ops.conv3d_wgrad(dys, xs, taps, operands=operands)
-    b.record(); torch.cuda.synchronize()
-    ms = a.elapsed_time(b) / 5
-    what = "channels-last operands through MN-major descriptors" if operands == "channels_last" else "incl. planar re-layout of dY and 3 z-shifted copies of X"
-    print(f"wgrad head layer ({what}): {ms:.3f} ms, {fl / ms / 1e9:.1f} TFLOP/s algorithmic (fprop of the same layer: 0.42 ms)")
+for _ in range(2):
+    dw = ops.conv3d_wgrad(dys, xs, taps)
+torch.cuda.synchronize()
+a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+a.record()
+for _ in range(5):
+    dw = ops.conv3d_wgrad(dys, xs, taps)
+b.record(); torch.cuda.synchronize()
+ms = a.elapsed_time(b) / 5
+print(f"wgrad head layer: {ms:.3f} ms, {fl / ms / 1e9:.1f} TFLOP/s algorithmic")
