@@ -454,7 +454,7 @@ int nrpn_fcos_loss(const nrpn_fcos_loss_desc *desc /*host*/, const float *labels
 void nrpn_set_nms_cull_mode(int mode);
 int nrpn_get_nms_cull_mode(void);
 
-/* Diagnostics of the cell-list NMS path (n >= 16 384 boxes): cumulative counters since the last reset -- out16[0..4] for the cross passes
+/* Diagnostics of the cell-list NMS path (n >= 12 288 boxes): cumulative counters since the last reset -- out16[0..4] for the cross passes
  * (records streamed, record x query pair slots, exact IoU evaluations, hits, work items), out16[8..12] the same for the adjacency passes.  Synchronises. */
 int nrpn_nms_cells_stats(unsigned long long *out16, int reset);
 

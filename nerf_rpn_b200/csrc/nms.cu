@@ -5,10 +5,14 @@
 // suppression bit-matrix only for same-group upper-triangle tiles (one thread per row, 64 columns per word,
 // exact-zero culling by bounding circle / z range), resolve each group with one CTA that walks the matrix
 // 64 rows at a time (warp-shuffle resolve of the diagonal word, coalesced OR of the kept rows), then sort
-// the survivors by score.  No host round trips; everything is stream-ordered.  Beyond a scene's proposals: chunked kept-list scan (groups above
-// 3 072 boxes) and, from 12 288 boxes, the cell-list path of nms_cells.cuh (levels: cross / adjacency / dependency rounds; reads a counter back per
-// batch of rounds, so it is skipped under stream capture).  Every path decides a pair with the exact IoU of the sequential loop; what may skip the
-// polygon clip is controlled by nrpn_set_nms_cull_mode (default: exact-zero tests only -> the keep set is provably the reference's).
+// the survivors by score.  No host round trips; everything is stream-ordered.  Three paths reach the same keep set:
+//   1. the bit matrix above, for up to 32 768 boxes with no group above 3 072 boxes (a scene's 4 x 2 500 proposals);
+//   2. the chunked kept-list scan, for larger inputs;
+//   3. from 12 288 boxes, the cell-list path of nms_cells.cuh (levels: cross / adjacency / dependency rounds).  It reads a counter back per
+//      batch of rounds, so it is skipped under stream capture, and it also leaves thr < 0 and NRPN_NMS_CELLS=0 to the other two.  An input
+//      it declines (predecessor-list overflow in dense crowds, or the round cap) goes to path 1 or 2 as if the cell-list path did not exist.
+// Every path decides a pair with the exact IoU of the sequential loop; what may skip the polygon clip is controlled by nrpn_set_nms_cull_mode
+// (default: exact-zero tests only -> the keep set is provably the reference's).
 namespace nrpn { static __device__ int g_iou_mode = 3; }      // see box_iou.cuh: which build of the reference chain is reproduced
 namespace nrpn { static __device__ int g_lens_cull = 0; }     // footprint-lens cull, bit 1 of the NMS cull mode
 #define NRPN_IOU_MODE (::nrpn::g_iou_mode)
@@ -272,35 +276,11 @@ constexpr int kNmsDirectMax = 3072;         // the full matrix (all same-group p
 static inline bool nms_use_matrix(int n, int max_group) { return n <= kNmsMatrixMax && max_group <= kNmsDirectMax; }
 static inline int nms_chunk_size(int n) { return n <= 65536 ? 1024 : kChunk; }
 constexpr int kPrepFloats = 16;
-
-// ---- binned chunked path ------------------------------------------------------------------------------------------------------
-// With n in the hundreds of thousands the chunk-against-kept-list scan is O(n * kept): 1 M boxes spent 3.7 s in it.  Whether box j
-// can be suppressed by kept box k is decided by two necessary conditions that can be INDEXED: (a) their volumes are within a factor
-// 1 / thr_m of each other (IoU <= min V / max V), (b) their bounding circles and z ranges intersect.  Kept boxes are therefore filed in
-// a uniform grid per volume class -- class width log2(1 / thr_m), so partners sit in the same or an adjacent class; cell size >= the
-// class's largest diameter / depth -- and a box only visits the cells its circle and z range can reach in its three classes.
-// Every candidate still goes through the same cull + exact polygon clip: the keep set is the sequential greedy loop's, bit for bit.
-constexpr int kBinMinBoxes = 65536;
 constexpr int kCellMinBoxes = 12288;     // cell-list path (nms_cells.cuh) from here (above the 4 x 2 500 boxes of a scene's proposals, whose NMS runs
-                                         // inside the captured launch sequence); it shares the grid / box_cell buffers below
+                                         // inside the captured launch sequence)
 constexpr int kRatioCullMinBoxes = 16384; // opt-in geometric culls (nrpn_set_nms_cull_mode) never apply below this
-static int cell_min_boxes() {            // NRPN_NMS_CELLS_MIN: where the cell-list path takes over (tuning runs); the ratio culls keep their 16 384 floor
-    static const int v = [] { const char* e = getenv("NRPN_NMS_CELLS_MIN"); const int k = e ? atoi(e) : kCellMinBoxes; return k < 1024 ? 1024 : k; }();
-    return v;
-}
-constexpr int kBinClasses = 16;
-constexpr int kBinMaxXY = 32, kBinMaxZ = 16;
-constexpr int kBinCellsPerClass = kBinMaxXY * kBinMaxXY * kBinMaxZ;
-constexpr int kBinCells = kBinClasses * kBinCellsPerClass + 1;      // + one cell for boxes the culls cannot reason about (visited by everyone)
-constexpr int kBinStatWords = 8 + 2 * kBinClasses;
 
-struct BinGrid {
-    float x0, y0, z0, lv0, inv_lw;       // origin of the box centres, log2-volume origin, 1 / class width
-    int n_cls;
-    float S[kBinClasses], Sz[kBinClasses], rmax[kBinClasses], dmax[kBinClasses];
-    int nx[kBinClasses], ny[kBinClasses], nz[kBinClasses];
-};
-
+// workspace of the matrix and chunked paths; the cell-list path lays out its own (CellWs) behind it
 struct NmsWs {
     unsigned long long* keys;     // n_pad
     unsigned long long* keys2;    // n_pad
@@ -312,13 +292,6 @@ struct NmsWs {
     unsigned long long* removed0; // 64 words: suppression by earlier chunks (chunked path)
     int* kept_pos;                // n (chunked path)
     int* state;                   // [0] kept count, [1..256] first kept index per group
-    // binned chunked path (n >= kBinMinBoxes): kept boxes filed by (volume class, x, y, z) cell
-    struct BinGrid* grid;         // grid parameters (device)
-    unsigned* bstats;             // reduction scratch of the grid (ordered-uint min / max)
-    int* box_cell;                // n: cell of every box
-    int* cell_start;              // kBinCells + 1: exclusive scan of the per-cell box counts (capacity of the cell's segment)
-    int* cell_fill;               // kBinCells: kept boxes filed so far
-    float4* cell_recs;            // n x 3 float4: per kept box {cull record (8 floats), position, group, -, -}, cell by cell
     size_t total;
 };
 
@@ -339,14 +312,7 @@ static NmsWs nms_layout(void* base, int n) {
     w.mask = (unsigned long long*)(b + take(chunked ? (size_t)kChunk * 64 * 8 : (size_t)n * W * 8));
     w.removed0 = (unsigned long long*)(b + take(64 * 8));
     w.kept_pos = (int*)(b + take((size_t)n * 4));
-    w.state = (int*)(b + take(258 * 4));          // [0] kept count, [1..256] per-group starts, [257] kept boxes already filed in the grid
-    const bool binned = n >= (cell_min_boxes() < kBinMinBoxes ? cell_min_boxes() : kBinMinBoxes);
-    w.grid = (BinGrid*)(b + take(sizeof(BinGrid)));
-    w.bstats = (unsigned*)(b + take(kBinStatWords * 4));
-    w.box_cell = (int*)(b + take(binned ? (size_t)n * 4 : 4));
-    w.cell_start = (int*)(b + take(binned ? (size_t)(kBinCells + 1) * 4 : 4));
-    w.cell_fill = (int*)(b + take(binned ? (size_t)kBinCells * 4 : 4));
-    w.cell_recs = (float4*)(b + take(binned ? (size_t)n * 48 : 16));
+    w.state = (int*)(b + take(257 * 4));          // [0] kept count, [1..256] per-group starts
     w.total = off;
     return w;
 }
@@ -387,7 +353,7 @@ __global__ void nms_prep_kernel(const unsigned long long* __restrict__ keys, con
         float b[6];
 #pragma unroll
         for (int i = 0; i < 6; ++i) { b[i] = boxes[(size_t)idx * 6 + i]; o[i] = b[i]; }
-        // cull record of an axis-aligned box (binned path only): volume, z range, bounding circle of the footprint
+        // cull record of an axis-aligned box (cell-list path only): volume, z range, bounding circle of the footprint
         const float w = b[3] - b[0], h = b[4] - b[1], d = b[5] - b[2];
         bool fin = true;
 #pragma unroll
@@ -535,6 +501,42 @@ __device__ __forceinline__ unsigned long long shfl64(unsigned long long v, int s
     return ((unsigned long long)hi << 32) | lo;
 }
 
+// The two resolve kernels below walk a bit matrix (row stride W words) 64 rows at a time with one 256-thread CTA.  Per word c:
+// warp 0 resolves the diagonal 64 x 64 block of word c: rows c * 64 + i with lo <= row < hi take part, `removed` holds what earlier words
+// suppressed; returns the kept rows
+__device__ __forceinline__ unsigned long long resolve_diag_word(const unsigned long long* __restrict__ mask, int W, int c, int lo, int hi,
+                                                                const unsigned long long* removed, int lane) {
+    const int r_lo = c * 64 + lane, r_hi = r_lo + 32;
+    const bool v_lo = r_lo >= lo && r_lo < hi, v_hi = r_hi >= lo && r_hi < hi;
+    const unsigned long long d_lo = v_lo ? mask[(size_t)r_lo * W + c] : 0ull;
+    const unsigned long long d_hi = v_hi ? mask[(size_t)r_hi * W + c] : 0ull;
+    const unsigned b_lo = __ballot_sync(0xffffffffu, v_lo), b_hi = __ballot_sync(0xffffffffu, v_hi);
+    const unsigned long long valid = ((unsigned long long)b_hi << 32) | b_lo;
+    unsigned long long rem = removed[c] | ~valid;
+    unsigned long long kept = 0ull;
+#pragma unroll 8
+    for (int i = 0; i < 64; ++i) {
+        const unsigned long long rowbits = shfl64(i < 32 ? d_lo : d_hi, i & 31);
+        if (!((rem >> i) & 1ull)) { kept |= 1ull << i; rem |= rowbits; }
+    }
+    return kept;
+}
+
+// all 8 warps OR the kept rows of word c into the removed words c + 1 .. w_end - 1: lane <-> word (coalesced), warp <-> 8 of the 64 rows,
+// so up to 8 independent loads per thread are in flight (one thread per word walking the kept rows serially costs 64 dependent L2 round trips)
+__device__ __forceinline__ void or_kept_rows(const unsigned long long* __restrict__ mask, int W, int c, int w_end, unsigned long long kept,
+                                             unsigned long long* removed, int warp, int lane) {
+    const unsigned long long mine = (kept >> (warp * 8)) & 0xFFull;
+    if (!mine) return;
+    for (int w = c + 1 + lane; w < w_end; w += 32) {
+        unsigned long long acc = 0ull;
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+            if ((mine >> i) & 1ull) acc |= mask[(size_t)(c * 64 + warp * 8 + i) * W + w];
+        if (acc) atomicOr(&removed[w], acc);
+    }
+}
+
 // one CTA per group id
 __global__ void __launch_bounds__(256) nms_resolve_kernel(const unsigned long long* __restrict__ mask, int W, int n,
                                                           const int* __restrict__ seg, int ignore_group,
@@ -551,46 +553,22 @@ __global__ void __launch_bounds__(256) nms_resolve_kernel(const unsigned long lo
     __syncthreads();
     for (int c = c0; c <= c1; ++c) {
         if (warp == 0) {
-            const int r_lo = c * 64 + lane, r_hi = r_lo + 32;
-            const bool v_lo = r_lo >= s && r_lo < e, v_hi = r_hi >= s && r_hi < e;
-            const unsigned long long d_lo = v_lo ? mask[(size_t)r_lo * W + c] : 0ull;
-            const unsigned long long d_hi = v_hi ? mask[(size_t)r_hi * W + c] : 0ull;
-            const unsigned b_lo = __ballot_sync(0xffffffffu, v_lo), b_hi = __ballot_sync(0xffffffffu, v_hi);
-            const unsigned long long valid = ((unsigned long long)b_hi << 32) | b_lo;
-            unsigned long long rem = removed[c] | ~valid;
-            unsigned long long kept = 0ull;
-#pragma unroll 8
-            for (int i = 0; i < 64; ++i) {
-                const unsigned long long rowbits = shfl64(i < 32 ? d_lo : d_hi, i & 31);
-                if (!((rem >> i) & 1ull)) { kept |= 1ull << i; rem |= rowbits; }
-            }
+            const unsigned long long kept = resolve_diag_word(mask, W, c, s, e, removed, lane);
             if (lane == 0) { kept_sh = kept; if (kept) atomicOr(&keepbits[c], kept); }
         }
         __syncthreads();
-        // OR the kept rows into the removed words right of the diagonal: lane <-> word (coalesced), warp <-> 8 of the 64
-        // rows, so up to 8 independent loads per thread are in flight (this loop used to be one thread per word walking
-        // the kept rows serially: 64 dependent L2 round trips per chunk)
-        const unsigned long long kept = kept_sh;
-        const unsigned long long mine = (kept >> (warp * 8)) & 0xFFull;
-        if (mine) {
-            for (int w = c + 1 + lane; w <= c1; w += 32) {
-                unsigned long long acc = 0ull;
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    if ((mine >> i) & 1ull) acc |= mask[(size_t)(c * 64 + warp * 8 + i) * W + w];
-                if (acc) atomicOr(&removed[w], acc);
-            }
-        }
+        or_kept_rows(mask, W, c, c1 + 1, kept_sh, removed, warp, lane);
         __syncthreads();
     }
 }
 
 // ------------------------------------------------------------------------------ chunked path (n > 32 768)
-// Sorted boxes are processed in chunks of 4096: (a) every box of the chunk is tested against the boxes KEPT so far
-// (one warp per box, lanes stride over the kept list of its group, exact-zero culling first), (b) the 4096 x 4096 bit
-// matrix of the chunk is built with the same tile kernel as the matrix path, (c) one CTA resolves the chunk and appends
-// the survivors to the kept list. Greedy semantics are unchanged: a box is suppressed iff a higher-scored KEPT box of
-// its group overlaps it by more than the threshold.
+// Sorted boxes are processed in chunks of 1024 (up to 65 536 boxes) or 4096: (a) every box of the chunk is tested against the
+// boxes KEPT so far (one warp per box, lanes stride over the kept list of its group, exact-zero culling first), (b) the chunk's
+// own bit matrix is built with the same tile kernel as the matrix path, (c) one CTA resolves the chunk and appends the
+// survivors to the kept list. Greedy semantics are unchanged: a box is suppressed iff a higher-scored KEPT box of its group
+// overlaps it by more than the threshold.  The scan costs O(n * kept); from 12 288 boxes it runs only where the cell-list path
+// does not (top of this file), mostly on the dense crowds that path declines, and those keep few boxes.
 constexpr int kCrossTile = 256;      // kept records staged per step (one per thread)
 
 // One warp per box of the chunk, 8 boxes per CTA.  The kept list is streamed through shared memory in tiles of 256 cull
@@ -734,19 +712,7 @@ __global__ void __launch_bounds__(256) nms_chunk_resolve_kernel(const unsigned l
     __syncthreads();
     for (int c = 0; c < Wc; ++c) {
         if (warp == 0) {
-            const int r_lo = c * 64 + lane, r_hi = r_lo + 32;
-            const bool v_lo = r_lo < chunk_n, v_hi = r_hi < chunk_n;
-            const unsigned long long d_lo = v_lo ? cmask[(size_t)r_lo * Wc + c] : 0ull;
-            const unsigned long long d_hi = v_hi ? cmask[(size_t)r_hi * Wc + c] : 0ull;
-            const unsigned b_lo = __ballot_sync(0xffffffffu, v_lo), b_hi = __ballot_sync(0xffffffffu, v_hi);
-            const unsigned long long valid = ((unsigned long long)b_hi << 32) | b_lo;
-            unsigned long long rem = removed[c] | ~valid;
-            unsigned long long kept = 0ull;
-#pragma unroll 8
-            for (int i = 0; i < 64; ++i) {
-                const unsigned long long rowbits = shfl64(i < 32 ? d_lo : d_hi, i & 31);
-                if (!((rem >> i) & 1ull)) { kept |= 1ull << i; rem |= rowbits; }
-            }
+            const unsigned long long kept = resolve_diag_word(cmask, Wc, c, 0, chunk_n, removed, lane);
             // append survivors in order; remember where each group's kept boxes start
             const int base = kept_base;
 #pragma unroll
@@ -762,245 +728,11 @@ __global__ void __launch_bounds__(256) nms_chunk_resolve_kernel(const unsigned l
             if (lane == 0) { kept_sh = kept; kept_base = base + __popcll(kept); keepbits[(chunk_begin >> 6) + c] = kept; }
         }
         __syncthreads();
-        const unsigned long long kept = kept_sh;
-        const unsigned long long mine = (kept >> (warp * 8)) & 0xFFull;
-        if (mine) {
-            for (int w = c + 1 + lane; w < Wc; w += 32) {
-                unsigned long long acc = 0ull;
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    if ((mine >> i) & 1ull) acc |= cmask[(size_t)(c * 64 + warp * 8 + i) * Wc + w];
-                if (acc) atomicOr(&removed[w], acc);
-            }
-        }
+        or_kept_rows(cmask, Wc, c, Wc, kept_sh, removed, warp, lane);
         __syncthreads();
     }
     if (tid == 0) state[0] = kept_base;
 }
-
-
-// ------------------------------------------------------------------------------ binned chunked path (n >= kBinMinBoxes)
-__device__ __forceinline__ float ordered_to_float(unsigned u) { return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u); }
-
-// pass 0 (pass == 0): min / max of centre x, y, z and of log2(volume) over the cullable boxes.  pass 1: per-class max radius / depth.
-__global__ void nms_bin_stats_kernel(const float* __restrict__ prep, int n, int pass, const BinGrid* __restrict__ grid, unsigned* __restrict__ st) {
-    const int p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= n) return;
-    const float* t = prep + (size_t)p * kPrepFloats + 8;
-    if (!__float_as_int(t[7])) return;
-    const float zc = 0.5f * (t[2] + t[3]), lv = log2f(t[1]);
-    if (pass == 0) {
-        atomicMin(&st[0], float_to_ordered(t[4])); atomicMax(&st[1], float_to_ordered(t[4]));
-        atomicMin(&st[2], float_to_ordered(t[5])); atomicMax(&st[3], float_to_ordered(t[5]));
-        atomicMin(&st[4], float_to_ordered(zc)); atomicMax(&st[5], float_to_ordered(zc));
-        atomicMin(&st[6], float_to_ordered(lv)); atomicMax(&st[7], float_to_ordered(lv));
-    } else {
-        int c = (int)floorf((lv - grid->lv0) * grid->inv_lw);
-        c = c < 0 ? 0 : (c >= grid->n_cls ? grid->n_cls - 1 : c);
-        atomicMax(&st[8 + c], float_to_ordered(t[6]));
-        atomicMax(&st[8 + kBinClasses + c], float_to_ordered(t[3] - t[2]));
-    }
-}
-
-__global__ void nms_bin_stats_init_kernel(unsigned* __restrict__ st) {
-    const int t = threadIdx.x;
-    if (t < kBinStatWords) st[t] = (t < 8 && !(t & 1)) ? 0xFFFFFFFFu : 0u;          // mins start at +max, maxes at the lowest key
-}
-
-// stage 0: class mapping from the global extents; stage 1: per-class cell sizes / counts from the per-class maxima
-__global__ void nms_bin_grid_kernel(const unsigned* __restrict__ st, float thr_m, int stage, BinGrid* __restrict__ g) {
-    if (threadIdx.x != 0) return;
-    if (stage == 0) {
-        const bool any = st[0] != 0xFFFFFFFFu;
-        g->x0 = any ? ordered_to_float(st[0]) : 0.f; g->y0 = any ? ordered_to_float(st[2]) : 0.f; g->z0 = any ? ordered_to_float(st[4]) : 0.f;
-        g->lv0 = any ? ordered_to_float(st[6]) : 0.f;
-        const float span = any ? ordered_to_float(st[7]) - g->lv0 : 0.f;
-        float width = (thr_m > 0.f && thr_m < 1.f) ? log2f(1.0f / thr_m) : 1e30f;        // no ratio cull: a single class
-        if (span / width > (float)(kBinClasses - 1)) width = span / (float)(kBinClasses - 1) * 1.0001f;   // wider classes stay conservative
-        g->inv_lw = 1.0f / width;
-        int nc = (int)floorf(span * g->inv_lw) + 1;
-        g->n_cls = nc < 1 ? 1 : (nc > kBinClasses ? kBinClasses : nc);
-        return;
-    }
-    const float ex = ordered_to_float(st[1]) - g->x0, ey = ordered_to_float(st[3]) - g->y0, ez = ordered_to_float(st[5]) - g->z0;
-    for (int c = 0; c < kBinClasses; ++c) {
-        const float r = st[8 + c] ? ordered_to_float(st[8 + c]) : 0.f, d = st[8 + kBinClasses + c] ? ordered_to_float(st[8 + kBinClasses + c]) : 0.f;
-        g->rmax[c] = r; g->dmax[c] = d;
-        // cells half of the class's largest diameter / depth wide: a query window of +-(r_j + r_c) / S cells then hugs the volume that can
-        // hold a partner (3 x 3 cells of size 2 r_c would cover 3x that area) while a box still visits only ~100 cells per class
-        float S = fmaxf(r, fmaxf(ex, ey) / (float)kBinMaxXY * 1.0001f);
-        float Sz = fmaxf(0.5f * d, ez / (float)kBinMaxZ * 1.0001f);
-        if (!(S > 0.f)) S = 1.0f;
-        if (!(Sz > 0.f)) Sz = 1.0f;
-        g->S[c] = S; g->Sz[c] = Sz;
-        int nx = (int)floorf(ex / S) + 1, ny = (int)floorf(ey / S) + 1, nz = (int)floorf(ez / Sz) + 1;
-        g->nx[c] = nx < 1 ? 1 : (nx > kBinMaxXY ? kBinMaxXY : nx);
-        g->ny[c] = ny < 1 ? 1 : (ny > kBinMaxXY ? kBinMaxXY : ny);
-        g->nz[c] = nz < 1 ? 1 : (nz > kBinMaxZ ? kBinMaxZ : nz);
-    }
-}
-
-__device__ __forceinline__ int bin_clampi(int v, int n) { return v < 0 ? 0 : (v >= n ? n - 1 : v); }
-
-// cell of every box (kBinCells - 1 = the "everywhere" cell of boxes without a usable cull record) + per-cell counts
-__global__ void nms_bin_assign_kernel(const float* __restrict__ prep, int n, const BinGrid* __restrict__ g, int* __restrict__ box_cell,
-                                      int* __restrict__ cell_count) {
-    const int p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= n) return;
-    const float* t = prep + (size_t)p * kPrepFloats + 8;
-    int cell = kBinCells - 1;
-    if (__float_as_int(t[7])) {
-        int c = (int)floorf((log2f(t[1]) - g->lv0) * g->inv_lw);
-        c = bin_clampi(c, g->n_cls);
-        const int ix = bin_clampi((int)floorf((t[4] - g->x0) / g->S[c]), g->nx[c]);
-        const int iy = bin_clampi((int)floorf((t[5] - g->y0) / g->S[c]), g->ny[c]);
-        const int iz = bin_clampi((int)floorf((0.5f * (t[2] + t[3]) - g->z0) / g->Sz[c]), g->nz[c]);
-        cell = c * kBinCellsPerClass + (iz * kBinMaxXY + iy) * kBinMaxXY + ix;
-    }
-    box_cell[p] = cell;
-    atomicAdd(&cell_count[cell], 1);
-}
-
-// exclusive scan of cell_count (kBinCells entries) into cell_start (kBinCells + 1), one CTA
-__global__ void __launch_bounds__(1024) nms_bin_scan_kernel(const int* __restrict__ cell_count, int* __restrict__ cell_start) {
-    __shared__ int part[1024];
-    const int t = threadIdx.x;
-    const int per = (kBinCells + 1023) / 1024;
-    const int b = t * per, e = b + per < kBinCells ? b + per : kBinCells;
-    int s = 0;
-    for (int i = b; i < e; ++i) s += cell_count[i];
-    part[t] = s;
-    __syncthreads();
-    for (int o = 1; o < 1024; o <<= 1) { const int v = t >= o ? part[t - o] : 0; __syncthreads(); part[t] += v; __syncthreads(); }
-    int run = part[t] - s;
-    for (int i = b; i < e; ++i) { cell_start[i] = run; run += cell_count[i]; }
-    if (t == 1023) cell_start[kBinCells] = part[1023];
-}
-
-// One warp per box of the chunk.  Lanes take the cells of the box's 3-D window in the current volume class (32 cells per batch), each lane walks
-// its own cell's kept records -- 48-byte records {cull record, position, group} stored cell by cell, so the walk is one sequential stream per
-// lane with no dependent look-ups; entries that survive the group / cull tests are queued and the exact IoU runs on full batches of 32
-// (cf. nms_cross_kernel).
-__global__ void __launch_bounds__(256, 2) nms_cross_binned_kernel(const float* __restrict__ prep, const int* __restrict__ sgroup, int box_dim,
-                                                                  float thr, float thr_m, int ignore_group, int chunk_begin, int chunk_n,
-                                                                  const BinGrid* __restrict__ grid, const int* __restrict__ cell_start,
-                                                                  const int* __restrict__ cell_fill, const float4* __restrict__ cell_recs,
-                                                                  unsigned long long* __restrict__ removed0) {
-    __shared__ int queue[8][64];
-    const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31;
-    const int w = blockIdx.x * 8 + wid;
-    if (w >= chunk_n) return;
-    const int p = chunk_begin + w;
-    const int g = sgroup[p];
-    if (g == ignore_group) { if (lane == 0) atomicOr(&removed0[w >> 6], 1ull << (w & 63)); return; }
-    const float* bp = prep + (size_t)p * kPrepFloats;
-    float btail[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) btail[i] = bp[8 + i];
-    const bool cull_ok = (0.0f <= thr);
-    const BinGrid& G = *grid;
-    const bool j_cull = __float_as_int(btail[7]) != 0 && cull_ok;
-    int cj = 0;
-    if (j_cull) cj = bin_clampi((int)floorf((log2f(btail[1]) - G.lv0) * G.inv_lw), G.n_cls);
-    const float zc = 0.5f * (btail[2] + btail[3]), dj = btail[3] - btail[2];
-    int qn = 0;
-    bool sup = false;
-
-    auto exact = [&](int pos) -> bool {                 // the decision of the sequential loop for one kept box
-        const float* ap = prep + (size_t)pos * kPrepFloats;
-        if (box_dim == 7) { ObbPrep a, b; load_prep(ap, a); load_prep(bp, b); return obb_suppresses(a, b, thr); }
-        float aa[6], bb[6];
-#pragma unroll
-        for (int i = 0; i < 6; ++i) { aa[i] = ap[i]; bb[i] = bp[i]; }
-        return !(iou3d_aabb(aa, bb) <= thr);
-    };
-    auto visit = [&](int beg, int end) {                // every lane walks its own record range; reports through `sup`
-        int e = beg;
-        while (true) {
-            const bool have = e < end;
-            if (!__any_sync(0xffffffffu, have)) break;
-            bool c = false;
-            int pos = 0;
-            if (have) {
-                const float4* r = cell_recs + (size_t)e * 3;
-                const float4 r0 = __ldg(r), r1 = __ldg(r + 1), r2 = __ldg(r + 2);
-                pos = __float_as_int(r2.x);
-                if (__float_as_int(r2.y) == g) {
-                    const float at[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-                    c = !(cull_ok && obb_surely_not_above(at, btail, thr_m));
-                }
-                ++e;
-            }
-            const unsigned m = __ballot_sync(0xffffffffu, c);
-            if (m) {
-                if (c) queue[wid][qn + __popc(m & ((1u << lane) - 1u))] = pos;
-                qn += __popc(m);
-                __syncwarp();
-                if (qn >= 32) {
-                    const bool hit = exact(queue[wid][lane]);
-                    if (__any_sync(0xffffffffu, hit)) { sup = true; return; }
-                    const int rest = qn - 32;
-                    const int moved = lane < rest ? queue[wid][32 + lane] : 0;
-                    __syncwarp();
-                    if (lane < rest) queue[wid][lane] = moved;
-                    qn = rest;
-                    __syncwarp();
-                }
-            }
-        }
-    };
-
-    {   // boxes without a cull record sit in the last cell: everyone visits it, the lanes share its records in contiguous pieces
-        const int cs = cell_start[kBinCells - 1], cf = cell_fill[kBinCells - 1];
-        const int per = (cf + 31) / 32;
-        const int b0 = cs + lane * per, b1 = min(cs + cf, b0 + per);
-        visit(b0, b1 > b0 ? b1 : b0);
-    }
-    if (!sup) {
-        const int c_lo = j_cull ? max(cj - 1, 0) : 0, c_hi = j_cull ? min(cj + 1, G.n_cls - 1) : G.n_cls - 1;
-        for (int c = c_lo; c <= c_hi && !sup; ++c) {
-            int ix0 = 0, ix1 = G.nx[c] - 1, iy0 = 0, iy1 = G.ny[c] - 1, iz0 = 0, iz1 = G.nz[c] - 1;
-            if (j_cull) {
-                const float R = btail[6] + G.rmax[c], Rz = 0.5f * (dj + G.dmax[c]);
-                ix0 = bin_clampi((int)floorf((btail[4] - R - G.x0) / G.S[c]), G.nx[c]); ix1 = bin_clampi((int)floorf((btail[4] + R - G.x0) / G.S[c]), G.nx[c]);
-                iy0 = bin_clampi((int)floorf((btail[5] - R - G.y0) / G.S[c]), G.ny[c]); iy1 = bin_clampi((int)floorf((btail[5] + R - G.y0) / G.S[c]), G.ny[c]);
-                iz0 = bin_clampi((int)floorf((zc - Rz - G.z0) / G.Sz[c]), G.nz[c]); iz1 = bin_clampi((int)floorf((zc + Rz - G.z0) / G.Sz[c]), G.nz[c]);
-            }
-            const int wx = ix1 - ix0 + 1, wy = iy1 - iy0 + 1, wxy = wx * wy, n_cells = wxy * (iz1 - iz0 + 1);
-            for (int k0 = 0; k0 < n_cells && !sup; k0 += 32) {
-                const int k = k0 + lane;
-                int beg = 0, end = 0;
-                if (k < n_cells) {
-                    const int kz = k / wxy, kr = k - kz * wxy;
-                    const int cell = c * kBinCellsPerClass + ((iz0 + kz) * kBinMaxXY + (iy0 + kr / wx)) * kBinMaxXY + ix0 + kr % wx;
-                    beg = cell_start[cell]; end = beg + cell_fill[cell];
-                }
-                visit(beg, end);
-            }
-        }
-    }
-    if (!sup && qn > 0) {
-        bool hit = false;
-        if (lane < qn) hit = exact(queue[wid][lane]);
-        if (__any_sync(0xffffffffu, hit)) sup = true;
-    }
-    if (sup && lane == 0) atomicOr(&removed0[w >> 6], 1ull << (w & 63));
-}
-
-// files the survivors of a resolved chunk (kept_pos[k0 .. k1)) in their cells
-__global__ void nms_bin_file_kernel(const int* __restrict__ kept_pos, const int* __restrict__ state, int* __restrict__ filed, const int* __restrict__ box_cell,
-                                    const float* __restrict__ prep, const int* __restrict__ sgroup, const int* __restrict__ cell_start,
-                                    int* __restrict__ cell_fill, float4* __restrict__ cell_recs) {
-    const int k0 = filed[0], k1 = state[0];
-    for (int k = k0 + blockIdx.x * blockDim.x + threadIdx.x; k < k1; k += gridDim.x * blockDim.x) {
-        const int pos = kept_pos[k], cell = box_cell[pos];
-        const float4* t = reinterpret_cast<const float4*>(prep + (size_t)pos * kPrepFloats + 8);
-        float4* r = cell_recs + (size_t)(cell_start[cell] + atomicAdd(&cell_fill[cell], 1)) * 3;
-        r[0] = t[0]; r[1] = t[1];
-        r[2] = make_float4(__int_as_float(pos), __int_as_float(sgroup[pos]), 0.f, 0.f);
-    }
-}
-__global__ void nms_bin_filed_kernel(const int* __restrict__ state, int* __restrict__ filed) { filed[0] = state[0]; }
 
 __global__ void nms_state_init_kernel(int* __restrict__ state) {
     const int t = threadIdx.x;
@@ -1031,16 +763,14 @@ __global__ void nms_emit_kernel(const unsigned long long* __restrict__ keys2, in
 
 #include "nms_cells.cuh"
 
-static int level_growth_pct() {          // level e -> e * pct / 100 (NRPN_NMS_LEVEL_GROWTH_PCT, tuning runs; >= 110)
-    static const int v = [] { const char* e = getenv("NRPN_NMS_LEVEL_GROWTH_PCT"); const int k = e ? atoi(e) : kLevelGrowth * 100; return k < 110 ? 110 : k; }();
-    return v;
-}
-
 static size_t cl_layout(void* base, int n, CellWs* out) {
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
     char* b = (char*)base;
     CellWs c;
+    c.grid = (BinGrid*)(b + take(sizeof(BinGrid)));
+    c.bstats = (unsigned*)(b + take(kBinStatWords * 4));
+    c.box_cell = (int*)(b + take((size_t)n * 4));
     c.state = (signed char*)(b + take((size_t)n));
     c.adj_cnt = (int*)(b + take((size_t)n * 4));
     c.adj = (int*)(b + take((size_t)n * kAdjSlots * 4));
@@ -1071,16 +801,8 @@ static int nms_run_cells(const float* boxes, int box_dim, const float* scores, c
     if (rc) return rc;
     nms_prep_kernel<<<ceil_div(n, 128), 128, 0, st>>>(w.keys, boxes, box_dim, n, w.prep, w.sgroup, w.seg, group);
     NRPN_LAUNCH_CHECK();
-    // grid of the cell lists (shared with the chunked path's index: extents -> volume classes -> per-class cell sizes -> cell of every box)
-    nms_bin_stats_init_kernel<<<1, 64, 0, st>>>(w.bstats);
-    nms_bin_stats_kernel<<<ceil_div(n, 256), 256, 0, st>>>(w.prep, n, 0, w.grid, w.bstats);
-    nms_bin_grid_kernel<<<1, 32, 0, st>>>(w.bstats, thr_m, 0, w.grid);
-    nms_bin_stats_kernel<<<ceil_div(n, 256), 256, 0, st>>>(w.prep, n, 1, w.grid, w.bstats);
-    nms_bin_grid_kernel<<<1, 32, 0, st>>>(w.bstats, thr_m, 1, w.grid);
-    NRPN_LAUNCH_CHECK();
-    NRPN_CUDA_TRY(cudaMemsetAsync(w.cell_fill, 0, (size_t)kBinCells * 4, st));
-    nms_bin_assign_kernel<<<ceil_div(n, 256), 256, 0, st>>>(w.prep, n, w.grid, w.box_cell, w.cell_fill);
-    NRPN_LAUNCH_CHECK();
+    rc = cl_build_grid(c, w.prep, n, thr_m, st);
+    if (rc) return rc;
     NRPN_CUDA_TRY(cudaMemsetAsync(c.A.cursor, 0, (size_t)kBinCells * 4, st));
     NRPN_CUDA_TRY(cudaMemsetAsync(c.B.cursor, 0, (size_t)kBinCells * 4, st));
     NRPN_CUDA_TRY(cudaMemsetAsync(c.fail, 0, 4, st));
@@ -1089,7 +811,7 @@ static int nms_run_cells(const float* boxes, int box_dim, const float* scores, c
 
     static const int pair_grid = [] { int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); return 2 * sms; }();
     PairArgs pa;
-    pa.prep = w.prep; pa.box_dim = box_dim; pa.thr = thr; pa.thr_m = thr_m; pa.grid = w.grid;
+    pa.prep = w.prep; pa.box_dim = box_dim; pa.thr = thr; pa.thr_m = thr_m; pa.grid = c.grid;
     pa.qstart = c.B.start; pa.qrecs = c.B.recs; pa.item_start = c.B.item_start; pa.items = c.B.items; pa.work = c.meta;
     pa.state = c.state; pa.adj_cnt = c.adj_cnt; pa.adj = c.adj; pa.fail = c.fail;
     int b = 0;
@@ -1123,7 +845,7 @@ static int nms_run_cells(const float* boxes, int box_dim, const float* scores, c
             if (h[0] == 0) break;
         }
         b = e;
-        { const long long nx = (long long)e * level_growth_pct() / 100; e = nx > (long long)n ? n : (int)nx; }
+        { const long long nx = (long long)e * kLevelGrowth; e = nx > (long long)n ? n : (int)nx; }
     }
     const int nblk = ceil_div(n, 1024);
     cl_keep_count_kernel<<<nblk, 1024, 0, st>>>(c.state, n, c.blk);
@@ -1135,7 +857,7 @@ static int nms_run_cells(const float* boxes, int box_dim, const float* scores, c
 
 size_t nms_workspace_bytes(int n) {
     if (n <= 0) return 256;
-    return nms_layout(nullptr, n).total + (n >= cell_min_boxes() ? cl_layout(nullptr, n, nullptr) : 0) + 256;
+    return nms_layout(nullptr, n).total + (n >= kCellMinBoxes ? cl_layout(nullptr, n, nullptr) : 0) + 256;
 }
 
 int nms_run(const float* boxes, int box_dim, const float* scores, const int32_t* group, int n, float thr, int ignore_group,
@@ -1162,7 +884,7 @@ int nms_run(const float* boxes, int box_dim, const float* scores, const int32_t*
             applied.store(lens, std::memory_order_relaxed);
         }
     }
-    if (n >= cell_min_boxes() && thr >= 0.0f) {
+    if (n >= kCellMinBoxes && thr >= 0.0f) {
         static const bool cells_off = [] { const char* e = getenv("NRPN_NMS_CELLS"); return e && e[0] == '0'; }();
         cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
         cudaStreamIsCapturing(st, &cap);                    // the level loop reads counters back: not capturable
@@ -1194,42 +916,11 @@ int nms_run(const float* boxes, int box_dim, const float* scores, const int32_t*
         nms_state_init_kernel<<<1, 256, 0, st>>>(w.state);
         NRPN_LAUNCH_CHECK();
         const int chunk = nms_chunk_size(n);
-        static const bool bin_off = [] { const char* e = getenv("NRPN_NMS_BINNED"); return e && e[0] == '0'; }();
-        const bool binned = n >= kBinMinBoxes && !bin_off;
-        int* filed = w.state + 257;
-        if (binned) {
-            // grid of the kept-box index: extents -> classes -> per-class cell sizes -> cell of every box -> segment capacities
-            nms_bin_stats_init_kernel<<<1, 64, 0, st>>>(w.bstats);
-            NRPN_LAUNCH_CHECK();
-            nms_bin_stats_kernel<<<ceil_div(n, 256), 256, 0, st>>>(w.prep, n, 0, w.grid, w.bstats);
-            NRPN_LAUNCH_CHECK();
-            nms_bin_grid_kernel<<<1, 32, 0, st>>>(w.bstats, thr_m, 0, w.grid);
-            NRPN_LAUNCH_CHECK();
-            nms_bin_stats_kernel<<<ceil_div(n, 256), 256, 0, st>>>(w.prep, n, 1, w.grid, w.bstats);
-            NRPN_LAUNCH_CHECK();
-            nms_bin_grid_kernel<<<1, 32, 0, st>>>(w.bstats, thr_m, 1, w.grid);
-            NRPN_LAUNCH_CHECK();
-            NRPN_CUDA_TRY(cudaMemsetAsync(w.cell_fill, 0, (size_t)kBinCells * 4, st));
-            nms_bin_assign_kernel<<<ceil_div(n, 256), 256, 0, st>>>(w.prep, n, w.grid, w.box_cell, w.cell_fill);
-            NRPN_LAUNCH_CHECK();
-            nms_bin_scan_kernel<<<1, 1024, 0, st>>>(w.cell_fill, w.cell_start);
-            NRPN_LAUNCH_CHECK();
-            NRPN_CUDA_TRY(cudaMemsetAsync(w.cell_fill, 0, (size_t)kBinCells * 4, st));
-            NRPN_CUDA_TRY(cudaMemsetAsync(filed, 0, 4, st));
-        }
         for (int cb = 0; cb < n; cb += chunk) {
             const int cn = n - cb < chunk ? n - cb : chunk;
             const int Wc = ceil_div(cn, 64);
-            if (binned) {
-                nms_bin_file_kernel<<<8, 256, 0, st>>>(w.kept_pos, w.state, filed, w.box_cell, w.prep, w.sgroup, w.cell_start, w.cell_fill, w.cell_recs);
-                NRPN_LAUNCH_CHECK();
-                nms_bin_filed_kernel<<<1, 1, 0, st>>>(w.state, filed);
-                NRPN_LAUNCH_CHECK();
-                nms_cross_binned_kernel<<<ceil_div(cn, 8), 256, 0, st>>>(w.prep, w.sgroup, box_dim, thr, thr_m, ignore_group, cb, cn, w.grid,
-                                                                         w.cell_start, w.cell_fill, w.cell_recs, w.removed0);
-            } else
             nms_cross_kernel<<<ceil_div(cn, 8), 256, 0, st>>>(w.prep, w.sgroup, box_dim, thr, thr_m, ignore_group, cb, cn,
-                                                                     w.kept_pos, w.state, w.removed0);
+                                                              w.kept_pos, w.state, w.removed0);
             NRPN_LAUNCH_CHECK();
             nms_mask_kernel<<<dim3(Wc, Wc), kMaskThreads, 0, st>>>(w.prep + (size_t)cb * kPrepFloats, w.sgroup + cb, cn, Wc, box_dim, thr, thr_m,
                                                         ignore_group, w.mask);

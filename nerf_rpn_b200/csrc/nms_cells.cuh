@@ -1,11 +1,11 @@
 // Cell-list greedy NMS for tens of thousands to millions of boxes (BASELINE config 5: utils.py:215-265 at 1 k .. 1 M proposals).
-// Included by nms.cu inside namespace nrpn (uses its BinGrid, prepared records and culls).
+// Included by nms.cu inside namespace nrpn (uses its prepared records and culls).
 //
 // The greedy loop "keep the best remaining box, drop what it overlaps" decides box i from the boxes j that score higher AND overlap it:
 //     i is dropped  <=>  some such j is kept.
 // That is a dependency graph, not a sequence.  This path resolves it without walking the boxes one chunk after another:
-//   * boxes are sorted by score once (position = rank; groups only filter pairs) and assigned to the cells of the uniform grid per volume
-//     class that the chunked path already uses (BinGrid);
+//   * boxes are sorted by score once (position = rank; groups only filter pairs) and assigned to the cells of a uniform grid per volume
+//     class (BinGrid, below);
 //   * positions are processed in a handful of LEVELS [b, e) of geometrically growing size.  Per level
 //       (1) cross:      every box of the level is tested against the KEPT boxes of the earlier levels (early exit on the first hit);
 //       (2) adjacency:  the survivors are tested against each other; hits (j before i) go to a short per-box list;
@@ -16,8 +16,106 @@
 //     their circles / z ranges can reach -- stored cell by cell, so a window row is one contiguous range -- one record per thread, and
 //     every thread loops over the queries: cheap necessary conditions first, the exact polygon clip only on full warps of queued pairs.
 // Every decision is the exact IoU of the sequential loop (same operand order), so the keep set is the reference's bit for bit; the
-// chunked path stays as the fallback for what this path declines (adjacency overflow, thr < 0, stream capture).
+// chunked path stays as the fallback for what this path declines (adjacency overflow, round cap, thr < 0, stream capture).
 
+// ---- the grid
+// Whether box j can suppress box k is bounded by two necessary conditions that can be INDEXED: (a) their volumes are within a factor 1 / thr_m
+// of each other (IoU <= min V / max V), (b) their bounding circles and z ranges intersect.  Boxes are therefore filed in a uniform grid per
+// volume class -- class width log2(1 / thr_m), so partners sit in the same or an adjacent class; cells half of the class's largest diameter /
+// depth -- and a box only visits the cells its circle and z range can reach in its three classes.  Every candidate still goes through the
+// same culls and exact polygon clip.
+constexpr int kBinClasses = 16;
+constexpr int kBinMaxXY = 32, kBinMaxZ = 16;
+constexpr int kBinCellsPerClass = kBinMaxXY * kBinMaxXY * kBinMaxZ;
+constexpr int kBinCells = kBinClasses * kBinCellsPerClass + 1;      // + one cell for boxes the culls cannot reason about (visited by everyone)
+constexpr int kBinStatWords = 8 + 2 * kBinClasses;
+
+struct BinGrid {
+    float x0, y0, z0, lv0, inv_lw;       // origin of the box centres, log2-volume origin, 1 / class width
+    int n_cls;
+    float S[kBinClasses], Sz[kBinClasses], rmax[kBinClasses], dmax[kBinClasses];
+    int nx[kBinClasses], ny[kBinClasses], nz[kBinClasses];
+};
+
+__device__ __forceinline__ float ordered_to_float(unsigned u) { return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u); }
+__device__ __forceinline__ int bin_clampi(int v, int n) { return v < 0 ? 0 : (v >= n ? n - 1 : v); }
+
+// pass 0 (pass == 0): min / max of centre x, y, z and of log2(volume) over the cullable boxes.  pass 1: per-class max radius / depth.
+__global__ void nms_bin_stats_kernel(const float* __restrict__ prep, int n, int pass, const BinGrid* __restrict__ grid, unsigned* __restrict__ st) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    const float* t = prep + (size_t)p * kPrepFloats + 8;
+    if (!__float_as_int(t[7])) return;
+    const float zc = 0.5f * (t[2] + t[3]), lv = log2f(t[1]);
+    if (pass == 0) {
+        atomicMin(&st[0], float_to_ordered(t[4])); atomicMax(&st[1], float_to_ordered(t[4]));
+        atomicMin(&st[2], float_to_ordered(t[5])); atomicMax(&st[3], float_to_ordered(t[5]));
+        atomicMin(&st[4], float_to_ordered(zc)); atomicMax(&st[5], float_to_ordered(zc));
+        atomicMin(&st[6], float_to_ordered(lv)); atomicMax(&st[7], float_to_ordered(lv));
+    } else {
+        int c = (int)floorf((lv - grid->lv0) * grid->inv_lw);
+        c = c < 0 ? 0 : (c >= grid->n_cls ? grid->n_cls - 1 : c);
+        atomicMax(&st[8 + c], float_to_ordered(t[6]));
+        atomicMax(&st[8 + kBinClasses + c], float_to_ordered(t[3] - t[2]));
+    }
+}
+
+__global__ void nms_bin_stats_init_kernel(unsigned* __restrict__ st) {
+    const int t = threadIdx.x;
+    if (t < kBinStatWords) st[t] = (t < 8 && !(t & 1)) ? 0xFFFFFFFFu : 0u;          // mins start at +max, maxes at the lowest key
+}
+
+// stage 0: class mapping from the global extents; stage 1: per-class cell sizes / counts from the per-class maxima
+__global__ void nms_bin_grid_kernel(const unsigned* __restrict__ st, float thr_m, int stage, BinGrid* __restrict__ g) {
+    if (threadIdx.x != 0) return;
+    if (stage == 0) {
+        const bool any = st[0] != 0xFFFFFFFFu;
+        g->x0 = any ? ordered_to_float(st[0]) : 0.f; g->y0 = any ? ordered_to_float(st[2]) : 0.f; g->z0 = any ? ordered_to_float(st[4]) : 0.f;
+        g->lv0 = any ? ordered_to_float(st[6]) : 0.f;
+        const float span = any ? ordered_to_float(st[7]) - g->lv0 : 0.f;
+        float width = (thr_m > 0.f && thr_m < 1.f) ? log2f(1.0f / thr_m) : 1e30f;        // no ratio cull: a single class
+        if (span / width > (float)(kBinClasses - 1)) width = span / (float)(kBinClasses - 1) * 1.0001f;   // wider classes stay conservative
+        g->inv_lw = 1.0f / width;
+        int nc = (int)floorf(span * g->inv_lw) + 1;
+        g->n_cls = nc < 1 ? 1 : (nc > kBinClasses ? kBinClasses : nc);
+        return;
+    }
+    const float ex = ordered_to_float(st[1]) - g->x0, ey = ordered_to_float(st[3]) - g->y0, ez = ordered_to_float(st[5]) - g->z0;
+    for (int c = 0; c < kBinClasses; ++c) {
+        const float r = st[8 + c] ? ordered_to_float(st[8 + c]) : 0.f, d = st[8 + kBinClasses + c] ? ordered_to_float(st[8 + kBinClasses + c]) : 0.f;
+        g->rmax[c] = r; g->dmax[c] = d;
+        // cells half of the class's largest diameter / depth wide: a query window of +-(r_j + r_c) / S cells then hugs the volume that can
+        // hold a partner (3 x 3 cells of size 2 r_c would cover 3x that area) while a box still visits only ~100 cells per class
+        float S = fmaxf(r, fmaxf(ex, ey) / (float)kBinMaxXY * 1.0001f);
+        float Sz = fmaxf(0.5f * d, ez / (float)kBinMaxZ * 1.0001f);
+        if (!(S > 0.f)) S = 1.0f;
+        if (!(Sz > 0.f)) Sz = 1.0f;
+        g->S[c] = S; g->Sz[c] = Sz;
+        int nx = (int)floorf(ex / S) + 1, ny = (int)floorf(ey / S) + 1, nz = (int)floorf(ez / Sz) + 1;
+        g->nx[c] = nx < 1 ? 1 : (nx > kBinMaxXY ? kBinMaxXY : nx);
+        g->ny[c] = ny < 1 ? 1 : (ny > kBinMaxXY ? kBinMaxXY : ny);
+        g->nz[c] = nz < 1 ? 1 : (nz > kBinMaxZ ? kBinMaxZ : nz);
+    }
+}
+
+// cell of every box (kBinCells - 1 = the "everywhere" cell of boxes without a usable cull record)
+__global__ void nms_bin_assign_kernel(const float* __restrict__ prep, int n, const BinGrid* __restrict__ g, int* __restrict__ box_cell) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    const float* t = prep + (size_t)p * kPrepFloats + 8;
+    int cell = kBinCells - 1;
+    if (__float_as_int(t[7])) {
+        int c = (int)floorf((log2f(t[1]) - g->lv0) * g->inv_lw);
+        c = bin_clampi(c, g->n_cls);
+        const int ix = bin_clampi((int)floorf((t[4] - g->x0) / g->S[c]), g->nx[c]);
+        const int iy = bin_clampi((int)floorf((t[5] - g->y0) / g->S[c]), g->ny[c]);
+        const int iz = bin_clampi((int)floorf((0.5f * (t[2] + t[3]) - g->z0) / g->Sz[c]), g->nz[c]);
+        cell = c * kBinCellsPerClass + (iz * kBinMaxXY + iy) * kBinMaxXY + ix;
+    }
+    box_cell[p] = cell;
+}
+
+// ---- the cell lists
 constexpr int kAdjSlots = 32;             // inline predecessors per box; more -> fallback
 constexpr int kQB = 256;                  // queries per work item
 constexpr int kPairThreads = 256;
@@ -428,15 +526,31 @@ __global__ void __launch_bounds__(1024) cl_keep_emit_kernel(const signed char* _
 }
 
 struct CellWs {
+    BinGrid* grid;       // grid parameters
+    unsigned* bstats;    // kBinStatWords: reduction scratch of the grid (ordered-uint min / max)
+    int* box_cell;       // n: cell of every box
     signed char* state; int* adj_cnt; int* adj;
     CellIndex A, B;
     unsigned long long* totals; int* meta; int* und; int* fail; int* blk;
 };
 
+// the grid of the n prepared records: extents -> volume classes -> per-class cell sizes -> cell of every box
+static int cl_build_grid(const CellWs& c, const float* prep, int n, float thr_m, cudaStream_t st) {
+    nms_bin_stats_init_kernel<<<1, 64, 0, st>>>(c.bstats);
+    nms_bin_stats_kernel<<<ceil_div(n, 256), 256, 0, st>>>(prep, n, 0, c.grid, c.bstats);
+    nms_bin_grid_kernel<<<1, 32, 0, st>>>(c.bstats, thr_m, 0, c.grid);
+    nms_bin_stats_kernel<<<ceil_div(n, 256), 256, 0, st>>>(prep, n, 1, c.grid, c.bstats);
+    nms_bin_grid_kernel<<<1, 32, 0, st>>>(c.bstats, thr_m, 1, c.grid);
+    NRPN_LAUNCH_CHECK();
+    nms_bin_assign_kernel<<<ceil_div(n, 256), 256, 0, st>>>(prep, n, c.grid, c.box_cell);
+    NRPN_LAUNCH_CHECK();
+    return NRPN_OK;
+}
+
 static void cl_build_index(const CellIndex& X, const CellWs& c, const NmsWs& w, int b, int e, int want, bool with_items, cudaStream_t st) {
-    if (e > b) cl_count_kernel<<<ceil_div(e - b, 256), 256, 0, st>>>(c.state, w.box_cell, b, e, want, X.cursor);
+    if (e > b) cl_count_kernel<<<ceil_div(e - b, 256), 256, 0, st>>>(c.state, c.box_cell, b, e, want, X.cursor);
     cl_scan_local_kernel<<<kScanBlocks, kScanTile, 0, st>>>(X.cursor, X.start, X.item_start, c.totals);
     cl_scan_add_kernel<<<kScanBlocks, kScanTile, 0, st>>>(X.start, X.item_start, c.totals, c.meta);
     if (with_items) cl_items_kernel<<<ceil_div(kBinCells, 256), 256, 0, st>>>(X.item_start, X.items);
-    if (e > b) cl_scatter_kernel<<<ceil_div(e - b, 256), 256, 0, st>>>(c.state, w.box_cell, w.prep, w.sgroup, b, e, want, X.start, X.cursor, X.recs);
+    if (e > b) cl_scatter_kernel<<<ceil_div(e - b, 256), 256, 0, st>>>(c.state, c.box_cell, w.prep, w.sgroup, b, e, want, X.start, X.cursor, X.recs);
 }

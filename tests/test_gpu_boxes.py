@@ -119,7 +119,7 @@ def test_nms_chunked_path_large_inputs(ops):
     """BASELINE config 5 sizes (beyond the 32 768-box bit-matrix path): exact against the oracle at 40k-70k boxes,
     size-independent properties at 300k (sorted by score, idempotent, kept set pairwise below the threshold)."""
     rng = np.random.default_rng(17)
-    for n, dim, ext, ngroups in ((40000, 7, 200.0, 1), (50000, 7, 160.0, 4), (70000, 6, 260.0, 1), (66000, 7, 130.0, 1), (72000, 7, 180.0, 3)):   # >= 65 536: binned kept-box index
+    for n, dim, ext, ngroups in ((40000, 7, 200.0, 1), (50000, 7, 160.0, 4), (70000, 6, 260.0, 1), (66000, 7, 130.0, 1), (72000, 7, 180.0, 3)):   # >= 12 288: cell-list path
         boxes = rand_obb(n, rng, ext, 3, 24) if dim == 7 else rand_aabb(n, rng, ext, 3, 28)
         if dim == 7:
             boxes[:, 2] = rng.random(n) * ext * 0.625
@@ -143,9 +143,9 @@ def test_nms_chunked_path_large_inputs(ops):
 
 
 def test_nms_cell_list_path_equals_chunked_kept_list_scan(ops, tmp_path):
-    """n >= 16 384 runs the cell-list path (levels: cross against the kept boxes, adjacency among the survivors, dependency rounds); the keep
-    list must equal the plain chunk-by-chunk kept-list scan (NRPN_NMS_CELLS=0 NRPN_NMS_BINNED=0, read when the library initialises: run in a
-    second process) at 300 000 boxes, 2 groups, 40 degenerate boxes."""
+    """n >= 12 288 runs the cell-list path (levels: cross against the kept boxes, adjacency among the survivors, dependency rounds); the keep
+    list must equal the plain chunk-by-chunk kept-list scan (NRPN_NMS_CELLS=0, read when the library initialises: run in a second process)
+    at 300 000 boxes, 2 groups, 40 degenerate boxes."""
     import subprocess, sys, textwrap
     rng = np.random.default_rng(23)
     n = 300000
@@ -166,7 +166,7 @@ def test_nms_cell_list_path_equals_chunked_kept_list_scan(ops, tmp_path):
         k, nk = ops.nms_device(torch.from_numpy(d['boxes']).cuda(), torch.from_numpy(d['scores']).cuda(), torch.from_numpy(d['groups']).cuda(), 0.3)
         np.save({str(tmp_path / 'ref.npy')!r}, k[: int(nk.item())].cpu().numpy())
     """)
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=900, env={**os.environ, "NRPN_NMS_BINNED": "0", "NRPN_NMS_CELLS": "0"})
+    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=900, env={**os.environ, "NRPN_NMS_CELLS": "0"})
     assert r.returncode == 0, r.stderr[-2000:]
     ref = np.load(str(tmp_path / "ref.npy"))
     assert 1000 < ref.shape[0] < n
@@ -175,7 +175,8 @@ def test_nms_cell_list_path_equals_chunked_kept_list_scan(ops, tmp_path):
 
 def test_nms_cell_list_path_declines_crowds_and_handles_ties(ops):
     """More than 32 higher-scored overlapping survivors per box overflow the inline predecessor lists: the path must hand over to the chunked
-    one (same keep set as the oracle).  Exact score ties and long suppression chains stay on the cell-list path."""
+    one (same keep set as the oracle), with 1 024-box chunks at 20 000 boxes and 4 096-box chunks at 70 000.  Exact score ties and long
+    suppression chains stay on the cell-list path."""
     rng = np.random.default_rng(29)
     base = rand_obb(40, rng, 120.0, 8, 20)
     crowd = np.repeat(base, 500, axis=0) + rng.normal(0, 0.05, (20000, 7)).astype(np.float32)      # 500 near-copies of each of 40 boxes
@@ -191,6 +192,11 @@ def test_nms_cell_list_path_declines_crowds_and_handles_ties(ops):
     np.testing.assert_array_equal(run_nms(ops, chain, s2, None, 0.3), obox.nms(chain, s2, 0.3))
     groups = rng.integers(0, 3, n).astype(np.int32)
     np.testing.assert_array_equal(run_nms(ops, chain, s2, groups, 0.3), obox.batched_nms(chain, s2, groups, 0.3))
+    base = rand_obb(140, rng, 180.0, 8, 20)                     # a crowd above 65 536 boxes: 500 near-copies of each of 140 boxes
+    crowd = np.repeat(base, 500, axis=0) + rng.normal(0, 0.05, (70000, 7)).astype(np.float32)
+    crowd[:, 3:6] = np.abs(crowd[:, 3:6])
+    scores = rng.random(70000).astype(np.float32)
+    np.testing.assert_array_equal(run_nms(ops, crowd, scores, None, 0.3), obox.nms(crowd, scores, 0.3))
 
 
 def test_nms_geometric_cull_modes_stay_within_a_few_boxes_of_the_exact_set(ops):

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Diagnostic: the keep list of one config-5 input (n boxes) from every NMS path (cell lists / chunked + binned index / plain chunked) with the
-cull modes 0 / 1 / 3, each in its own process (the switches are read once per process)."""
+"""Diagnostic: the keep list of one config-5 input (n boxes) from both NMS paths for large inputs (cell lists / plain chunked kept-list scan)
+with the cull modes 0 / 1 / 3, each in its own process (the switches are read once per process)."""
 import json
 import os
 import subprocess
@@ -28,7 +28,7 @@ code = textwrap.dedent(f"""
 import numpy as np
 res = {}
 os.makedirs("gpurun_out", exist_ok=True)
-for name, env in (("cells", {}), ("binned", {"NRPN_NMS_CELLS": "0"}), ("plain", {"NRPN_NMS_CELLS": "0", "NRPN_NMS_BINNED": "0"})):
+for name, env in (("cells", {}), ("plain", {"NRPN_NMS_CELLS": "0"})):
     for lens in ("0", "1", "3"):
         key = f"{name}_mode{lens}"
         out = f"gpurun_out/_paths_{key}.npy"
@@ -40,4 +40,7 @@ for name, env in (("cells", {}), ("binned", {"NRPN_NMS_CELLS": "0"}), ("plain", 
 base = res.get("plain_mode0")
 for k, v in res.items():
     same = v.shape == base.shape and bool((v == base).all())
-    print(f"{k}: kept {v.shape[0]}  == plain_mode0: {same}  only_here {np.setdiff1d(v, base)[:8].tolist()}  missing {np.setdiff1d(base, v)[:8].tolist()}")
+    plain = res.get("plain_" + k.split("_")[1])
+    same_mode = plain is not None and v.shape == plain.shape and bool((v == plain).all())
+    print(f"{k}: kept {v.shape[0]}  == plain_mode0: {same}  == plain, same mode: {same_mode}  only_here {np.setdiff1d(v, base)[:8].tolist()}  "
+          f"missing {np.setdiff1d(base, v)[:8].tolist()}")
