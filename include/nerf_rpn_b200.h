@@ -118,9 +118,12 @@ typedef struct {
     int32_t xi, yi, zi; /* input extent */
     int32_t xo, yo, zo; /* output extent */
     int32_t xr, yr, zr; /* residual extent (ignored when res == NULL) */
-    int32_t ldy;        /* output row pitch in elements */
-    int32_t ldr;        /* residual row pitch in elements */
+    int32_t ldy;        /* output row pitch in elements, >= cout, % 8 == 0 */
+    int32_t ldr;        /* residual row pitch in elements, >= cout, % 8 == 0 */
 } nrpn_conv_level;
+/* Alignment: y must be aligned to one output channel pair (4 bytes for 16-bit, 8 bytes for fp32 y), res to 4 bytes and
+ * shift to 8 bytes; otherwise nrpn_conv3d_fprop returns NRPN_ERR_INVALID before any launch.  Split-K (see
+ * nrpn_conv3d_workspace_bytes) also needs y, res and shift 16-byte aligned: a layer whose pointers are not runs unsplit. */
 
 typedef struct {
     int32_t cin, cout;              /* cin % 64 == 0 */

@@ -408,6 +408,17 @@ static int choose_splits(int total_tiles, int kblocks, bool short_k) {
     return s < 2 ? 1 : s;
 }
 
+// The split-K fix-up moves 8 channels at a time as 16-byte vectors of y, res and shift: their base pointers must be 16-byte
+// aligned (row pitches are multiples of 8 elements).  A layer whose pointers are not runs unsplit, as without a workspace.
+static bool splitk_aligned(const nrpn_conv_desc* d) {
+    if (reinterpret_cast<uintptr_t>(d->shift) % 16 != 0) return false;
+    for (int l = 0; l < d->n_levels; ++l) {
+        const nrpn_conv_level& S = d->level[l];
+        if (reinterpret_cast<uintptr_t>(S.y) % 16 != 0 || reinterpret_cast<uintptr_t>(S.res) % 16 != 0) return false;
+    }
+    return true;
+}
+
 struct ConvGeom { int pad_n, cout_pad, block_n, kblocks, m_tiles, n_tiles_n, splits; bool short_k, tma_epi; size_t ws_bytes, counter_bytes; };
 
 static int conv_geometry(const nrpn_conv_desc* d, ConvGeom& g) {
@@ -430,7 +441,7 @@ static int conv_geometry(const nrpn_conv_desc* d, ConvGeom& g) {
     // tile runs a long reduction.  Two remedies: split-K over the full-width tiles (opt-in, NRPN_SPLITK=1, decided first so that it
     // reaches the layers it is meant for), otherwise -- the default -- 64-wide tiles when even those fit in one wave: 4x the CTAs
     // (same reduction order per output element, bit-identical results).
-    g.splits = d->wsplit ? 1 : choose_splits(tiles * g.n_tiles_n, g.kblocks, g.short_k);
+    g.splits = (d->wsplit || !splitk_aligned(d)) ? 1 : choose_splits(tiles * g.n_tiles_n, g.kblocks, g.short_k);
     if (g.splits == 1 && !g.short_k && g.block_n > 64 && tiles * (g.cout_pad / 64) <= num_sms()) {
         const char* e = getenv("NRPN_CONV_NARROW");
         if (!(e && e[0] == '0')) { g.block_n = 64; g.n_tiles_n = g.cout_pad / 64; }
@@ -469,6 +480,7 @@ int nrpn_conv3d_block_n(int cout) { return cout <= 64 ? 64 : (cout <= 128 ? 128 
 const char* nrpn_conv3d_variant(const nrpn_conv_desc* d) {
     if (!d || d->n_taps < 1 || d->n_taps > NRPN_CONV_MAX_TAPS || d->n_levels < 1 || d->n_levels > NRPN_CONV_MAX_LEVELS) return "invalid";
     if (d->cin < 64 || d->cin % 64 != 0 || d->cout < 8 || d->cout % 8 != 0 || (d->stride != 1 && d->stride != 2)) return "unsupported";
+    if (!conv_pairs_aligned(d)) return "invalid";
     if (!d->wsplit && conv3d_slab_eligible(d)) return "slab<4x16x8,N64>";
     ConvGeom g;
     if (conv_geometry(d, g) != NRPN_OK) return "invalid";
@@ -490,6 +502,7 @@ int nrpn_conv3d_fprop(const nrpn_conv_desc* d, nrpn_stream_t stream) {
         for (int t = 0; t < d->n_taps; ++t)
             if (d->tap_off[t][0] || d->tap_off[t][1] || d->tap_off[t][2]) return NRPN_ERR_UNSUPPORTED;
     }
+    if (!conv_pairs_aligned(d)) return NRPN_ERR_INVALID;
     EncodeTiledFn encode = get_encode();
     if (!encode) return NRPN_ERR_NO_DEVICE;
     if (!d->wsplit && conv3d_slab_eligible(d)) return conv3d_slab_launch(d, (cudaStream_t)stream);

@@ -271,7 +271,7 @@ int conv3d_slab_launch(const nrpn_conv_desc* d, cudaStream_t st) {
     if (!slab_plan(d, P)) return NRPN_ERR_UNSUPPORTED;
     const nrpn_conv_level& S = d->level[0];
     if (!S.x || !S.y || S.n < 1 || S.xo < 1 || S.yo < 1 || S.zo < 1) return NRPN_ERR_INVALID;
-    if (S.ldy < d->cout || S.ldy % 8 != 0) return NRPN_ERR_INVALID;
+    if (S.ldy < d->cout || S.ldy % 8 != 0 || !conv_pairs_aligned(d)) return NRPN_ERR_INVALID;
     EncodeTiledFn encode = get_encode();
     if (!encode) return NRPN_ERR_NO_DEVICE;
     P.n = S.n; P.xo = S.xo; P.yo = S.yo; P.zo = S.zo;

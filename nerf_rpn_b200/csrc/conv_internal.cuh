@@ -43,6 +43,17 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
+// The epilogues store an output channel pair as one 4-byte (16-bit y) or 8-byte (fp32 y) word, and load a residual pair as one
+// 4-byte word and a shift pair as one 8-byte word.  Row pitches are multiples of 8 elements, so aligned base pointers suffice.
+inline bool conv_pairs_aligned(const nrpn_conv_desc* d) {
+    if (reinterpret_cast<uintptr_t>(d->shift) % 8 != 0) return false;
+    for (int l = 0; l < d->n_levels; ++l) {
+        const nrpn_conv_level& S = d->level[l];
+        if (reinterpret_cast<uintptr_t>(S.y) % (d->out_fp32 ? 8 : 4) != 0 || reinterpret_cast<uintptr_t>(S.res) % 4 != 0) return false;
+    }
+    return true;
+}
+
 // conv3d_slab.cu: halo-slab kernel for 64 -> (<=64)-channel stride-1 convolutions with a full box of filter taps.
 // Returns true when the descriptor is of that shape (the caller then launches it with conv3d_slab_launch).
 bool conv3d_slab_eligible(const nrpn_conv_desc* d);

@@ -1,5 +1,7 @@
 """Pure-torch statement of what nrpn_conv3d_fprop / nrpn_pack_stem_input compute (TEST helper, CPU or GPU).
-Used to check the host-side packing logic without a GPU and as the fp32 reference for the CUDA kernels."""
+Used to check the host-side packing logic without a GPU and as the fp32 / float64 references for the CUDA kernels."""
+import math
+
 import torch
 import torch.nn.functional as F
 
@@ -37,6 +39,63 @@ def emulate_conv(x, w_packed, taps, shift, out_dims, stride=1, relu=False, res=N
     if relu:
         out = out.clamp_min(0)
     return out
+
+
+def nearest_source_index(out_size: int, in_size: int, device=None) -> torch.Tensor:
+    """Source index of each output index of a nearest up-sampling from in_size to out_size, as the kernel (row_pos) and
+    F.interpolate(mode='nearest', size=...) compute it: min(floor(float32(o) * float32(in / out)), in - 1), all in float32.
+    A float64 ratio can pick a different voxel (in 14 -> out 46: output 23 takes voxel 6, not 7)."""
+    scale = torch.tensor(float(in_size), dtype=torch.float32) / torch.tensor(float(out_size), dtype=torch.float32)
+    idx = torch.floor(torch.arange(out_size, dtype=torch.float32) * scale).to(torch.int64).clamp_max(in_size - 1)
+    return idx.to(device)
+
+
+def reference_conv64(x, w, taps, shift, out_dims, stride=1, act=0, res=None):
+    """float64 statement of nrpn_conv3d_fprop on the exact operands the kernel reads (CPU or GPU).
+
+    x (N,X,Y,Z,Cin) 16-bit; w the packed weights, (taps,CoutPad,Cin) or wsplit (taps,2,CoutPad,Cin) whose hi + lo planes are
+    summed in float64; shift (CoutPad) fp32; res None or (N,Xr,Yr,Zr,C) 16-bit, nearest-upsampled when its extent differs from
+    out_dims and added to the first C channels; act 0 none, 1 ReLU, 2 exact (erf) GELU.
+    Returns (ref, mag), float64 (N,Xo,Yo,Zo,CoutPad): ref the result; mag the same sum taken over the absolute value of every
+    term (|x|.|w| products, |shift|, |res|, before the activation) -- the scale of the rounding error of a float accumulation."""
+    dev = x.device
+    x = x.double()
+    w = w.double()
+    wabs = w.abs()
+    if w.dim() == 4:
+        w, wabs = w[:, 0] + w[:, 1], wabs[:, 0] + wabs[:, 1]
+    n, X, Y, Z, cin = x.shape
+    out_dims = tuple(int(v) for v in out_dims)
+    P = max(max(abs(int(v)) for v in t) for t in taps)
+    hi = [max(0, P + (o - 1) * stride + 1 - i) for o, i in zip(out_dims, (X, Y, Z))]
+    xp = F.pad(x, (0, 0, P, hi[2], P, hi[1], P, hi[0]))
+    xa = xp.abs()
+    ref = torch.zeros((n, *out_dims, w.shape[1]), dtype=torch.float64, device=dev)
+    mag = torch.zeros_like(ref)
+    xo, yo, zo = out_dims
+    for t, (dx, dy, dz) in enumerate(taps):
+        ix = slice(P + dx, P + dx + (xo - 1) * stride + 1, stride)
+        iy = slice(P + dy, P + dy + (yo - 1) * stride + 1, stride)
+        iz = slice(P + dz, P + dz + (zo - 1) * stride + 1, stride)
+        ref += xp[:, ix, iy, iz] @ w[t].t()
+        mag += xa[:, ix, iy, iz] @ wabs[t].t()
+    s = shift.to(dev).double()
+    ref += s
+    mag += s.abs()
+    if res is not None:
+        r = res.double()
+        if tuple(r.shape[1:4]) != out_dims:
+            r = r[:, nearest_source_index(xo, r.shape[1], dev)]
+            r = r[:, :, nearest_source_index(yo, r.shape[2], dev)]
+            r = r[:, :, :, nearest_source_index(zo, r.shape[3], dev)]
+        c = r.shape[-1]
+        ref[..., :c] += r
+        mag[..., :c] += r.abs()
+    if act == 1:
+        ref = ref.clamp_min(0)
+    elif act == 2:
+        ref = 0.5 * ref * (1.0 + torch.erf(ref / math.sqrt(2.0)))
+    return ref, mag
 
 
 def emulate_pack_stem_s1(grid: torch.Tensor) -> torch.Tensor:
