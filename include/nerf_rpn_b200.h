@@ -122,8 +122,7 @@ typedef struct {
     int32_t ldr;        /* residual row pitch in elements, >= cout, % 8 == 0 */
 } nrpn_conv_level;
 /* Alignment: y must be aligned to one output channel pair (4 bytes for 16-bit, 8 bytes for fp32 y), res to 4 bytes and
- * shift to 8 bytes; otherwise nrpn_conv3d_fprop returns NRPN_ERR_INVALID before any launch.  Split-K (see
- * nrpn_conv3d_workspace_bytes) also needs y, res and shift 16-byte aligned: a layer whose pointers are not runs unsplit. */
+ * shift to 8 bytes; otherwise nrpn_conv3d_fprop returns NRPN_ERR_INVALID before any launch. */
 
 typedef struct {
     int32_t cin, cout;              /* cin % 64 == 0 */
@@ -136,8 +135,6 @@ typedef struct {
     const float *shift;             /* fp32 (CoutPad) */
     int32_t n_levels;
     nrpn_conv_level level[NRPN_CONV_MAX_LEVELS];
-    void *workspace;                /* optional split-K scratch (see nrpn_conv3d_workspace_bytes) or NULL */
-    size_t workspace_bytes;
     int32_t act_fp16;               /* 16-bit format of x / w / res / 16-bit y: 0 = bf16, 1 = fp16 (IEEE half) */
     int32_t wsplit;                 /* 1: w is (taps, 2, CoutPad, cin) = every weight as the sum hi + lo of two 16-bit numbers (both
                                      * planes are multiplied with the same activation tile into one fp32 accumulator): the weights
@@ -149,12 +146,6 @@ int nrpn_conv3d_block_n(int cout);
 /* Name of the kernel variant nrpn_conv3d_fprop would launch for this descriptor ("slab<4x16x8,N64>", "igemm<256,4,1>", ...;
  * "invalid" / "unsupported" when it would be rejected).  Pure host logic: pointers inside the descriptor are not dereferenced. */
 const char *nrpn_conv3d_variant(const nrpn_conv_desc *desc);
-/* Layers with few output tiles and a long reduction are split along K over several CTAs; each stores its partial tile
- * into its own fp32 slab and the last CTA to arrive sums the slabs in a fixed order (bit-reproducible).  Returns the
- * bytes such a layer wants (0: the layer is not split).  The first 256-byte-aligned counters region must be zero-filled
- * ONCE by the caller (simplest: zero the whole buffer); every launch leaves the counters at zero, so one buffer can serve
- * all layers of a stream.  Passing workspace == NULL (or too small) is legal: the layer then runs unsplit. */
-size_t nrpn_conv3d_workspace_bytes(const nrpn_conv_desc *desc /*host*/);
 int nrpn_conv3d_fprop(const nrpn_conv_desc *desc /*host*/, nrpn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------

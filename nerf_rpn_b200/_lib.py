@@ -28,8 +28,8 @@ class ConvDesc(ctypes.Structure):
     _fields_ = [("cin", ctypes.c_int32), ("cout", ctypes.c_int32), ("n_taps", ctypes.c_int32),
                 ("tap_off", (ctypes.c_int8 * 3) * MAX_TAPS), ("stride", ctypes.c_int32), ("relu", ctypes.c_int32),
                 ("out_fp32", ctypes.c_int32), ("w", ctypes.c_void_p), ("shift", ctypes.c_void_p),
-                ("n_levels", ctypes.c_int32), ("level", ConvLevel * MAX_LEVELS), ("workspace", ctypes.c_void_p),
-                ("workspace_bytes", ctypes.c_size_t), ("act_fp16", ctypes.c_int32), ("wsplit", ctypes.c_int32)]
+                ("n_levels", ctypes.c_int32), ("level", ConvLevel * MAX_LEVELS), ("act_fp16", ctypes.c_int32),
+                ("wsplit", ctypes.c_int32)]
 
 
 class RpnLevel(ctypes.Structure):
@@ -110,7 +110,6 @@ _SIGNATURES = {
                                 ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, c_stream]),
     "nrpn_conv3d_block_n": (ctypes.c_int, [ctypes.c_int]),
     "nrpn_conv3d_variant": (ctypes.c_char_p, [ctypes.POINTER(ConvDesc)]),
-    "nrpn_conv3d_workspace_bytes": (ctypes.c_size_t, [ctypes.POINTER(ConvDesc)]),
     "nrpn_conv3d_fprop": (ctypes.c_int, [ctypes.POINTER(ConvDesc), c_stream]),
     "nrpn_conv3d_wgrad_workspace_bytes": (ctypes.c_size_t, [ctypes.POINTER(WgradDesc)]),
     "nrpn_conv3d_wgrad": (ctypes.c_int, [ctypes.POINTER(WgradDesc), c_stream]),

@@ -22,7 +22,7 @@
 //     top-down path), ReLU / GELU, convert to bf16 / fp16 / fp32; or -- TMA_EPI variant of the 1^3 layers -- residual tiles
 //     prefetched by TMA into shared memory and output tiles stored with cp.async.bulk.tensor.
 //   - variants: <256,4,1> <128,6,1> <64,8,1> (long reductions; <64,8,1> also for layers with fewer tiles than SMs),
-//     <64,2,3> / <64,2,2,TMA_EPI> (reductions of at most 8 k-blocks), optional split-K (NRPN_SPLITK=1, off by default).
+//     <64,2,3> / <64,2,2,TMA_EPI> (reductions of at most 8 k-blocks).
 #include <cstdlib>
 #include <type_traits>
 #include "common.cuh"
@@ -54,9 +54,6 @@ struct ConvLevelDev {
 struct ConvDev {
     int n_levels, n_taps, kc_blocks, n_tiles_n, cout, relu, out_fp32, fp16;
     int total_m_tiles;
-    int splits, cout_pad;      // split-K: `splits` CTAs share one output tile and reduce through `ws`
-    float* ws;                 // fp32 (tiles, splits, 128, BLOCK_N) partial tiles, rewritten by every launch
-    unsigned* counters;        // one arrival counter per output tile, zero between launches
     signed char tap[NRPN_CONV_MAX_TAPS][4];
     const float* shift;
     ConvLevelDev lv[NRPN_CONV_MAX_LEVELS];
@@ -141,7 +138,6 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
     uint64_t* empty_bar = bars + STAGES;
     uint64_t* rfull_bar = bars + 2 * STAGES;
     uint64_t* rempty_bar = bars + 2 * STAGES + 2;
-    uint32_t* ticket_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
 
     const int warp = threadIdx.x >> 5;
 
@@ -157,7 +153,7 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
     __syncthreads();
     ptx::pdl_wait();                    // everything above overlapped the previous layer's tail; its outputs are visible from here
 
-    const int total_tiles = P.total_m_tiles * P.n_tiles_n * P.splits;     // work items = (output tile, k-split)
+    const int total_tiles = P.total_m_tiles * P.n_tiles_n;     // work items = output tiles
     const int kblocks = P.n_taps * P.kc_blocks;
 
     if (warp == kConsumerThreads / 32) {
@@ -165,14 +161,12 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
         const bool leader = ptx::elect_one();
         int stage = 0; uint32_t phase = 0;
         int rslot = 0; uint32_t rphase = 0;
-        for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
-            const int split = item % P.splits, tile = item / P.splits;
-            const int kb0 = (kblocks * split) / P.splits, kb1 = (kblocks * (split + 1)) / P.splits;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int n_tile = tile % P.n_tiles_n, m_tile = tile / P.n_tiles_n;
             const TilePos tp = tile_pos(P, m_tile);
             const ConvLevelDev& L = P.lv[tp.l];
             const int x0 = tp.tix * L.bx, y0 = tp.tiy * L.by, z0 = tp.tiz * L.bz, n0 = n_tile * BLOCK_N;
-            for (int kb = kb0; kb < kb1; ++kb) {
+            for (int kb = 0; kb < kblocks; ++kb) {
                 const int tap = kb / P.kc_blocks, kc = kb - tap * P.kc_blocks;
                 const int dx = P.tap[tap][0], dy = P.tap[tap][1], dz = P.tap[tap][2];
                 ptx::mbar_wait(&empty_bar[stage], phase ^ 1u);
@@ -204,9 +198,7 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
     int stage = 0; uint32_t phase = 0;
     int rslot = 0; uint32_t rphase = 0;
     float acc[BLOCK_N / 2];
-    for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
-        const int split = item % P.splits, tile = item / P.splits;
-        const int nkb = (kblocks * (split + 1)) / P.splits - (kblocks * split) / P.splits;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int n_tile = tile % P.n_tiles_n, m_tile = tile / P.n_tiles_n;
         const TilePos tp = tile_pos(P, m_tile);
         const ConvLevelDev& L = P.lv[tp.l];
@@ -214,7 +206,7 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
 
         ptx::reg_fence(acc);
         int prev = 0;
-        for (int kb = 0; kb < nkb; ++kb) {
+        for (int kb = 0; kb < kblocks; ++kb) {
             ptx::mbar_wait(&full_bar[stage], phase);
             const uint32_t sa = ptx::smem_u32(smem + stage * kStageBytes);
             const uint64_t da = ptx::make_desc_sw128(sa + (uint32_t)(wg * (kABytes / 2)));      // this warpgroup's 64 rows
@@ -240,66 +232,8 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
         }
         ptx::wgmma_wait<0>();
         ptx::reg_fence(acc);
-        if (nkb > 0 && t == 0) ptx::mbar_arrive(&empty_bar[prev]);
+        if (t == 0) ptx::mbar_arrive(&empty_bar[prev]);
 
-        if (P.splits > 1) {
-            // ---- split-K (deterministic): every CTA stores its partial tile into its own fp32 slab of the workspace with
-            // plain stores; the last CTA to arrive sums the slabs in split order and runs the normal epilogue.
-            float* slab0 = P.ws + ((size_t)tile * P.splits) * (kBlockM * BLOCK_N);          // slabs of this output tile
-            float* wslab = slab0 + (size_t)split * (kBlockM * BLOCK_N);
-#pragma unroll
-            for (int j = 0; j < BLOCK_N / 8; ++j)
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    __stcg(reinterpret_cast<float2*>(wslab + (size_t)(wg * 64 + ptx::frag_row(t, h)) * BLOCK_N + ptx::frag_col(t, j)),
-                           make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
-            __threadfence();
-            ptx::named_barrier(1, kConsumerThreads);
-            if (threadIdx.x == 0) *ticket_slot = atomicAdd(P.counters + tile, 1u);
-            ptx::named_barrier(1, kConsumerThreads);
-            const bool last = (*ticket_slot == (uint32_t)(P.splits - 1));
-            if (last && threadIdx.x < kBlockM) {
-                __threadfence();
-                const int row = threadIdx.x;                 // one accumulator row per thread
-                const RowPos rp = row_pos(L, tp, row);
-                if (rp.valid) {
-                    const float* rrow0 = slab0 + (size_t)row * BLOCK_N;
-                    for (int ch = n0; ch < n0 + BLOCK_N && ch < P.cout; ch += 8) {
-                        float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), a1 = a0;
-                        for (int sp = 0; sp < P.splits; ++sp) {                                  // fixed order => reproducible
-                            const float* wp = rrow0 + (size_t)sp * (kBlockM * BLOCK_N) + (ch - n0);
-                            const float4 b0 = __ldcg(reinterpret_cast<const float4*>(wp));
-                            const float4 b1 = __ldcg(reinterpret_cast<const float4*>(wp + 4));
-                            a0.x += b0.x; a0.y += b0.y; a0.z += b0.z; a0.w += b0.w;
-                            a1.x += b1.x; a1.y += b1.y; a1.z += b1.z; a1.w += b1.w;
-                        }
-                        const float4 s0 = __ldg(reinterpret_cast<const float4*>(P.shift + ch));
-                        const float4 s1 = __ldg(reinterpret_cast<const float4*>(P.shift + ch + 4));
-                        float v[8] = {a0.x + s0.x, a0.y + s0.y, a0.z + s0.z, a0.w + s0.w, a1.x + s1.x, a1.y + s1.y, a1.z + s1.z, a1.w + s1.w};
-                        if (rp.rrow != nullptr) {
-                            const uint4 rv4 = __ldg(reinterpret_cast<const uint4*>(rp.rrow + ch));
-                            const uint32_t* rb = reinterpret_cast<const uint32_t*>(&rv4);
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) { const float2 f = unpack_act2(rb[i], P.fp16); v[2 * i] += f.x; v[2 * i + 1] += f.y; }
-                        }
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) v[i] = activate(v[i], P.relu);
-                        if (P.out_fp32) {
-                            float* o = reinterpret_cast<float*>(L.y) + rp.vox * L.ldy + ch;
-                            *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
-                            *reinterpret_cast<float4*>(o + 4) = make_float4(v[4], v[5], v[6], v[7]);
-                        } else {
-                            __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(L.y) + rp.vox * L.ldy + ch;
-                            *reinterpret_cast<uint4*>(o) = make_uint4(pack_act2(v[0], v[1], P.fp16), pack_act2(v[2], v[3], P.fp16),
-                                                                      pack_act2(v[4], v[5], P.fp16), pack_act2(v[6], v[7], P.fp16));
-                        }
-                    }
-                }
-                if (row == 0) P.counters[tile] = 0u;
-            }
-            ptx::named_barrier(1, kConsumerThreads);         // ticket_slot is reused by the next work item
-            continue;
-        }
         if constexpr (TMA_EPI) {
             // ---- shared-memory epilogue: residual from the TMA-fed ring, output through a swizzled staging tile + TMA store
             const bool res_smem = L.res_tma != 0;
@@ -393,33 +327,7 @@ static void choose_brick(int xo, int yo, int zo, int& bx, int& by, int& bz) {
     }
 }
 
-// Split-K: layers with far fewer output tiles than SMs and a long reduction (late ResNet stages: 5x8x8 .. 10x16x16 voxels,
-// K up to 13 824) are latency bound on streaming their weights through a handful of CTAs. The kernel can spread the
-// k-blocks of each tile over `splits` CTAs (per-split fp32 slabs, last CTA reduces in a fixed order: bit-reproducible).
-// The single-CTA slab reduction is serial, so the split is OFF unless NRPN_SPLITK=1 is set; batching several scenes per
-// launch (bench.py --scenes-per-step) is what feeds these layers instead.
-static int choose_splits(int total_tiles, int kblocks, bool short_k) {
-    static const bool enabled = [] { const char* e = getenv("NRPN_SPLITK"); return e && e[0] == '1'; }();
-    if (!enabled) return 1;
-    if (short_k || kblocks < 8 || total_tiles * 2 > num_sms()) return 1;
-    int s = num_sms() / total_tiles;
-    if (s > kblocks / 4) s = kblocks / 4;
-    if (s > 32) s = 32;
-    return s < 2 ? 1 : s;
-}
-
-// The split-K fix-up moves 8 channels at a time as 16-byte vectors of y, res and shift: their base pointers must be 16-byte
-// aligned (row pitches are multiples of 8 elements).  A layer whose pointers are not runs unsplit, as without a workspace.
-static bool splitk_aligned(const nrpn_conv_desc* d) {
-    if (reinterpret_cast<uintptr_t>(d->shift) % 16 != 0) return false;
-    for (int l = 0; l < d->n_levels; ++l) {
-        const nrpn_conv_level& S = d->level[l];
-        if (reinterpret_cast<uintptr_t>(S.y) % 16 != 0 || reinterpret_cast<uintptr_t>(S.res) % 16 != 0) return false;
-    }
-    return true;
-}
-
-struct ConvGeom { int pad_n, cout_pad, block_n, kblocks, m_tiles, n_tiles_n, splits; bool short_k, tma_epi; size_t ws_bytes, counter_bytes; };
+struct ConvGeom { int pad_n, cout_pad, block_n, kblocks, m_tiles, n_tiles_n; bool short_k, tma_epi; };
 
 static int conv_geometry(const nrpn_conv_desc* d, ConvGeom& g) {
     g.pad_n = nrpn_conv3d_block_n(d->cout);
@@ -438,19 +346,15 @@ static int conv_geometry(const nrpn_conv_desc* d, ConvGeom& g) {
     }
     g.m_tiles = tiles;
     // Late ResNet stages (5x8x8 .. 10x16x16 voxels, K up to 13 824): a handful of 128 x 256 tiles leaves most SMs idle while each
-    // tile runs a long reduction.  Two remedies: split-K over the full-width tiles (opt-in, NRPN_SPLITK=1, decided first so that it
-    // reaches the layers it is meant for), otherwise -- the default -- 64-wide tiles when even those fit in one wave: 4x the CTAs
-    // (same reduction order per output element, bit-identical results).
-    g.splits = (d->wsplit || !splitk_aligned(d)) ? 1 : choose_splits(tiles * g.n_tiles_n, g.kblocks, g.short_k);
-    if (g.splits == 1 && !g.short_k && g.block_n > 64 && tiles * (g.cout_pad / 64) <= num_sms()) {
+    // tile runs a long reduction.  When even 64-wide tiles fit in one wave, they are used instead: 4x the CTAs (same reduction
+    // order per output element, bit-identical results).
+    if (!g.short_k && g.block_n > 64 && tiles * (g.cout_pad / 64) <= num_sms()) {
         const char* e = getenv("NRPN_CONV_NARROW");
         if (!(e && e[0] == '0')) { g.block_n = 64; g.n_tiles_n = g.cout_pad / 64; }
     }
-    g.counter_bytes = align_up((size_t)tiles * g.n_tiles_n * 4, 256);
-    g.ws_bytes = g.splits > 1 ? g.counter_bytes + (size_t)tiles * g.n_tiles_n * g.splits * kBlockM * g.block_n * 4 : 0;
     // shared-memory (TMA) epilogue: the HBM-bound short reductions with whole 64-channel bf16 output tiles
     { const char* e = getenv("NRPN_CONV_TMA_EPI"); g.tma_epi = !(e && e[0] == '0'); }       // A/B switch for tests and profiling
-    g.tma_epi = g.tma_epi && g.short_k && g.splits == 1 && !d->out_fp32 && d->cout % 64 == 0;
+    g.tma_epi = g.tma_epi && g.short_k && !d->out_fp32 && d->cout % 64 == 0;
     for (int l = 0; l < d->n_levels && g.tma_epi; ++l) {
         const nrpn_conv_level& S = d->level[l];
         if (reinterpret_cast<uintptr_t>(S.y) % 16 != 0 || (S.res && reinterpret_cast<uintptr_t>(S.res) % 16 != 0)) g.tma_epi = false;
@@ -467,13 +371,6 @@ using namespace nrpn;
 
 extern "C" {
 #pragma GCC visibility push(default)
-
-size_t nrpn_conv3d_workspace_bytes(const nrpn_conv_desc* d) {
-    if (!d || d->cin < 64 || d->cin % 64 != 0 || d->n_levels < 1 || d->n_levels > NRPN_CONV_MAX_LEVELS || d->n_taps < 1) return 0;
-    ConvGeom g;
-    if (conv_geometry(d, g) != NRPN_OK) return 0;
-    return g.ws_bytes;
-}
 
 int nrpn_conv3d_block_n(int cout) { return cout <= 64 ? 64 : (cout <= 128 ? 128 : 256); }
 
@@ -515,8 +412,6 @@ int nrpn_conv3d_fprop(const nrpn_conv_desc* d, nrpn_stream_t stream) {
     const int cout_pad = geo.cout_pad;
     const bool short_k = geo.short_k;
     const int block_n = geo.block_n;
-    int splits = geo.splits;
-    if (splits > 1 && (!d->workspace || d->workspace_bytes < geo.ws_bytes)) splits = 1;      // no (or too small a) workspace: run unsplit
     ConvMaps maps;
     ConvDev P;
     memset(&P, 0, sizeof(P));
@@ -589,20 +484,16 @@ int nrpn_conv3d_fprop(const nrpn_conv_desc* d, nrpn_stream_t stream) {
         if (r != CUDA_SUCCESS) { g_last_cuda_error = (int)r; return NRPN_ERR_CUDA; }
     }
     P.total_m_tiles = tiles;
-    P.splits = splits; P.cout_pad = cout_pad;
-    P.counters = reinterpret_cast<unsigned*>(d->workspace);
-    P.ws = splits > 1 ? reinterpret_cast<float*>(reinterpret_cast<char*>(d->workspace) + geo.counter_bytes) : nullptr;
-    const int total_tiles = tiles * P.n_tiles_n * splits;
+    const int total_tiles = tiles * P.n_tiles_n;
     cudaStream_t st = (cudaStream_t)stream;
     if (d->wsplit) {
-        if (splits != 1) return NRPN_ERR_UNSUPPORTED;
         if (short_k && geo.tma_epi) return launch_conv<64, 2, 2, true, true>(maps, P, total_tiles, st);
         if (short_k) return launch_conv<64, 2, 3, false, true>(maps, P, total_tiles, st);
         if (block_n == 64) return launch_conv<64, 6, 1, false, true>(maps, P, total_tiles, st);
         if (block_n == 128) return launch_conv<128, 4, 1, false, true>(maps, P, total_tiles, st);
         return launch_conv<256, 2, 1, false, true>(maps, P, total_tiles, st);
     }
-    if (short_k && geo.tma_epi && splits == 1) return launch_conv<64, 2, 2, true>(maps, P, total_tiles, st);
+    if (short_k && geo.tma_epi) return launch_conv<64, 2, 2, true>(maps, P, total_tiles, st);
     if (short_k) return launch_conv<64, 2, 3>(maps, P, total_tiles, st);
     if (block_n == 64) return launch_conv<64, 8, 1>(maps, P, total_tiles, st);
     if (block_n == 128) return launch_conv<128, 6, 1>(maps, P, total_tiles, st);

@@ -288,7 +288,7 @@ int nrpn_pack_stem_input_s1(const float* grid, int n, int x, int y, int z, void*
     return NRPN_OK;
 }
 
-int nrpn_version(void) { return 101; }
+int nrpn_version(void) { return 102; }
 
 const char* nrpn_status_string(int status) {
     switch (status) {

@@ -13,7 +13,6 @@ only the top-k candidates are decoded, and NMS never leaves the device.
 PyTorch's role here: owning device buffers, the stream and the CUDA graph object.  Training-mode forward
 (BatchNorm batch statistics, losses) is not implemented in this round and raises.
 """
-import os
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -312,8 +311,6 @@ class _Plan:
         self._valid = None
         self._graph = None
         self._post = []
-        # split-K scratch shared by every conv of this plan's main stream: zero-filled once, each launch restores the zeros
-        self._splitk_ws = torch.zeros(64 << 20, dtype=torch.uint8, device=device)
         self.names = {}              # id(callable) -> (layer name, algorithmic flops of the launch)
         self.launches = []           # backbone stage: list of zero-arg callables
         self.head_launches = []      # head stage
@@ -329,12 +326,8 @@ class _Plan:
                 r = None if res is None else res[i]
                 args.append(ops.ConvLevelArgs(xs[i], ys[i], n, in_dims[i], out_dims[i], ys[i].shape[-1], res=r,
                                               res_dims=None if r is None else res_dims[i], ldr=0 if r is None else r.shape[-1]))
-            need = ops.conv3d_workspace_bytes(args, layer.w, layer.shift, layer.cin, layer.cout, layer.taps, layer.stride,
-                                              layer.relu, out_fp32)
-            if need > self._splitk_ws.numel():
-                raise RuntimeError(f"split-K workspace too small: need {need} bytes")
             self._cur.append(lambda a=args, l=layer, f=out_fp32: ops.conv3d_fprop(
-                a, l.w, l.shift, l.cin, l.cout, l.taps, stride=l.stride, relu=l.relu, out_fp32=f, workspace=self._splitk_ws))
+                a, l.w, l.shift, l.cin, l.cout, l.taps, stride=l.stride, relu=l.relu, out_fp32=f))
             fl = 0.0
             for od in out_dims:
                 vox = n * od[0] * od[1] * od[2]
@@ -387,13 +380,15 @@ class _Plan:
                           scores=torch.zeros((n, eng.post_n), dtype=torch.float32, device=device),
                           levels=torch.zeros((n, eng.post_n), dtype=torch.float32, device=device),
                           count=torch.zeros((n,), dtype=torch.int32, device=device)) for _ in range(2)]
+        self._init_post()
+
+    def _init_post(self):
         # post-processing = ~45 tiny kernels per scene: high priority so that they slip into the SMs as conv CTAs retire instead of
         # queueing behind whole layers (the main stream depends on them two steps later through the double-buffered predictions)
-        self.side = torch.cuda.Stream(device=device, priority=-1 if os.environ.get("NRPN_SIDE_PRIORITY", "1") != "0" else 0)
+        self.side = torch.cuda.Stream(device=self.device, priority=-1)
         self._ev_pred = [torch.cuda.Event() for _ in range(2)]
         self._ev_done = [torch.cuda.Event() for _ in range(2)]
         self._parity = 0
-        self._post_graph = [None, None]
         self._build_post(None)
 
     def _build_resnet(self, L, n, dims, bf):
@@ -623,15 +618,7 @@ class _Plan:
         self._out = [dict(boxes=torch.zeros((n, cap, 1 + dim), dtype=torch.float32, device=device),
                           scores=torch.zeros((n, cap), dtype=torch.float32, device=device),
                           count=torch.zeros((n,), dtype=torch.int32, device=device)) for _ in range(2)]
-        # post-processing = ~45 tiny kernels per scene: high priority so that they slip into the SMs as conv CTAs retire instead of
-        # queueing behind whole layers (the main stream depends on them two steps later through the double-buffered predictions)
-        self.side = torch.cuda.Stream(device=device, priority=-1 if os.environ.get("NRPN_SIDE_PRIORITY", "1") != "0" else 0)
-        self._ev_pred = [torch.cuda.Event() for _ in range(2)]
-        self._ev_done = [torch.cuda.Event() for _ in range(2)]
-        self._parity = 0
-        self._post_graph = [None, None]
-        self._valid = "unset"
-        self._build_post(None)
+        self._init_post()
 
     def _build_post_fcos(self, valid_dims):
         import ctypes
@@ -703,7 +690,6 @@ class _Plan:
                                       eng.nms_thresh, eng.score_thresh, eng.min_size, self.dims, valid=v)
                 self._descs.append(d)
                 ws_bytes = max(ws_bytes, lib().nrpn_rpn_workspace_bytes(ctypes.byref(d)))
-        # one workspace per scene: the scenes of a batch are post-processed concurrently (parallel branches of the side-stream graph)
         if self._rpn_ws is None or self._rpn_ws[0].numel() < ws_bytes or len(self._rpn_ws) != self.n:
             self._rpn_ws = [torch.empty(ws_bytes, dtype=torch.uint8, device=self.device) for _ in range(self.n)]
         for par in range(2):
@@ -725,29 +711,11 @@ class _Plan:
                 f()
 
     def _run_post_eager(self, par):
-        """Post-processing of every scene of the batch.  The scenes are independent chains of ~45 small kernels (top-k, decode, NMS): scene 0
-        runs on the current stream, the others on branch streams forked from / joined to it -- eagerly, or as parallel branches of the
-        captured side-stream graph -- so the chain's critical path is one scene long, not n."""
-        fs = self._post[par]
-        # The chain is off the critical path already (high-priority side stream) and four concurrent chains only take SM slots from the
-        # convolutions; the serial chain is the default, NRPN_POST_PARALLEL=1 selects the branches.
-        if len(fs) == 1 or os.environ.get("NRPN_POST_PARALLEL", "0") != "1":
-            for f in fs:
-                f()
-            return
-        cur = torch.cuda.current_stream(self.device)
-        if getattr(self, "_branch", None) is None or len(self._branch) < len(fs) - 1:
-            self._branch = [torch.cuda.Stream(device=self.device, priority=-1) for _ in range(len(fs) - 1)]
-        for i, f in enumerate(fs):
-            if i == 0:
-                continue
-            b = self._branch[i - 1]
-            b.wait_stream(cur)
-            with torch.cuda.stream(b):
-                f()
-        fs[0]()
-        for i in range(1, len(fs)):
-            cur.wait_stream(self._branch[i - 1])
+        """Post-processing of every scene of the batch: independent chains of ~45 small kernels (top-k, decode, NMS), run one
+        after the other on the current stream.  The chains are off the critical path already (high-priority side stream), and
+        running them concurrently would only take SM slots from the convolutions."""
+        for f in self._post[par]:
+            f()
 
     def _run_eager(self):
         """Everything for one batch on the current stream (warm-up, launch counting, profiling)."""

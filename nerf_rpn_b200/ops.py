@@ -180,17 +180,10 @@ def _conv_desc(levels, w, shift, cin, cout, taps, stride, relu, out_fp32) -> Con
         lv.xo, lv.yo, lv.zo = (int(v) for v in L.out_dims)
         lv.xr, lv.yr, lv.zr = (int(v) for v in L.res_dims)
         lv.ldy, lv.ldr = int(L.ldy), int(L.ldr)
-    d.workspace, d.workspace_bytes = 0, 0
     d.act_fp16 = 1 if levels[0].x.dtype == torch.float16 else 0
     if w.dtype != levels[0].x.dtype:
         raise TypeError(f"conv3d: weights are {w.dtype} but activations are {levels[0].x.dtype}")
     return d
-
-
-def conv3d_workspace_bytes(levels, w, shift, cin, cout, taps, stride=1, relu=False, out_fp32=False) -> int:
-    """Bytes of (zero-filled) split-K scratch this layer would like; 0 if it is not split."""
-    d = _conv_desc(levels, w, shift, cin, cout, taps, stride, relu, out_fp32)
-    return int(lib().nrpn_conv3d_workspace_bytes(ctypes.byref(d)))
 
 
 def conv3d_variant(levels, w, shift, cin, cout, taps, stride=1, relu=False, out_fp32=False) -> str:
@@ -200,13 +193,9 @@ def conv3d_variant(levels, w, shift, cin, cout, taps, stride=1, relu=False, out_
 
 
 def conv3d_fprop(levels: Sequence[ConvLevelArgs], w: torch.Tensor, shift: torch.Tensor, cin: int, cout: int,
-                 taps: Sequence[Sequence[int]], stride: int = 1, relu: bool = False, out_fp32: bool = False,
-                 workspace: Optional[torch.Tensor] = None):
-    """One persistent wgmma implicit-GEMM launch over 1..4 levels sharing (w, shift).  `workspace`: optional uint8
-    tensor that was zero-filled once (split-K scratch, left zero-filled by every launch)."""
+                 taps: Sequence[Sequence[int]], stride: int = 1, relu: bool = False, out_fp32: bool = False):
+    """One persistent wgmma implicit-GEMM launch over 1..4 levels sharing (w, shift)."""
     d = _conv_desc(levels, w, shift, cin, cout, taps, stride, relu, out_fp32)
-    if workspace is not None:
-        d.workspace, d.workspace_bytes = workspace.data_ptr(), workspace.numel()
     check(lib().nrpn_conv3d_fprop(ctypes.byref(d), _stream()), "conv3d_fprop")
 
 

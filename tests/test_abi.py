@@ -34,13 +34,14 @@ def test_host_only_queries():
     assert L.nrpn_nms_workspace_bytes(0) > 0
 
 
-def test_struct_layouts_match_c():
+def test_ctypes_struct_layouts_match_c():
     code = r'''
 #include <stdio.h>
 #include <stddef.h>
 #include "nerf_rpn_b200.h"
 int main(void) {
-  printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\n", offsetof(nrpn_conv_desc, workspace), sizeof(nrpn_conv_level), sizeof(nrpn_conv_desc), offsetof(nrpn_conv_desc, stride),
+  printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\n", offsetof(nrpn_conv_desc, act_fp16), offsetof(nrpn_conv_desc, wsplit),
+         sizeof(nrpn_conv_level), sizeof(nrpn_conv_desc), offsetof(nrpn_conv_desc, stride),
          offsetof(nrpn_conv_desc, w), offsetof(nrpn_conv_desc, level), sizeof(nrpn_rpn_level), sizeof(nrpn_rpn_desc),
          offsetof(nrpn_rpn_desc, cell_anchors), offsetof(nrpn_rpn_desc, nms_thresh), offsetof(nrpn_rpn_desc, valid));
   printf("%zu %zu %zu %zu %zu %zu\n", sizeof(nrpn_wgrad_level), sizeof(nrpn_wgrad_desc), offsetof(nrpn_wgrad_desc, level),
@@ -52,7 +53,7 @@ int main(void) {
         subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), src, "-o", exe])
         vals = [int(v) for v in subprocess.check_output([exe]).split()]
     C, R, W = _lib.ConvDesc, _lib.RpnDesc, _lib.WgradDesc
-    mine = [C.workspace.offset, ctypes.sizeof(_lib.ConvLevel), ctypes.sizeof(C), C.stride.offset, C.w.offset, C.level.offset,
+    mine = [C.act_fp16.offset, C.wsplit.offset, ctypes.sizeof(_lib.ConvLevel), ctypes.sizeof(C), C.stride.offset, C.w.offset, C.level.offset,
             ctypes.sizeof(_lib.RpnLevel), ctypes.sizeof(R), R.cell_anchors.offset, R.nms_thresh.offset, R.valid.offset,
             ctypes.sizeof(_lib.WgradLevel), ctypes.sizeof(W), W.level.offset, W.dw.offset, W.workspace_bytes.offset, W.accumulate.offset]
     assert mine == vals

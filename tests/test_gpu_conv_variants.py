@@ -16,10 +16,7 @@ unnoticed.  Every row checks the same things:
 Run with -s to see the worst err / bound of every row."""
 import dataclasses
 import math
-import os
 import re
-import subprocess
-import sys
 import zlib
 from typing import Optional, Tuple
 
@@ -90,15 +87,6 @@ ROWS = {
                                       exact=True),
     "exact_long64_fp16_f32_gelu_res": Row("igemm<64,8,1>", (6, 9, 10), 128, 64, dtype="fp16", out_fp32=True, relu=2, res="same",
                                           exact=True),
-}
-
-SPLITK_ROWS = {
-    # NRPN_SPLITK=1: few output tiles, long reduction; the variant names the tile, conv3d_workspace_bytes > 0 the split
-    "splitk_full256_bf16_res": Row("igemm<256,4,1>", (5, 8, 8), 512, 512, res="same", n=1),
-    "splitk_full128_bf16_relu_z2": Row("igemm<128,6,1>", (3, 5, 2), 128, 120, relu=1, res="same"),
-    "splitk_64_fp16_f32_gelu_up": Row("igemm<64,8,1>", (6, 7, 9), 256, 64, dtype="fp16", out_fp32=True, relu=2, res=(3, 4, 5),
-                                      n=1),
-    "splitk_exact_256_f32_gelu": Row("igemm<256,4,1>", (5, 8, 8), 512, 256, out_fp32=True, relu=2, res="same", n=1, exact=True),
 }
 
 
@@ -178,10 +166,7 @@ class Case:
     def variant(self, ys):
         return self.call(self.ops.conv3d_variant, ys)
 
-    def workspace_bytes(self, ys):
-        return self.call(self.ops.conv3d_workspace_bytes, ys)
-
-    def run(self, levels=None, workspace=None):
+    def run(self, levels=None):
         """Launch over all levels (or the given level indices); returns the NaN-guarded output buffers."""
         keep = range(len(self.levels)) if levels is None else levels
         outs = self.outputs()
@@ -189,7 +174,7 @@ class Case:
         saved = self.levels
         self.levels = [saved[i] for i in keep]
         try:
-            self.call(self.ops.conv3d_fprop, ys, workspace=workspace)
+            self.call(self.ops.conv3d_fprop, ys)
         finally:
             self.levels = saved
         torch.cuda.synchronize()
@@ -256,13 +241,12 @@ def ops():
 
 
 @pytest.mark.parametrize("name", list(ROWS))
-def test_conv_variant_matrix(ops, monkeypatch, name):
+def test_conv_variant_row(ops, monkeypatch, name):
     row = ROWS[name]
     case = Case(ops, row)
     probe = [y for _, y in case.outputs()]
     variant = case.variant(probe)
     assert variant == row.variant, f"{name}: the tile rule now picks {variant}"
-    assert case.workspace_bytes(probe) == 0
     items, slots = _items_and_slots(case, variant)
     if row.wrap:
         assert items > slots, f"{name}: {items} work items do not wrap {slots} resident CTAs"
@@ -312,50 +296,18 @@ def test_conv_rejects_misaligned_pointers(ops):
     assert torch.isnan(y).all()
 
 
-def _in_split_k_child(test_name):
-    """Split-K is opt-in and NRPN_SPLITK is read once per process: run the test again in a child process that sets it."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-s", "-p", "no:cacheprovider", os.path.abspath(__file__) + "::" + test_name],
-                       cwd=root, capture_output=True, text=True, timeout=900, env={**os.environ, "NRPN_SPLITK": "1"})
-    print("".join(line + "\n" for line in r.stdout.splitlines() if line.startswith("[conv variant]")), end="")
-    assert r.returncode == 0 and "1 passed" in r.stdout, (r.stdout + r.stderr)[-3000:]
-
-
-def test_conv_split_k_matrix(ops):
-    """Split-K over a 256-wide, a 128-wide and a 64-wide tile; the fix-up epilogue with ReLU, GELU, fp32 and 16-bit outputs and
-    same-extent / up-sampled residuals.  Every launch must leave the arrival counters at zero."""
-    if os.environ.get("NRPN_SPLITK") != "1":
-        _in_split_k_child("test_conv_split_k_matrix")
-        return
-    ws = torch.zeros(64 << 20, dtype=torch.uint8, device="cuda")
-    for name, row in SPLITK_ROWS.items():
-        case = Case(ops, row)
-        probe = [y for _, y in case.outputs()]
-        assert case.variant(probe) == row.variant, f"{name}: the tile rule now picks {case.variant(probe)}"
-        need = case.workspace_bytes(probe)
-        assert 0 < need <= ws.numel(), f"{name}: expected to be split along K ({need} bytes)"
-        worst = case.check(case.run(workspace=ws), f"{name} [{row.variant} split-K]")
-        assert int(ws[:256].count_nonzero()) == 0, f"{name}: split-K arrival counters not restored to zero"
-        _report(name, row.variant + " split-K", worst)
-
-
-def test_conv_split_k_declined_on_misaligned_output(ops):
-    """The split-K fix-up stores 16-byte vectors: an fp32 y that is 8- but not 16-byte aligned must run unsplit (no workspace
-    wanted), match the reference and equal the unsplit launch of an aligned y bit for bit."""
-    if os.environ.get("NRPN_SPLITK") != "1":
-        _in_split_k_child("test_conv_split_k_declined_on_misaligned_output")
-        return
-    row = Row("igemm<256,4,1>", (5, 8, 8), 512, 256, out_fp32=True, relu=1, res="same", n=1)
+def test_conv_fp32_output_needs_only_pair_alignment(ops):
+    """An fp32 y that is 8- but not 16-byte aligned (one output pair) is accepted, matches the reference and equals the launch
+    on an aligned y bit for bit."""
+    row = Row("igemm<64,8,1>", (5, 8, 8), 512, 256, out_fp32=True, relu=1, res="same", n=1)
     aligned = Case(ops, row)
-    assert aligned.workspace_bytes([y for _, y in aligned.outputs()]) > 0
     shifted = Case(ops, row, y_offset=2)                                     # fp32 y at an 8-byte offset
     _, y = shifted.outputs()[0]
     assert y.data_ptr() % 16 == 8
-    assert shifted.workspace_bytes([y]) == 0 and shifted.variant([y]) == "igemm<64,8,1>"      # unsplit, hence narrowed
-    ws = torch.zeros(64 << 20, dtype=torch.uint8, device="cuda")
-    got = shifted.run(workspace=ws)
-    worst = shifted.check(got, "misaligned fp32 y under NRPN_SPLITK=1")
-    unsplit = aligned.run()                                                 # no workspace: runs unsplit
+    assert shifted.variant([y]) == row.variant
+    got = shifted.run()
+    worst = shifted.check(got, "fp32 y at an 8-byte offset")
+    ref = aligned.run()
     n = math.prod((row.n, *_out_dims(row.dims, 1), aligned.ldy))
-    assert torch.equal(got[0][GUARD + 2: GUARD + 2 + n].view(torch.int32), unsplit[0][GUARD: GUARD + n].view(torch.int32))
-    _report("splitk_declined_misaligned_f32", shifted.variant([y]), worst)
+    assert torch.equal(got[0][GUARD + 2: GUARD + 2 + n].view(torch.int32), ref[0][GUARD: GUARD + n].view(torch.int32))
+    _report("pair_aligned_f32", row.variant, worst)
