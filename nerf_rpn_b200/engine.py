@@ -18,15 +18,15 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 
 from . import ops, packing
-from .precision import resolve as _resolve_precision
+from .precision import resolve as _resolve_precision, split_weights, storage_dtype
 
 
 class _Conv:
-    """One pre-packed convolution (+ folded BN / bias, optional ReLU)."""
+    """One pre-packed convolution (+ folded BN / bias, optional ReLU).  `precision` gives the 16-bit storage format and, with `role`,
+    whether the weights are split into hi + lo planes (precision.split_weights).  Roles "stem" / "stem_s1" pack the 7^3 stem for
+    the stride-2 space-to-depth / stride-1 row-packed input."""
 
-    dtype = torch.bfloat16      # 16-bit storage format of the weights being packed (set by the engine around _pack)
-
-    def __init__(self, weight, bias=None, bn=None, stride=1, relu=False, stem=False, cout_pad_to=None, device="cuda", wsplit=False):
+    def __init__(self, weight, bias=None, bn=None, *, precision, role="backbone", stride=1, relu=False, cout_pad_to=None, device="cuda"):
         scale = shift = None
         if bn is not None:
             scale, shift = (t.cpu() for t in packing.fold_bn(bn))
@@ -40,12 +40,14 @@ class _Conv:
             scale = scale.cpu()
         if shift is not None:
             shift = shift.cpu()
-        if stem == "s1":
-            wp, taps = packing.pack_stem_s1_weight(weight, scale, dtype=_Conv.dtype)
-        elif stem:
-            wp, taps = packing.pack_stem_weight(weight, scale, dtype=_Conv.dtype)
+        dtype = storage_dtype(precision)
+        if role == "stem_s1":
+            wp, taps = packing.pack_stem_s1_weight(weight, scale, dtype=dtype)
+        elif role == "stem":
+            wp, taps = packing.pack_stem_weight(weight, scale, dtype=dtype)
         else:
-            wp, taps = packing.pack_conv_weight(weight, scale, cout_pad_to=cout_pad_to, dtype=_Conv.dtype, split=bool(wsplit))
+            wp, taps = packing.pack_conv_weight(weight, scale, cout_pad_to=cout_pad_to, dtype=dtype,
+                                                split=split_weights(precision, role, weight, stride))
         self.w = wp.to(device)
         self.taps = taps
         self.cin = wp.shape[-1]
@@ -55,12 +57,103 @@ class _Conv:
         self.shift = packing.pad_shift(shift, wp.shape[-2]).to(device)
         self.stride, self.relu = stride, relu
 
-    def flops(self, out_voxels: int, real_cin: Optional[int] = None, real_taps: Optional[int] = None) -> float:
-        return 2.0 * out_voxels * self.cout * (real_cin or self.cin) * (real_taps or len(self.taps))
-
 
 def _down(d: Sequence[int]) -> Tuple[int, int, int]:
     return tuple((v - 1) // 2 + 1 for v in d)
+
+
+def _f32(t, device):
+    return t.detach().float().to(device).contiguous()
+
+
+# ---------------------------------------------------------------- packers: one per module kind, shared by the engine and model/_eager.py
+def pack_stem(conv, bn, precision, device):
+    """7^3 stem conv + BN + ReLU of ResNet_FPN_256 / VGG_FPN: stride 2 on the space-to-depth packed input, or stride 1 (VGG_FPN
+    below 160) on the row-packed input."""
+    return _Conv(conv.weight, conv.bias, bn, precision=precision, role="stem" if conv.stride[0] == 2 else "stem_s1", relu=True,
+                 device=device)
+
+
+def pack_bottleneck(blk, precision, device):
+    """Bottleneck (feature_extractor.py:31-68) with its BatchNorms folded."""
+    def conv(c, bn, stride=1, relu=True):
+        return _Conv(c.weight, None, bn, precision=precision, stride=stride, relu=relu, device=device)
+    s = blk.stride
+    return {"c1": conv(blk.conv1, blk.bn1, s), "c2": conv(blk.conv2, blk.bn2),
+            "c3": conv(blk.conv3, blk.bn3),                                           # ReLU after the residual add
+            "ds": None if blk.downsample is None else conv(blk.downsample[0], blk.downsample[1], s, relu=False), "stride": s}
+
+
+def pack_fpn(laterals, outs, p2, precision, device):
+    """FPN neck: (1^3 lateral convs, 3^3 output convs); outs[p2] is the P2 output conv."""
+    return ([_Conv(m.weight, m.bias, precision=precision, device=device) for m in laterals],
+            [_Conv(m.weight, m.bias, precision=precision, role="p2" if i == p2 else "backbone", device=device) for i, m in enumerate(outs)])
+
+
+def pack_rpn_head(hd, precision, device):
+    """RPNHead (anchor.py:177-213): the 3^3 conv + ReLU stack, and the cls (A) and bbox (A*code) predictors fused into one 1^3 GEMM
+    zero-padded to 128 output channels."""
+    w = torch.cat([hd.cls_logits.weight, hd.bbox_pred.weight], 0)
+    b = torch.cat([hd.cls_logits.bias, hd.bbox_pred.bias], 0)
+    if w.shape[0] > 128:
+        raise ValueError("fused predictor supports at most 128 output channels")
+    return {"head": [_Conv(m.weight, m.bias, precision=precision, role="head", relu=True, device=device)
+                     for m in hd.conv if isinstance(m, torch.nn.Conv3d)],
+            "pred": _Conv(w, b, precision=precision, role="head", cout_pad_to=128, device=device)}
+
+
+def pack_fcos_head(hd, precision, device):
+    """FCOSHead (fcos/fcos.py:43-102): two towers of num_convs x [Conv3d 3^3 + GroupNorm(32) + ReLU] shared over levels, 3^3 predictors
+    for class (1) and distances (6|8) | centerness (1, from the bbox tower), one Scale per level."""
+    def conv(w, b):
+        return _Conv(w, b, precision=precision, role="head", device=device)
+
+    def tower(seq):
+        mods = list(seq.children())
+        return [(conv(c.weight, c.bias), _f32(gn.weight, device), _f32(gn.bias, device), float(gn.eps)) for c, gn in zip(mods[0::3], mods[1::3])]
+    return {"cls_tower": tower(hd.cls_tower), "bbox_tower": tower(hd.bbox_tower), "cls_pred": conv(hd.cls_logits.weight, hd.cls_logits.bias),
+            "reg_pred": conv(torch.cat([hd.bbox_pred.weight, hd.centerness.weight], 0), torch.cat([hd.bbox_pred.bias, hd.centerness.bias], 0)),
+            "scales": [float(s.scale.detach().item()) for s in hd.scales]}
+
+
+# ---------------------------------------------------------------- layer orders shared by the plan and model/_eager.py
+# conv(layer, xs, ys, in_dims, out_dims, res=, res_dims=, name=) issues one launch; buf(dims, channels) allocates an activation.
+def bottleneck_launches(conv, buf, e, x, xd, name):
+    """Bottleneck.forward (feature_extractor.py:48-68) on the layers pack_bottleneck made: c1, c2, [ds], c3 + residual.
+    Returns (output, dims)."""
+    od = _down(xd) if e["stride"] == 2 else xd
+    a = buf(od, e["c1"].cout)
+    conv(e["c1"], [x], [a], [xd], [od], name=f"{name}.c1")
+    b = buf(od, e["c2"].cout)
+    conv(e["c2"], [a], [b], [od], [od], name=f"{name}.c2")
+    r = x
+    if e["ds"] is not None:
+        r = buf(od, e["ds"].cout)
+        conv(e["ds"], [x], [r], [xd], [od], name=f"{name}.ds")
+    o = buf(od, e["c3"].cout)
+    conv(e["c3"], [b], [o], [od], [od], res=[r], res_dims=[od], name=f"{name}.c3+res")
+    return o, od
+
+
+def fpn_launches(conv, buf, lat, out, xs):
+    """FPN.forward (fpn.py:134-161) on the layers pack_fpn made: laterals top-down, each adding the nearest-upsampled level above in
+    its epilogue (the reference's in-place accumulation), then a 3^3 conv on every level.  xs, and the result: [(tensor, dims)] from P2 up."""
+    top = len(xs) - 1
+    q = [None] * len(xs)
+    for i in range(top, -1, -1):
+        f, fd = xs[i]
+        y = buf(fd, lat[i].cout)
+        if i == top:
+            conv(lat[i], [f], [y], [fd], [fd], name=f"fpn.lateral{i}")
+        else:
+            conv(lat[i], [f], [y], [fd], [fd], res=[q[i + 1][0]], res_dims=[q[i + 1][1]], name=f"fpn.lateral{i}+up")
+        q[i] = (y, fd)
+    feats = []
+    for i, (y, yd) in enumerate(q):
+        o = buf(yd, out[i].cout)
+        conv(out[i], [y], [o], [yd], [yd], name=f"fpn.conv{i}")
+        feats.append((o, yd))
+    return feats
 
 
 class RPNInferenceEngine:
@@ -72,8 +165,7 @@ class RPNInferenceEngine:
                  density_to_alpha: bool = False):
         precision = _resolve_precision(precision)            # "bf16" | "fp16" | "fp16_w2" (nerf_rpn_b200/precision.py)
         self.precision = precision
-        self.act_dtype = torch.bfloat16 if precision == "bf16" else torch.float16
-        self.wsplit = precision == "fp16_w2"                 # backbone / FPN weights as hi + lo halves
+        self.act_dtype = storage_dtype(precision)
         # datasets.py:50-52 (--normalize_density) applied by the stem packing kernel instead of numpy on the host (ResNet / VGG strided stems)
         self.density_to_alpha = bool(density_to_alpha)
         self.backbone, self.head = backbone, head
@@ -105,7 +197,6 @@ class RPNInferenceEngine:
 
     def _pack(self, device):
         bb, hd = self.backbone, self.head
-        L = {}
         kinds = {"ResNet_FPN_256": "resnet", "VGG_FPN": "vgg", "SwinTransformer_FPN": "swin"}
         if type(bb).__name__ not in kinds:
             raise NotImplementedError(f"nerf_rpn_b200: backbone {type(bb).__name__} is not implemented by the CUDA engine "
@@ -119,139 +210,59 @@ class RPNInferenceEngine:
             if not ok:
                 raise NotImplementedError("nerf_rpn_b200: the ResNet engine implements ResNet_FPN_256(Bottleneck, [3,4,6,3], input_dim=4, "
                                           "is_max_pool=True) (7^3 stride-2 stem on 4 channels + max-pool), the configuration run_rpn.py:276 builds")
-        _Conv.dtype = self.act_dtype
-        if self.kind == "vgg":
-            self._pack_vgg(L, device)
-        elif self.kind == "swin":
-            self._pack_swin(L, device)
-        else:
-            self._pack_resnet(L, device)
-        if hd is None:
-            self.layers = L
-            self._plans.clear()
-            return
-        if self.fcos is not None:
-            self._pack_fcos(L, device)
-            self.layers = L
-            self._plans.clear()
-            return
-        convs = [m for m in hd.conv if isinstance(m, torch.nn.Conv3d)]
-        L["head"] = [_Conv(m.weight, m.bias, relu=True, device=device) for m in convs]
-        # cls (A) and bbox (A*code) predictors fused into one 1x1x1 GEMM, zero-padded to 128 output channels
-        w = torch.cat([hd.cls_logits.weight, hd.bbox_pred.weight], 0)
-        b = torch.cat([hd.cls_logits.bias, hd.bbox_pred.bias], 0)
-        if w.shape[0] > 128:
-            raise ValueError("fused predictor supports at most 128 output channels")
-        L["pred"] = _Conv(w, b, device=device, cout_pad_to=128)
+        p = self.precision
+        L = {"vgg": self._pack_vgg, "swin": self._pack_swin, "resnet": self._pack_resnet}[self.kind](device)
+        if self.kind != "resnet":
+            L["lat"], L["fpn"] = pack_fpn(bb.fpn_neck.lateral_convs, bb.fpn_neck.fpn_convs, 0, p, device)
+        if hd is not None:
+            L.update(pack_rpn_head(hd, p, device) if self.fcos is None else pack_fcos_head(hd, p, device))
         self.layers = L
         self._plans.clear()
 
-    def _pack_swin(self, L, device):
+    def _pack_swin(self, device):
         """SwinTransformer_FPN (feature_extractor.py:689-789). Every Linear becomes a 1x1x1 conv of the wgmma kernel; widths
         that are not multiples of 64 (96 at stage 0) live in rows padded with zero channels."""
         bb = self.backbone
-        f32 = lambda t: t.detach().float().to(device).contiguous()
-        pe_conv, pe_ln = bb.patch_partition[0], bb.patch_partition[2]
-        C0 = pe_conv.weight.shape[0]
-        L["pe"] = _Conv(pe_conv.weight.reshape(C0, -1, 1, 1, 1), pe_conv.bias, device=device, wsplit=self.wsplit)
-        L["pe_ln"] = (f32(pe_ln.weight), f32(pe_ln.bias), float(pe_ln.eps))
+        ln = lambda m: (_f32(m.weight, device), _f32(m.bias, device), float(m.eps))
+        lin = lambda m, act=0: _Conv(m.weight.reshape(m.weight.shape[0], -1, 1, 1, 1), m.bias, precision=self.precision, relu=act,
+                                     device=device)
         stages = []
         for si, stage in enumerate(bb.stages):
             mods = list(stage.children())
             st = {"merge": None, "blocks": []}
             if si > 0:
                 pm = mods[0]; mods = mods[1:]
-                st["merge"] = dict(ln=(f32(pm.norm.weight), f32(pm.norm.bias), float(pm.norm.eps)), c_in=pm.dim,
-                                   red=_Conv(pm.reduction.weight.reshape(pm.reduction.weight.shape[0], -1, 1, 1, 1), None, device=device,
-                                             wsplit=self.wsplit))
+                st["merge"] = dict(ln=ln(pm.norm), c_in=pm.dim, red=lin(pm.reduction))
             for blk in mods:
                 a = blk.attn
-                C = a.qkv.weight.shape[1]
-                lin = lambda m, act=0: _Conv(m.weight.reshape(m.weight.shape[0], -1, 1, 1, 1), m.bias, relu=act, device=device,
-                                             wsplit=self.wsplit)
                 st["blocks"].append(dict(
-                    C=C, heads=a.num_heads, shift=int(a.shift_size[0]),
-                    ln1=(f32(blk.norm1.weight), f32(blk.norm1.bias), float(blk.norm1.eps)),
-                    ln2=(f32(blk.norm2.weight), f32(blk.norm2.bias), float(blk.norm2.eps)),
-                    qkv=lin(a.qkv), qkv_bias=f32(a.qkv.bias), table=f32(a.relative_position_bias_table),
+                    C=a.qkv.weight.shape[1], heads=a.num_heads, shift=int(a.shift_size[0]), ln1=ln(blk.norm1), ln2=ln(blk.norm2),
+                    qkv=lin(a.qkv), qkv_bias=_f32(a.qkv.bias, device), table=_f32(a.relative_position_bias_table, device),
                     proj=lin(a.proj), mlp0=lin(blk.mlp[0], 2), mlp3=lin(blk.mlp[3])))
             stages.append(st)
-        L["swin_stages"] = stages
-        L["lat"] = [_Conv(m.weight, m.bias, device=device, wsplit=self.wsplit) for m in bb.fpn_neck.lateral_convs]
-        L["fpn"] = [_Conv(m.weight, m.bias, device=device, wsplit=self.wsplit and i > 0) for i, m in enumerate(bb.fpn_neck.fpn_convs)]
+        return {"pe": lin(bb.patch_partition[0]), "pe_ln": ln(bb.patch_partition[2]), "swin_stages": stages}
 
-    def _pack_fcos(self, L, device):
-        """FCOSHead (fcos/fcos.py:43-102): two towers of num_convs x [Conv3d 3^3 + GroupNorm(32) + ReLU] shared over levels,
-        3^3 predictors for class (1), distances (6|8) and centerness (1, from the bbox tower), one Scale per level."""
-        hd = self.head
-        def tower(seq):
-            mods, out = list(seq.children()), []
-            for i in range(0, len(mods), 3):
-                conv, gn = mods[i], mods[i + 1]
-                out.append((_Conv(conv.weight, conv.bias, relu=False, device=device),
-                            gn.weight.detach().float().to(device).contiguous(), gn.bias.detach().float().to(device).contiguous(),
-                            float(gn.eps)))
-            return out
-        L["cls_tower"], L["bbox_tower"] = tower(hd.cls_tower), tower(hd.bbox_tower)
-        L["cls_pred"] = _Conv(hd.cls_logits.weight, hd.cls_logits.bias, device=device, cout_pad_to=None)
-        w = torch.cat([hd.bbox_pred.weight, hd.centerness.weight], 0)
-        b = torch.cat([hd.bbox_pred.bias, hd.centerness.bias], 0)
-        L["reg_pred"] = _Conv(w, b, device=device)
-        L["scales"] = [float(s.scale.detach().item()) for s in hd.scales]
+    def _pack_resnet(self, device):
+        bb, p = self.backbone, self.precision
+        lat, smooth = pack_fpn(bb.latlayers, bb.smooths, len(bb.smooths) - 1, p, device)          # the last smooth conv makes P2
+        return {"stem": pack_stem(bb.conv1, bb.bn1, p, device), "blocks": [pack_bottleneck(b, p, device) for s in bb.layers for b in s],
+                "lat": lat, "smooth": smooth}
 
-    def _pack_resnet(self, L, device):
-        bb = self.backbone
-        ws = self.wsplit
-        L["stem"] = _Conv(bb.conv1.weight, None, bb.bn1, relu=True, stem=True, device=device)
-        blocks = []
-        for stage in bb.layers:
-            for blk in stage:
-                s = blk.stride
-                slab = blk.conv2.weight.shape[0] <= 64 and blk.conv2.weight.shape[1] == 64     # 64-channel 3^3 layers stay on the slab kernel
-                e = {
-                    "c1": _Conv(blk.conv1.weight, None, blk.bn1, stride=s, relu=True, device=device, wsplit=ws),
-                    "c2": _Conv(blk.conv2.weight, None, blk.bn2, relu=True, device=device, wsplit=ws and not slab),
-                    "c3": _Conv(blk.conv3.weight, None, blk.bn3, relu=True, device=device, wsplit=ws),   # ReLU after the residual add
-                    "ds": None, "stride": s,
-                }
-                if blk.downsample is not None:
-                    e["ds"] = _Conv(blk.downsample[0].weight, None, blk.downsample[1], stride=s, relu=False, device=device, wsplit=ws)
-                blocks.append(e)
-        L["blocks"] = blocks
-        L["lat"] = [_Conv(m.weight, m.bias, device=device, wsplit=ws) for m in bb.latlayers]
-        # smooth convs: P4 and P3 carry split weights; the P2 smooth (15 % of the scene's FLOPs, tensor-pipe bound) keeps single
-        # halves -- its weight rounding alone contributes ~2e-4 to P2 (measured by emulation, DESIGN.md section 4)
-        nsm = len(bb.smooths)
-        L["smooth"] = [_Conv(m.weight, m.bias, device=device, wsplit=ws and i < nsm - 1) for i, m in enumerate(bb.smooths)]
-
-    def _pack_vgg(self, L, device):
+    def _pack_vgg(self, device):
         """VGG_FPN (feature_extractor.py:289-377): stem [conv7 (s2 + max-pool when input_size >= 160, else s1), BN, ReLU], then
         four stages of (Conv3d 3^3 + BN + ReLU)* [+ MaxPool3d(2,2,ceil)] and the mmdet-style FPN neck (fpn.py:105-161)."""
-        bb = self.backbone
-        mods = list(bb.layers.children())
-        stem_conv, stem_bn = mods[0], mods[1]
-        strided = stem_conv.stride[0] == 2
-        L["vgg_strided"] = strided
-        L["stem"] = _Conv(stem_conv.weight, stem_conv.bias, stem_bn, relu=True, stem=True if strided else "s1", device=device)
+        mods = list(self.backbone.layers.children())
         stages = []
         for grp in mods[-4:]:
             seq, items = list(grp.children()), []
-            i = 0
-            while i < len(seq):
-                m = seq[i]
+            for i, m in enumerate(seq):           # ReLU is fused into the conv epilogue
                 if isinstance(m, torch.nn.Conv3d):
                     bn = seq[i + 1] if i + 1 < len(seq) and isinstance(seq[i + 1], torch.nn.BatchNorm3d) else None
-                    slab = m.weight.shape[0] <= 64 and m.weight.shape[1] == 64
-                    items.append(("conv", _Conv(m.weight, m.bias, bn, relu=True, device=device, wsplit=self.wsplit and not slab)))
-                    i += 2 if bn is not None else 1
+                    items.append(("conv", _Conv(m.weight, m.bias, bn, precision=self.precision, relu=True, device=device)))
                 elif isinstance(m, torch.nn.MaxPool3d):
-                    items.append(("pool", None)); i += 1
-                else:
-                    i += 1                      # ReLU is fused into the conv epilogue
+                    items.append(("pool", None))
             stages.append(items)
-        L["vgg_stages"] = stages
-        L["lat"] = [_Conv(m.weight, m.bias, device=device, wsplit=self.wsplit) for m in bb.fpn_neck.lateral_convs]
-        L["fpn"] = [_Conv(m.weight, m.bias, device=device, wsplit=self.wsplit and i > 0) for i, m in enumerate(bb.fpn_neck.fpn_convs)]
+        return {"vgg_strided": mods[0].stride[0] == 2, "stem": pack_stem(mods[0], mods[1], self.precision, device), "vgg_stages": stages}
 
     # ---------------------------------------------------------------- plan
     def _get_plan(self, n, dims, device, channels_last: bool = False, u8: bool = False):
@@ -351,38 +362,8 @@ class _Plan:
         self.has_head = eng.head is not None
         if not self.has_head:
             return
-        if eng.fcos is not None:
-            self._build_fcos_head(L, n, buf, conv)
-            return
         self._cur = self.head_launches
-        cur = self.features
-        for layer in L["head"]:
-            nxt = [buf(d, 256) for d in self.feat_dims]
-            conv(layer, cur, nxt, self.feat_dims, self.feat_dims, name="head3x3x3")
-            cur = nxt
-        # cls|bbox predictor: two output sets (parity) so that the post-processing of scene i, which runs on a side
-        # stream, overlaps the backbone of scene i+1 without a buffer hazard
-        self.pred_sets = [[buf(d, 128, torch.float32) for d in self.feat_dims] for _ in range(2)]
-        self.pred_launch = []
-        for par in range(2):
-            self._cur = []
-            conv(L["pred"], cur, self.pred_sets[par], self.feat_dims, self.feat_dims, out_fp32=True,
-                 real=(256, 1, eng.A * (1 + eng.code)), name="pred(cls|bbox)")
-            self.pred_launch.append(self._cur[0])
-            if par == 1:
-                self.algorithmic_flops -= self.names[id(self._cur[0])][1] / n     # counted once per scene
-        self._cur = self.head_launches
-
-        # proposals
-        self.strides = [tuple(dims[k] // d[k] for k in range(3)) for d in self.feat_dims]
-        bd = 7 if eng.rotated else 6
-        self._out = [dict(boxes=torch.zeros((n, eng.post_n, bd), dtype=torch.float32, device=device),
-                          scores=torch.zeros((n, eng.post_n), dtype=torch.float32, device=device),
-                          levels=torch.zeros((n, eng.post_n), dtype=torch.float32, device=device),
-                          count=torch.zeros((n,), dtype=torch.int32, device=device)) for _ in range(2)]
-        self._init_post()
-
-    def _init_post(self):
+        (self._build_anchor_head if eng.fcos is None else self._build_fcos_head)(L, n, buf, conv)
         # post-processing = ~45 tiny kernels per scene: high priority so that they slip into the SMs as conv CTAs retire instead of
         # queueing behind whole layers (the main stream depends on them two steps later through the double-buffered predictions)
         self.side = torch.cuda.Stream(device=self.device, priority=-1)
@@ -391,42 +372,33 @@ class _Plan:
         self._parity = 0
         self._build_post(None)
 
-    def _build_resnet(self, L, n, dims, bf):
-        eng, device = self.eng, self.device
-        buf, conv = self._buf, self._conv
-        X, Y, Z = dims
+    def _launch(self, fn, name):
+        """Appends a launch that is not a convolution (no algorithmic FLOPs) to the current stage."""
+        self._cur.append(fn)
+        self.names[id(fn)] = (name, 0.0)
+
+    def _build_strided_stem(self, L, n, dims, bf):
+        """Space-to-depth input packing, the 7^3 stride-2 stem and the 3^3 stride-2 max-pool (ResNet, VGG at >= 160)."""
         d1 = _down(dims)
         self.packed = torch.empty((n, d1[0], d1[1], d1[2] + 1, 64), **bf)
-        self.launches.append(lambda: ops.pack_stem_input(self._src, self.packed, density_to_alpha=self.eng.density_to_alpha))
-        self.names[id(self.launches[-1])] = ("pack_stem_input", 0.0)
-        c1 = buf(d1, 64)
-        conv(L["stem"], [self.packed], [c1], [(d1[0], d1[1], d1[2] + 1)], [d1], real=(4, 343, 64), name="stem7x7x7s2(s2d)")
+        self._launch(lambda: ops.pack_stem_input(self._src, self.packed, density_to_alpha=self.eng.density_to_alpha), "pack_stem_input")
+        c1 = self._buf(d1, 64)
+        self._conv(L["stem"], [self.packed], [c1], [(d1[0], d1[1], d1[2] + 1)], [d1], real=(4, 343, 64), name="stem7x7x7s2(s2d)")
         d2 = _down(d1)
-        c1p = buf(d2, 64)
-        self.launches.append(lambda: ops.maxpool3d_k3s2(c1, c1p))
-        self.names[id(self.launches[-1])] = ("maxpool3d_k3s2", 0.0)
+        x = self._buf(d2, 64)
+        self._launch(lambda: ops.maxpool3d_k3s2(c1, x), "maxpool3d_k3s2")
+        return x, d2
+
+    def _build_resnet(self, L, n, dims, bf):
+        buf, conv = self._buf, self._conv
+        x, xd = self._build_strided_stem(L, n, dims, bf)
 
         # bottom-up
-        x, xd = c1p, d2
         c_out = []
-        bi = 0
-        for si, stage in enumerate(eng.backbone.layers):
+        blocks = iter(L["blocks"])
+        for si, stage in enumerate(self.eng.backbone.layers):
             for _ in stage:
-                e = L["blocks"][bi]; bi += 1
-                s = e["stride"]
-                od = _down(xd) if s == 2 else xd
-                a = buf(od, e["c1"].cout)
-                conv(e["c1"], [x], [a], [xd], [od], name=f"L{si}.c1")
-                b = buf(od, e["c2"].cout)
-                conv(e["c2"], [a], [b], [od], [od], name=f"L{si}.c2")
-                if e["ds"] is not None:
-                    r = buf(od, e["ds"].cout)
-                    conv(e["ds"], [x], [r], [xd], [od], name=f"L{si}.ds")
-                else:
-                    r = x
-                o = buf(od, e["c3"].cout)
-                conv(e["c3"], [b], [o], [od], [od], res=[r], res_dims=[od], name=f"L{si}.c3+res")
-                x, xd = o, od
+                x, xd = bottleneck_launches(conv, buf, next(blocks), x, xd, f"L{si}")
             c_out.append((x, xd))
 
         # top-down (feature_extractor.py:224-235): p5 = lat0(c5); p_i = up(p_{i+1}) + lat(c_i); smooth all but p5
@@ -448,27 +420,15 @@ class _Plan:
         feats.reverse()                                   # [P2, P3, P4, P5]
         return feats
 
-
     def _build_vgg(self, L, n, dims, bf):
         """VGG_FPN.forward (feature_extractor.py:362-377) + FPN.forward (fpn.py:134-161)."""
-        device = self.device
         buf, conv = self._buf, self._conv
         X, Y, Z = dims
         if L["vgg_strided"]:
-            d1 = _down(dims)
-            self.packed = torch.empty((n, d1[0], d1[1], d1[2] + 1, 64), **bf)
-            self.launches.append(lambda: ops.pack_stem_input(self._src, self.packed, density_to_alpha=self.eng.density_to_alpha))
-            self.names[id(self.launches[-1])] = ("pack_stem_input", 0.0)
-            c1 = buf(d1, 64)
-            conv(L["stem"], [self.packed], [c1], [(d1[0], d1[1], d1[2] + 1)], [d1], real=(4, 343, 64), name="stem7x7x7s2(s2d)")
-            xd = _down(d1)
-            x = buf(xd, 64)
-            self.launches.append(lambda a=c1, b=x: ops.maxpool3d_k3s2(a, b))
-            self.names[id(self.launches[-1])] = ("maxpool3d_k3s2", 0.0)
+            x, xd = self._build_strided_stem(L, n, dims, bf)
         else:
             self.packed = torch.empty((n, X, Y + 1, Z, 64), **bf)
-            self.launches.append(lambda: ops.pack_stem_input_s1(self._src, self.packed))
-            self.names[id(self.launches[-1])] = ("pack_stem_input_s1", 0.0)
+            self._launch(lambda: ops.pack_stem_input_s1(self._src, self.packed), "pack_stem_input_s1")
             xd = dims
             x = buf(xd, 64)
             conv(L["stem"], [self.packed], [x], [(X, Y + 1, Z)], [xd], real=(4, 343, 64), name="stem7x7x7s1(packed)")
@@ -482,37 +442,18 @@ class _Plan:
                 else:
                     od = tuple((v + 1) // 2 for v in xd)
                     y = buf(od, x.shape[-1])
-                    self.launches.append(lambda a=x, b=y: ops.maxpool3d_k2s2_ceil(a, b))
-                    self.names[id(self.launches[-1])] = ("maxpool3d_k2s2_ceil", 0.0)
+                    self._launch(lambda a=x, b=y: ops.maxpool3d_k2s2_ceil(a, b), "maxpool3d_k2s2_ceil")
                     x, xd = y, od
             stage_out.append((x, xd))
-        # FPN: laterals top-down (in-place accumulation in the reference), then a 3^3 conv on every level
-        lat = [None] * 4
-        for i in range(3, -1, -1):
-            f, fd = stage_out[i]
-            q = buf(fd, 256)
-            if i == 3:
-                conv(L["lat"][i], [f], [q], [fd], [fd], name=f"fpn.lateral{i}")
-            else:
-                conv(L["lat"][i], [f], [q], [fd], [fd], res=[lat[i + 1][0]], res_dims=[lat[i + 1][1]], name=f"fpn.lateral{i}+up")
-            lat[i] = (q, fd)
-        feats = []
-        for i in range(4):
-            q, qd = lat[i]
-            o = buf(qd, 256)
-            conv(L["fpn"][i], [q], [o], [qd], [qd], name=f"fpn.conv{i}")
-            feats.append((o, qd))
-        return feats
+        return fpn_launches(conv, buf, L["lat"], L["fpn"], stage_out)
 
     def _build_swin(self, L, n, dims, bf):
         """SwinTransformer_FPN.forward (feature_extractor.py:781-789): patch embedding, 4 stages of [PatchMerging] + blocks
         (x + attn(LN x); x + MLP(LN x)), FPN neck. Token grids are (n, H, W, D, ld) with ld = C rounded up to 64."""
         device = self.device
-        buf, conv = self._buf, self._conv
+        buf, conv, add = self._buf, self._conv, self._launch
         pad64 = lambda c: (c + 63) // 64 * 64
         zbuf = lambda d, c: torch.zeros((n, *d, c), dtype=self.eng.act_dtype, device=device)      # pad channels must stay zero
-        def add(fn, name):
-            self.launches.append(fn); self.names[id(fn)] = (name, 0.0)
         X, Y, Z = dims
         td = (X // 4, Y // 4, Z // 4)
         self.packed = torch.empty((n, *td, 256), **bf)
@@ -559,27 +500,42 @@ class _Plan:
                 x = x3
             # the stage output must survive the next stage's scratch: it is only read (by patch merging and the FPN lateral)
             stage_out.append((x, td))
-        lat = [None] * 4
-        for i in range(3, -1, -1):
-            f, fd = stage_out[i]
-            q = buf(fd, 256)
-            if i == 3:
-                conv(L["lat"][i], [f], [q], [fd], [fd], name=f"fpn.lateral{i}")
-            else:
-                conv(L["lat"][i], [f], [q], [fd], [fd], res=[lat[i + 1][0]], res_dims=[lat[i + 1][1]], name=f"fpn.lateral{i}+up")
-            lat[i] = (q, fd)
-        feats = []
-        for i in range(4):
-            q, qd = lat[i]
-            o = buf(qd, 256)
-            conv(L["fpn"][i], [q], [o], [qd], [qd], name=f"fpn.conv{i}")
-            feats.append((o, qd))
-        return feats
+        return fpn_launches(conv, buf, L["lat"], L["fpn"], stage_out)
+
+    def _build_pred(self, launch):
+        """Predictor launches into two output sets (parity), so that the post-processing of scene i, which runs on the side stream,
+        overlaps the backbone of scene i+1 without a buffer hazard.  launch(par) issues the predictor convs that write set par."""
+        self.pred_launch = []
+        for par in range(2):
+            self._cur = []
+            launch(par)
+            fs = self._cur
+            self.pred_launch.append(fs[0] if len(fs) == 1 else lambda fs=fs: [g() for g in fs])
+        for g in fs:
+            self.algorithmic_flops -= self.names[id(g)][1] / self.n         # counted once per scene
+        self._cur = self.head_launches
+
+    def _build_anchor_head(self, L, n, buf, conv):
+        eng, device = self.eng, self.device
+        cur = self.features
+        for layer in L["head"]:
+            nxt = [buf(d, 256) for d in self.feat_dims]
+            conv(layer, cur, nxt, self.feat_dims, self.feat_dims, name="head3x3x3")
+            cur = nxt
+        self.pred_sets = [[buf(d, 128, torch.float32) for d in self.feat_dims] for _ in range(2)]
+        self._build_pred(lambda par: conv(L["pred"], cur, self.pred_sets[par], self.feat_dims, self.feat_dims, out_fp32=True,
+                                          real=(256, 1, eng.A * (1 + eng.code)), name="pred(cls|bbox)"))
+        # proposals
+        self.strides = [tuple(self.dims[k] // d[k] for k in range(3)) for d in self.feat_dims]
+        bd = 7 if eng.rotated else 6
+        self._out = [dict(boxes=torch.zeros((n, eng.post_n, bd), dtype=torch.float32, device=device),
+                          scores=torch.zeros((n, eng.post_n), dtype=torch.float32, device=device),
+                          levels=torch.zeros((n, eng.post_n), dtype=torch.float32, device=device),
+                          count=torch.zeros((n,), dtype=torch.int32, device=device)) for _ in range(2)]
 
     def _build_fcos_head(self, L, n, buf, conv):
         eng, device, dims = self.eng, self.device, self.dims
         f = eng.fcos
-        self._cur = self.head_launches
         self._gn_ws = torch.empty(max(1, ops.lib().nrpn_groupnorm_workspace_bytes(len(self.features), n)), dtype=torch.uint8, device=device)
         ends = {}
         for name in ("cls_tower", "bbox_tower"):
@@ -587,66 +543,27 @@ class _Plan:
             for (layer, gamma, beta, eps) in L[name]:
                 nxt = [buf(d, 256) for d in self.feat_dims]
                 conv(layer, cur, nxt, self.feat_dims, self.feat_dims, name=f"fcos.{name}.conv3x3x3")
-                self.head_launches.append(lambda t=nxt, g=gamma, b=beta, e=eps: ops.groupnorm_relu_(t, g, b, e, True, 32, self._gn_ws))
-                self.names[id(self.head_launches[-1])] = (f"fcos.{name}.groupnorm+relu", 0.0)
+                self._launch(lambda t=nxt, g=gamma, b=beta, e=eps: ops.groupnorm_relu_(t, g, b, e, True, 32, self._gn_ws),
+                             f"fcos.{name}.groupnorm+relu")
                 cur = nxt
             ends[name] = cur
         code = 8 if f["use_obb"] else 6
         cls_c, reg_c = L["cls_pred"].cout, L["reg_pred"].cout
         self.pred_sets = [dict(cls=[buf(d, cls_c, torch.float32) for d in self.feat_dims],
                                reg=[buf(d, reg_c, torch.float32) for d in self.feat_dims]) for _ in range(2)]
-        self.pred_launch = []
-        for par in range(2):
-            self._cur = []
+
+        def pred(par):
             conv(L["cls_pred"], ends["cls_tower"], self.pred_sets[par]["cls"], self.feat_dims, self.feat_dims, out_fp32=True,
                  real=(256, 27, 1), name="fcos.cls_logits")
             conv(L["reg_pred"], ends["bbox_tower"], self.pred_sets[par]["reg"], self.feat_dims, self.feat_dims, out_fp32=True,
                  real=(256, 27, code + 1), name="fcos.bbox_pred|centerness")
-            fs = list(self._cur)
-            self.pred_launch.append(lambda fs=fs: [g() for g in fs])
-            if par == 1:
-                for g in fs:
-                    self.algorithmic_flops -= self.names[id(g)][1] / n
-        self._cur = self.head_launches
+        self._build_pred(pred)
         self.strides = list(f["fpn_strides"])[: len(self.feat_dims)]
-        self._fcos_desc0 = ops.make_fcos_desc([p[0].reshape(-1, cls_c) for p in self.pred_sets[0]["cls"]],
-                                              [p[0].reshape(-1, reg_c) for p in self.pred_sets[0]["reg"]], self.feat_dims, self.strides,
-                                              L["scales"], f["use_obb"], f["pre_nms_thresh"], f["pre_nms_top_n"], f["nms_thresh"],
-                                              f["post_nms_top_n"], f["min_size"], dims)
-        cap = ops.lib().nrpn_fcos_max_proposals(__import__("ctypes").byref(self._fcos_desc0))
+        cap = ops.lib().nrpn_fcos_max_proposals(__import__("ctypes").byref(self._post_desc(0, 0, dims)))
         dim = 7 if f["use_obb"] else 6
         self._out = [dict(boxes=torch.zeros((n, cap, 1 + dim), dtype=torch.float32, device=device),
                           scores=torch.zeros((n, cap), dtype=torch.float32, device=device),
                           count=torch.zeros((n,), dtype=torch.int32, device=device)) for _ in range(2)]
-        self._init_post()
-
-    def _build_post_fcos(self, valid_dims):
-        import ctypes
-        eng, L, f = self.eng, self.eng.layers, self.eng.fcos
-        cls_c, reg_c = L["cls_pred"].cout, L["reg_pred"].cout
-        self._post = [[], []]
-        ws_bytes = 0
-        descs = []
-        for par in range(2):
-            for i in range(self.n):
-                gs = self.dims if valid_dims is None else valid_dims[i]
-                d = ops.make_fcos_desc([p[i].reshape(-1, cls_c) for p in self.pred_sets[par]["cls"]],
-                                       [p[i].reshape(-1, reg_c) for p in self.pred_sets[par]["reg"]], self.feat_dims, self.strides,
-                                       L["scales"], f["use_obb"], f["pre_nms_thresh"], f["pre_nms_top_n"], f["nms_thresh"],
-                                       f["post_nms_top_n"], f["min_size"], gs, padded=self.n > 1)
-                descs.append(d)
-                ws_bytes = max(ws_bytes, ops.lib().nrpn_fcos_workspace_bytes(ctypes.byref(d)))
-        if self._rpn_ws is None or self._rpn_ws[0].numel() < ws_bytes or len(self._rpn_ws) != self.n:
-            self._rpn_ws = [torch.empty(ws_bytes, dtype=torch.uint8, device=self.device) for _ in range(self.n)]
-        for par in range(2):
-            o = self._out[par]
-            for i in range(self.n):
-                d = descs[par * self.n + i]
-                out = (o["boxes"][i], o["scores"][i], o["count"][i:i + 1])
-                self._post[par].append(lambda d=d, out=out, i=i: ops.fcos_proposals(d, self.device, out=out, workspace=self._rpn_ws[i]))
-        self._descs = descs
-        self._valid = valid_dims
-        self._post_graph = [None, None]
 
     # results of the most recent run (valid once `done` has completed)
     @property
@@ -673,31 +590,37 @@ class _Plan:
     def done(self):
         return self._ev_done[self._parity]
 
+    def _post_desc(self, par, i, valid):
+        """Post-processing descriptor of scene i's predictions in output set par; valid: the scene's own extent (None: the plan's)."""
+        eng, L, f = self.eng, self.eng.layers, self.eng.fcos
+        if f is None:
+            return ops.make_rpn_desc([p[i].reshape(-1, 128) for p in self.pred_sets[par]], self.feat_dims, self.strides, eng.cells, eng.A,
+                                     eng.rotated, eng.pre_n, eng.post_n, eng.nms_thresh, eng.score_thresh, eng.min_size, self.dims, valid=valid)
+        cls_c, reg_c = L["cls_pred"].cout, L["reg_pred"].cout
+        return ops.make_fcos_desc([p[i].reshape(-1, cls_c) for p in self.pred_sets[par]["cls"]],
+                                  [p[i].reshape(-1, reg_c) for p in self.pred_sets[par]["reg"]], self.feat_dims, self.strides,
+                                  L["scales"], f["use_obb"], f["pre_nms_thresh"], f["pre_nms_top_n"], f["nms_thresh"],
+                                  f["post_nms_top_n"], f["min_size"], valid or self.dims, padded=self.n > 1)
+
     def _build_post(self, valid_dims):
+        """Per parity and scene, one post-processing chain (top-k, decode, NMS) writing that scene's rows of the output set."""
         import ctypes
         from ._lib import lib
-        eng = self.eng
-        if eng.fcos is not None:
-            return self._build_post_fcos(valid_dims)
-        self._post = [[], []]
-        self._descs = []
-        ws_bytes = 0
-        for par in range(2):
-            for i in range(self.n):
-                preds = [p[i].reshape(-1, 128) for p in self.pred_sets[par]]
-                v = None if valid_dims is None else valid_dims[i]
-                d = ops.make_rpn_desc(preds, self.feat_dims, self.strides, eng.cells, eng.A, eng.rotated, eng.pre_n, eng.post_n,
-                                      eng.nms_thresh, eng.score_thresh, eng.min_size, self.dims, valid=v)
-                self._descs.append(d)
-                ws_bytes = max(ws_bytes, lib().nrpn_rpn_workspace_bytes(ctypes.byref(d)))
+        anchor = self.eng.fcos is None
+        self._descs = [self._post_desc(par, i, None if valid_dims is None else valid_dims[i]) for par in range(2) for i in range(self.n)]
+        ws_query = lib().nrpn_rpn_workspace_bytes if anchor else lib().nrpn_fcos_workspace_bytes
+        ws_bytes = max(ws_query(ctypes.byref(d)) for d in self._descs)
         if self._rpn_ws is None or self._rpn_ws[0].numel() < ws_bytes or len(self._rpn_ws) != self.n:
             self._rpn_ws = [torch.empty(ws_bytes, dtype=torch.uint8, device=self.device) for _ in range(self.n)]
+        run = ops.rpn_proposals if anchor else ops.fcos_proposals
+        keys = ("boxes", "scores", "levels") if anchor else ("boxes", "scores")
+        self._post = [[], []]
         for par in range(2):
             o = self._out[par]
             for i in range(self.n):
-                d = self._descs[par * self.n + i]
-                out = (o["boxes"][i], o["scores"][i], o["levels"][i], o["count"][i:i + 1])
-                self._post[par].append(lambda d=d, out=out, i=i: ops.rpn_proposals(d, self.device, out=out, workspace=self._rpn_ws[i]))
+                out = tuple(o[k][i] for k in keys) + (o["count"][i:i + 1],)
+                self._post[par].append(lambda d=self._descs[par * self.n + i], out=out, i=i:
+                                       run(d, self.device, out=out, workspace=self._rpn_ws[i]))
         self._valid = valid_dims
         self._post_graph = [None, None]
 

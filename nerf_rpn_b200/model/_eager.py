@@ -7,13 +7,13 @@ tensors in and out like the reference, channels-last 16-bit inside (the layout c
 convolution / normalisation is a libnerf_rpn_b200 launch).  Eval-mode semantics (BatchNorm running statistics); in training mode
 the whole-model training engine (nerf_rpn_b200/train.py) is the supported path and these functions raise.
 """
-from typing import List, Sequence, Tuple
+from typing import Sequence, Tuple
 
 import torch
 
 from .. import ops
-from ..engine import _Conv
-from ..precision import resolve as _resolve_precision
+from ..engine import _Conv, bottleneck_launches, fpn_launches, pack_bottleneck, pack_fcos_head, pack_fpn, pack_rpn_head
+from ..precision import resolve as _resolve_precision, storage_dtype
 
 _CACHE = {}
 
@@ -28,13 +28,7 @@ def _packed(module, precision, build):
     ver = _version(module)
     hit = _CACHE.get(key)
     if hit is None or hit[0] != ver:
-        old = _Conv.dtype
-        _Conv.dtype = torch.bfloat16 if precision == "bf16" else torch.float16
-        try:
-            hit = (ver, build())
-        finally:
-            _Conv.dtype = old
-        _CACHE[key] = hit
+        hit = _CACHE[key] = (ver, build())
     return hit[1]
 
 
@@ -55,26 +49,26 @@ def _from_cl(y: torch.Tensor, c: int = None) -> torch.Tensor:
     return y.permute(0, 4, 1, 2, 3).float()                           # NCDHW view semantics (channels_last_3d strides) like the engine
 
 
-def _conv(layer: _Conv, xs: Sequence[torch.Tensor], out_dims, res=None, out_fp32=False):
-    """One launch over the levels in xs (shared weights); returns the outputs (N, *out_dims[i], layer.cout)."""
-    n = xs[0].shape[0]
-    dt = torch.float32 if out_fp32 else xs[0].dtype
-    ys = [torch.empty((n, *od, layer.cout), dtype=dt, device=xs[0].device) for od in out_dims]
+def _launch(layer: _Conv, xs, ys, in_dims, out_dims, res=None, res_dims=None, out_fp32=False, name=None):
+    """One launch over the levels in xs (shared weights) into ys, issued now: the `conv` callback of the engine's layer orders."""
     args = []
     for i, x in enumerate(xs):
         r = None if res is None else res[i]
-        args.append(ops.ConvLevelArgs(x, ys[i], n, x.shape[1:4], out_dims[i], layer.cout, res=r, res_dims=None if r is None else r.shape[1:4],
-                                      ldr=0 if r is None else r.shape[-1]))
+        args.append(ops.ConvLevelArgs(x, ys[i], x.shape[0], in_dims[i], out_dims[i], ys[i].shape[-1], res=r,
+                                      res_dims=None if r is None else res_dims[i], ldr=0 if r is None else r.shape[-1]))
     ops.conv3d_fprop(args, layer.w, layer.shift, layer.cin, layer.cout, layer.taps, stride=layer.stride, relu=layer.relu, out_fp32=out_fp32)
+
+
+def _buf_like(x: torch.Tensor):
+    return lambda d, c: torch.empty((x.shape[0], *d, c), dtype=x.dtype, device=x.device)
+
+
+def _conv(layer: _Conv, xs: Sequence[torch.Tensor], out_dims, out_fp32=False):
+    """One launch over the levels in xs (shared weights); returns the outputs (N, *out_dims[i], layer.cout)."""
+    dt = torch.float32 if out_fp32 else xs[0].dtype
+    ys = [torch.empty((xs[0].shape[0], *od, layer.cout), dtype=dt, device=xs[0].device) for od in out_dims]
+    _launch(layer, xs, ys, [x.shape[1:4] for x in xs], out_dims, out_fp32=out_fp32)
     return ys
-
-
-def _down(d):
-    return tuple((v - 1) // 2 + 1 for v in d)
-
-
-def _dtype(precision):
-    return torch.bfloat16 if precision == "bf16" else torch.float16
 
 
 # ---------------------------------------------------------------------------------------------- Bottleneck
@@ -82,25 +76,9 @@ def bottleneck_forward(blk, x: torch.Tensor, precision=None) -> torch.Tensor:
     """feature_extractor.py:48-68: relu(bn3(conv3(relu(bn2(conv2(relu(bn1(conv1(x)))))))) + [downsample](x)), BatchNorm folded."""
     _check(x, blk.training, "Bottleneck")
     precision = _resolve_precision(precision)
-    ws = precision == "fp16_w2"
-
-    def build():
-        dev = x.device
-        s = blk.stride
-        L = dict(c1=_Conv(blk.conv1.weight, None, blk.bn1, stride=s, relu=True, device=dev, wsplit=ws),
-                 c2=_Conv(blk.conv2.weight, None, blk.bn2, relu=True, device=dev, wsplit=ws and blk.conv2.weight.shape[1] != 64),
-                 c3=_Conv(blk.conv3.weight, None, blk.bn3, relu=True, device=dev, wsplit=ws), ds=None)
-        if blk.downsample is not None:
-            L["ds"] = _Conv(blk.downsample[0].weight, None, blk.downsample[1], stride=s, relu=False, device=dev, wsplit=ws)
-        return L
-    L = _packed(blk, precision, build)
-    xc = _to_cl(x, _dtype(precision))
-    xd = tuple(xc.shape[1:4])
-    od = _down(xd) if blk.stride == 2 else xd
-    a = _conv(L["c1"], [xc], [od])[0]
-    b = _conv(L["c2"], [a], [od])[0]
-    r = xc if L["ds"] is None else _conv(L["ds"], [xc], [od])[0]
-    o = _conv(L["c3"], [b], [od], res=[r])[0]
+    L = _packed(blk, precision, lambda: pack_bottleneck(blk, precision, x.device))
+    xc = _to_cl(x, storage_dtype(precision))
+    o, _ = bottleneck_launches(_launch, _buf_like(xc), L, xc, tuple(xc.shape[1:4]), "bottleneck")
     return _from_cl(o)
 
 
@@ -110,20 +88,10 @@ def fpn_forward(fpn, inputs: Sequence[torch.Tensor], precision=None) -> Tuple[to
     assert len(inputs) == len(fpn.in_channels)
     _check(inputs[0], fpn.training, "FPN")
     precision = _resolve_precision(precision)
-    ws = precision == "fp16_w2"
-
-    def build():
-        dev = inputs[0].device
-        return dict(lat=[_Conv(m.weight, m.bias, device=dev, wsplit=ws) for m in fpn.lateral_convs],
-                    out=[_Conv(m.weight, m.bias, device=dev, wsplit=ws and i > 0) for i, m in enumerate(fpn.fpn_convs)])
-    L = _packed(fpn, precision, build)
-    xs = [_to_cl(t, _dtype(precision)) for t in inputs]
-    n_l = len(xs)
-    lat = [None] * n_l
-    for i in range(n_l - 1, -1, -1):
-        d = tuple(xs[i].shape[1:4])
-        lat[i] = _conv(L["lat"][i], [xs[i]], [d], res=None if i == n_l - 1 else [lat[i + 1]])[0]
-    return tuple(_from_cl(_conv(L["out"][i], [lat[i]], [tuple(lat[i].shape[1:4])])[0]) for i in range(n_l))
+    lat, out = _packed(fpn, precision, lambda: pack_fpn(fpn.lateral_convs, fpn.fpn_convs, 0, precision, inputs[0].device))
+    xs = [_to_cl(t, storage_dtype(precision)) for t in inputs]
+    feats = fpn_launches(_launch, _buf_like(xs[0]), lat, out, [(x, tuple(x.shape[1:4])) for x in xs])
+    return tuple(_from_cl(o) for o, _ in feats)
 
 
 # ---------------------------------------------------------------------------------------------- RPNHead
@@ -132,23 +100,10 @@ def rpn_head_pred(head, feats: Sequence[torch.Tensor], precision=None):
     post-processing kernel (nrpn_rpn_proposals) reads."""
     _check(feats[0], head.training, "RPNHead")
     precision = _resolve_precision(precision)
-    if precision == "fp16_w2":
-        precision_w = "fp16"                               # the head keeps single halves (precision.py)
-    else:
-        precision_w = precision
-
-    def build():
-        dev = feats[0].device
-        convs = [m for m in head.conv if isinstance(m, torch.nn.Conv3d)]
-        w = torch.cat([head.cls_logits.weight, head.bbox_pred.weight], 0)
-        b = torch.cat([head.cls_logits.bias, head.bbox_pred.bias], 0)
-        if w.shape[0] > 128:
-            raise ValueError("fused predictor supports at most 128 output channels")
-        return dict(conv=[_Conv(m.weight, m.bias, relu=True, device=dev) for m in convs], pred=_Conv(w, b, device=dev, cout_pad_to=128))
-    L = _packed(head, precision_w, build)
-    cur = [_to_cl(t, _dtype(precision_w)) for t in feats]
+    L = _packed(head, precision, lambda: pack_rpn_head(head, precision, feats[0].device))
+    cur = [_to_cl(t, storage_dtype(precision)) for t in feats]
     dims = [tuple(t.shape[1:4]) for t in cur]
-    for layer in L["conv"]:
+    for layer in L["head"]:
         cur = _conv(layer, cur, dims)
     return _conv(L["pred"], cur, dims, out_fp32=True)
 
@@ -169,35 +124,19 @@ def fcos_head_forward(head, feats: Sequence[torch.Tensor], precision=None):
     first six regressors and x stride -> (logits, bbox_reg, centerness) lists of (N,C,w,l,h) fp32."""
     _check(feats[0], head.training, "FCOSHead")
     precision = _resolve_precision(precision)
-    precision_w = "fp16" if precision == "fp16_w2" else precision
     code = head.bbox_pred.weight.shape[0]
-
-    def build():
-        dev = feats[0].device
-
-        def tower(seq):
-            mods, out = list(seq.children()), []
-            for i in range(0, len(mods), 3):
-                conv, gn = mods[i], mods[i + 1]
-                out.append((_Conv(conv.weight, conv.bias, relu=False, device=dev), gn.weight.detach().float().to(dev).contiguous(),
-                            gn.bias.detach().float().to(dev).contiguous(), float(gn.eps)))
-            return out
-        w = torch.cat([head.bbox_pred.weight, head.centerness.weight], 0)
-        b = torch.cat([head.bbox_pred.bias, head.centerness.bias], 0)
-        return dict(cls=tower(head.cls_tower), box=tower(head.bbox_tower), cls_pred=_Conv(head.cls_logits.weight, head.cls_logits.bias, device=dev),
-                    reg_pred=_Conv(w, b, device=dev), scales=[float(s.scale.detach().item()) for s in head.scales])
-    L = _packed(head, precision_w, build)
-    x0 = [_to_cl(t, _dtype(precision_w)) for t in feats]
+    L = _packed(head, precision, lambda: pack_fcos_head(head, precision, feats[0].device))
+    x0 = [_to_cl(t, storage_dtype(precision)) for t in feats]
     dims = [tuple(t.shape[1:4]) for t in x0]
     ends = {}
-    for name in ("cls", "box"):
+    for name in ("cls_tower", "bbox_tower"):
         cur = x0
         for (layer, gamma, beta, eps) in L[name]:
             cur = _conv(layer, cur, dims)
             ops.groupnorm_relu_(cur, gamma, beta, eps, True, 32)
         ends[name] = cur
-    cls = _conv(L["cls_pred"], ends["cls"], dims, out_fp32=True)
-    reg = _conv(L["reg_pred"], ends["box"], dims, out_fp32=True)
+    cls = _conv(L["cls_pred"], ends["cls_tower"], dims, out_fp32=True)
+    reg = _conv(L["reg_pred"], ends["bbox_tower"], dims, out_fp32=True)
     logits = [c[..., :1].permute(0, 4, 1, 2, 3).contiguous() for c in cls]
     bbox_reg, ctr = [], []
     for l, r in enumerate(reg):

@@ -85,12 +85,7 @@ class ResNet_FPN_256(EngineHolder, nn.Module):
 
     def forward(self, x: torch.Tensor) -> List[torch.Tensor]:
         """x: (N,4,W,L,H) fp32 CUDA -> [P2,P3,P4,P5], each (N,256,w,l,h) fp32 (channels_last_3d strides)."""
-        from ..engine import RPNInferenceEngine
-        precision = _resolve_precision(getattr(self, "precision", None))
-        if self._engine is None or self._engine.precision != precision:
-            self._engine = RPNInferenceEngine(self, precision=precision)
-        plan = self._engine.forward_device(x.contiguous())
-        return [f.permute(0, 4, 1, 2, 3).float() for f in plan.features]
+        return self._engine_features(x)
 
 
 def _not_built(name):
@@ -169,12 +164,7 @@ class VGG_FPN(EngineHolder, nn.Module):
 
     def forward(self, X):
         """(N,4,W,L,H) fp32 CUDA -> tuple of 4 (N,256,w,l,h) fp32 feature maps (channels_last_3d strides)."""
-        from ..engine import RPNInferenceEngine
-        precision = _resolve_precision(getattr(self, "precision", None))
-        if self._engine is None or self._engine.precision != precision:
-            self._engine = RPNInferenceEngine(self, precision=precision)
-        plan = self._engine.forward_device(X.contiguous())
-        return tuple(f.permute(0, 4, 1, 2, 3).float() for f in plan.features)
+        return tuple(self._engine_features(X))
 
 
 class ShiftedWindowAttention(nn.Module):
@@ -278,12 +268,7 @@ class SwinTransformer_FPN(EngineHolder, nn.Module):
         self._engine = None
 
     def forward(self, x):
-        from ..engine import RPNInferenceEngine
-        precision = _resolve_precision(getattr(self, "precision", None))
-        if self._engine is None or self._engine.precision != precision:
-            self._engine = RPNInferenceEngine(self, precision=precision)
-        plan = self._engine.forward_device(x.contiguous())
-        return tuple(f.permute(0, 4, 1, 2, 3).float() for f in plan.features)
+        return tuple(self._engine_features(x))
 
 
 ResNet_FPN_64 = _not_built("ResNet_FPN_64")

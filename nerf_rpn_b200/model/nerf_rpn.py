@@ -10,7 +10,7 @@ from torch import nn
 
 from ..precision import resolve as _resolve_precision
 from .anchor import AnchorGenerator3D, RPNHead
-from .rpn import RegionProposalNetwork
+from .rpn import RegionProposalNetwork, write_objectness
 
 
 def _default_anchorgen():
@@ -81,18 +81,6 @@ class NeRFRegionProposalNetwork(nn.Module):
         d = self.__dict__.copy()
         d["_engine"], d["_engine_key"], d["_train_engine"] = None, None, None
         return d
-
-    def _output_objectness(self, plan, ori_sizes, output_paths):
-        """--output_voxel_scores (rpn.py:538-549): per scene, per level, the maximum objectness logit over the anchors cropped to the
-        un-padded extent ceil(size / 2^(level+2)); npz with keys '0'..'3'."""
-        A = self.rpn.anchor_generator.num_anchors_per_location()[0]
-        for i in range(len(ori_sizes)):
-            all_levels = {}
-            for level, p in enumerate(plan.pred):
-                score = p[i][..., :A].max(dim=-1)[0]
-                w, l, h = np.ceil(np.array(ori_sizes[i]) / 2 ** (level + 2)).astype(int)
-                all_levels[str(level)] = score[:w, :l, :h].cpu().numpy()
-            np.savez_compressed(output_paths[i], **all_levels)
 
     def extra_repr(self):
         return f"precision={self.precision!r}"
@@ -173,7 +161,8 @@ class NeRFRegionProposalNetwork(nn.Module):
         counts = plan.out_count.tolist()                              # the one host sync: data-dependent output sizes
         features = [f.permute(0, 4, 1, 2, 3).float() for f in plan.features]
         if objectness_output_paths is not None:
-            self._output_objectness(plan, original_mesh_sizes, objectness_output_paths)
+            write_objectness(plan.pred, self.rpn.anchor_generator.num_anchors_per_location()[0], original_mesh_sizes,
+                             objectness_output_paths)
         proposals = [plan.out_boxes[i, :k].clone() for i, k in enumerate(counts)]
         level_index = [plan.out_levels[i, :k].clone() for i, k in enumerate(counts)]
         scores = [plan.out_scores[i, :k].clone() for i, k in enumerate(counts)]

@@ -71,10 +71,10 @@ class RegionProposalNetwork(nn.Module):
         if self.training:
             raise NotImplementedError("nerf_rpn_b200: RegionProposalNetwork.forward in training mode is not a stand-alone path; the losses "
                                       "are computed by the whole-model training engine (NeRFRegionProposalNetwork.forward / train.py)")
-        if objectness_output_paths is not None:
-            self.output_objectness_from(features, original_mesh_sizes, objectness_output_paths)
         from ._eager import rpn_head_pred
         pred = rpn_head_pred(self.head, features, getattr(self, "precision", None))
+        if objectness_output_paths is not None:
+            write_objectness(pred, self.head.cls_logits.weight.shape[0], original_mesh_sizes, objectness_output_paths)
         n = pred[0].shape[0]
         mesh = tuple(int(v) for v in meshes.shape[-3:])
         fdims = [tuple(p.shape[1:4]) for p in pred]
@@ -91,16 +91,16 @@ class RegionProposalNetwork(nn.Module):
             boxes.append(b[:k]); scores.append(s[:k]); levels.append(lv[:k])
         return boxes, levels, {}, scores
 
-    def output_objectness_from(self, features, ori_sizes, output_paths):
-        """--output_voxel_scores (rpn.py:538-549): per scene and level the maximum objectness LOGIT over the anchors, cropped to the
-        un-padded extent ceil(size / 2^(level+2)), written as npz with keys '0'..'3'."""
-        import numpy as np
-        from ._eager import rpn_head_forward
-        logits, _ = rpn_head_forward(self.head, features, getattr(self, "precision", None))
-        for i in range(len(ori_sizes)):
-            all_levels = {}
-            for level, lg in enumerate(logits):
-                score = lg[i].max(dim=0)[0]
-                w, l, h = np.ceil(np.array(ori_sizes[i]) / 2 ** (level + 2)).astype(int)
-                all_levels[str(level)] = score[:w, :l, :h].cpu().numpy()
-            np.savez_compressed(output_paths[i], **all_levels)
+
+def write_objectness(pred, A, ori_sizes, output_paths):
+    """--output_voxel_scores (rpn.py:538-549): per scene and level the maximum objectness LOGIT over the anchors, cropped to the
+    un-padded extent ceil(size / 2^(level+2)), written as npz with keys '0'..'3'.  pred: per level the head's fused channels-last
+    output (N, w, l, h, >= A) whose first A channels are the logits."""
+    import numpy as np
+    for i in range(len(ori_sizes)):
+        all_levels = {}
+        for level, p in enumerate(pred):
+            score = p[i][..., :A].max(dim=-1)[0]
+            w, l, h = np.ceil(np.array(ori_sizes[i]) / 2 ** (level + 2)).astype(int)
+            all_levels[str(level)] = score[:w, :l, :h].cpu().numpy()
+        np.savez_compressed(output_paths[i], **all_levels)

@@ -27,6 +27,7 @@ import torch
 
 from . import ops, packing
 from ._lib import RpnDesc, check, lib
+from .engine import _down
 
 
 _TRAIN_GRAPH = os.environ.get("NRPN_TRAIN_GRAPH", "1") != "0"          # static launch lists of the training step replayed as CUDA graphs
@@ -71,10 +72,6 @@ def _p(t):
 
 def _ru(v, m):
     return (v + m - 1) // m * m
-
-
-def _down(d):
-    return tuple((v - 1) // 2 + 1 for v in d)
 
 
 def bucket_schedule(bwd_lo: Sequence[int], n_params: int, bucket_elems: int):
