@@ -170,6 +170,20 @@ int nrpn_pack_stem_input_ex(const float *grid, int n, int x, int y, int z, void 
  * datasets.py:59-61 does on the host (.float() / 255.0); a quarter of the fp32 host-to-device traffic. */
 int nrpn_pack_stem_input_u8(const uint8_t *grid_xyzc, int n, int x, int y, int z, void *packed, int act_fp16, nrpn_stream_t stream);
 
+/* Same packing for a batch of differently sized fp32 scenes (the reference pads a training batch to its element-wise maximum,
+ * nerf_rpn.py:129-146): scene i is read through its own pointer, extent and memory order and written, in ONE launch, into slot i
+ * of the packed padded batch (n, ceil(X/2), ceil(Y/2), ceil(Z/2)+1, 64), (X, Y, Z) = element-wise maximum of the extents.
+ * Voxels outside a scene's extent are exactly 0 in all four channels; the padded fp32 batch is never materialised.
+ * density_to_alpha = 1 maps the real voxels only: the reference's dataset maps the densities before the batch is padded. */
+#define NRPN_STEM_MAX_SCENES 32
+typedef struct {
+    const float *grid;        /* device, fp32; 16-byte aligned when channels_last */
+    int32_t x, y, z;          /* extent of this scene */
+    int32_t channels_last;    /* 0: contiguous (4,x,y,z); 1: the (4,x,y,z) view of a contiguous (x,y,z,4) array, datasets.py:55-56 */
+} nrpn_stem_src;
+int nrpn_pack_stem_input_batch(const nrpn_stem_src *src /*host, n entries*/, int n, void *packed, int act_fp16, int density_to_alpha,
+                               nrpn_stream_t stream);
+
 /* F.max_pool3d(kernel 3, stride 2, padding 1) on (N,X,Y,Z,C) bf16, C % 8 == 0 (feature_extractor.py:219). */
 int nrpn_maxpool3d_k3s2(const void *in, int n, int x, int y, int z, int c, void *out, int act_fp16, nrpn_stream_t stream);
 
@@ -298,6 +312,15 @@ size_t nrpn_assign_targets_workspace_bytes(int n_anchors, int n_gt);
 int nrpn_assign_targets(const float *anchors, int n_anchors, const float *gt, int n_gt, int gt_dim, const uint8_t *valid,
                         float high_threshold, float low_threshold, int allow_low_quality_matches, float *labels,
                         int64_t *matched_idxs, void *workspace, size_t workspace_bytes, nrpn_stream_t stream);
+
+/* The per-anchor padding masks of a batch padded to (px, py, pz) (AnchorGenerator3D.get_padding_masks + permute_and_flatten,
+ * anchor.py:124-152, rpn.py:231-238): mask[i * total + k] = 1 when flat anchor k of scene i lies inside that scene's original
+ * extent ori_sizes[3i..3i+2], in the flat order the valid argument of nrpn_assign_targets reads (level, voxel (x,y,z) row-major,
+ * anchor); total = num_anchors * sum over levels of the grid's voxel count.  Per axis and level, the anchor is real when its voxel index is
+ * below ceil(ori / stride) with stride = padded // grid -- the reference's rule, which is not always the nominal stride (padded depth
+ * 130, P2 grid 33: stride 3).  n <= NRPN_STEM_MAX_SCENES, n_levels <= 8. */
+int nrpn_anchor_padding_mask(const int32_t *ori_sizes /*host, n x 3*/, int n, int px, int py, int pz, const int32_t *grid_dims /*host, n_levels x 3*/,
+                             int n_levels, int num_anchors, uint8_t *mask /*device, n x total*/, nrpn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------ weight gradient
  * dW[tap][co][ci] = sum_v dY[v][co] * X[v + tap_off][ci] of a stride-1 convolution (training, SURVEY.md 8(a) a18) on wgmma.

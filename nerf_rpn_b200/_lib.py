@@ -58,6 +58,14 @@ class WgradDesc(ctypes.Structure):
                 ("act_fp16", ctypes.c_int32), ("dw_layout", ctypes.c_int32), ("accumulate", ctypes.c_int32)]
 
 
+class StemSrc(ctypes.Structure):
+    """nrpn_stem_src: one scene of a ragged batch for nrpn_pack_stem_input_batch."""
+    _fields_ = [("grid", ctypes.c_void_p), ("x", ctypes.c_int32), ("y", ctypes.c_int32), ("z", ctypes.c_int32), ("channels_last", ctypes.c_int32)]
+
+
+STEM_MAX_SCENES = 32
+
+
 class GnLevel(ctypes.Structure):
     _fields_ = [("x", ctypes.c_void_p), ("voxels", ctypes.c_int32)]
 
@@ -123,6 +131,7 @@ _SIGNATURES = {
                                                ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_stream]),
     "nrpn_pack_stem_input_u8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                ctypes.c_void_p, ctypes.c_int, c_stream]),
+    "nrpn_pack_stem_input_batch": (ctypes.c_int, [ctypes.POINTER(StemSrc), ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, c_stream]),
     "nrpn_maxpool3d_k3s2": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                            ctypes.c_int, ctypes.c_void_p, ctypes.c_int, c_stream]),
     "nrpn_maxpool3d_k2s2_ceil": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
@@ -146,6 +155,8 @@ _SIGNATURES = {
     "nrpn_assign_targets_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int, ctypes.c_int]),
     "nrpn_assign_targets": (ctypes.c_int, [c_f32p, ctypes.c_int, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_float,
                                            ctypes.c_float, ctypes.c_int, c_f32p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, c_stream]),
+    "nrpn_anchor_padding_mask": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                                ctypes.c_int, ctypes.c_int, ctypes.c_void_p, c_stream]),
     "nrpn_rowmax_f32": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, c_f32p, ctypes.c_void_p, c_stream]),
     "nrpn_recall_match": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
     # ---- training step (csrc/train.cu)

@@ -16,34 +16,59 @@ __device__ __forceinline__ float density_to_alpha(float sigma) {
     return fminf(fmaxf(a, 0.0f), 1.0f);
 }
 
+// Per-chunk pieces shared by the fp32 stem packing kernels.
+// stem_chunk: coordinates of 16-byte chunk t of the packed (n, X2, Y2, Z2+1, 64) output -- scene b, first voxel (x, y, z) of the
+// chunk's z pair, and its space-to-depth block index kk along z (-1 / Z2 for the zero rows at either end).
+struct StemChunk { int b, x, y, z, kk; };
+__device__ __forceinline__ StemChunk stem_chunk(size_t t, int X2, int Y2, int Z2) {
+    StemChunk q;
+    const int s = (int)(t & 7);
+    size_t v = t >> 3;
+    const int k = (int)(v % (Z2 + 1)); v /= (Z2 + 1);
+    const int j = (int)(v % Y2); v /= Y2;
+    const int i = (int)(v % X2); q.b = (int)(v / X2);
+    const int half = s >> 2, rx = (s >> 1) & 1, ry = s & 1;
+    q.kk = k - 1 + half;                            // s2d block index along z
+    q.x = 2 * i + rx; q.y = 2 * j + ry; q.z = 2 * q.kk;
+    return q;
+}
+
+// The voxel pair (x,y,z), (x,y,z+1) of one NCDHW scene: p points at channel 0 of voxel (x,y,z), channel planes `plane` floats apart;
+// val = {4 channels of z, 4 channels of z+1} (rz major, c minor); `second`: z+1 lies inside the scene (else those stay 0).
+__device__ __forceinline__ void stem_load_ncdhw(const float* __restrict__ p, size_t plane, bool second, int alpha, float (&val)[8]) {
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        val[c] = p[c * plane];
+        if (second) val[4 + c] = p[c * plane + 1];
+    }
+    if (alpha) { val[3] = density_to_alpha(val[3]); if (second) val[7] = density_to_alpha(val[7]); }
+}
+
+// Same pair from a channels-last scene: one 128-bit load per voxel.
+__device__ __forceinline__ void stem_load_cl(const float4* __restrict__ p, bool second, int alpha, float4& a, float4& c) {
+    a = __ldg(p);
+    if (second) c = __ldg(p + 1);
+    if (alpha) { a.w = density_to_alpha(a.w); if (second) c.w = density_to_alpha(c.w); }
+}
+
+__device__ __forceinline__ void stem_store(__nv_bfloat16* __restrict__ out, size_t t, float4 a, float4 c, int fp16) {
+    const uint32_t h0 = pack_act2(a.x, a.y, fp16), h1 = pack_act2(a.z, a.w, fp16);
+    const uint32_t h2 = pack_act2(c.x, c.y, fp16), h3 = pack_act2(c.z, c.w, fp16);
+    *reinterpret_cast<uint4*>(out + (t << 3)) = make_uint4(h0, h1, h2, h3);
+}
+
 __global__ void pack_stem_kernel(const float* __restrict__ grid, int n, int X, int Y, int Z, int X2, int Y2, int Z2,
                                  __nv_bfloat16* __restrict__ out, int fp16, int alpha) {
     const size_t total = (size_t)n * X2 * Y2 * (Z2 + 1) * 8;
+    const size_t plane = (size_t)X * Y * Z;
     for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
-        const int s = (int)(t & 7);
-        size_t v = t >> 3;
-        const int k = (int)(v % (Z2 + 1)); v /= (Z2 + 1);
-        const int j = (int)(v % Y2); v /= Y2;
-        const int i = (int)(v % X2); const int b = (int)(v / X2);
-        const int half = s >> 2, rx = (s >> 1) & 1, ry = s & 1;
-        const int kk = k - 1 + half;                    // s2d block index along z
-        const int x = 2 * i + rx, y = 2 * j + ry, z = 2 * kk;
+        const StemChunk q = stem_chunk(t, X2, Y2, Z2);
         float val[8];                                   // order: rz major, c minor
 #pragma unroll
-        for (int q = 0; q < 8; ++q) val[q] = 0.f;
-        if (kk >= 0 && kk < Z2 && x < X && y < Y) {
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                const float* p = grid + ((((size_t)b * 4 + c) * X + x) * Y + y) * Z + z;
-                val[c] = p[0];
-                if (z + 1 < Z) val[4 + c] = p[1];
-            }
-            if (alpha) { val[3] = density_to_alpha(val[3]); if (z + 1 < Z) val[7] = density_to_alpha(val[7]); }
-        }
-        uint32_t h[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) h[q] = pack_act2(val[2 * q], val[2 * q + 1], fp16);
-        *reinterpret_cast<uint4*>(out + (t << 3)) = make_uint4(h[0], h[1], h[2], h[3]);
+        for (int e = 0; e < 8; ++e) val[e] = 0.f;
+        if (q.kk >= 0 && q.kk < Z2 && q.x < X && q.y < Y)
+            stem_load_ncdhw(grid + (size_t)q.b * 4 * plane + ((size_t)q.x * Y + q.y) * Z + q.z, plane, q.z + 1 < Z, alpha, val);
+        stem_store(out, t, make_float4(val[0], val[1], val[2], val[3]), make_float4(val[4], val[5], val[6], val[7]), fp16);
     }
 }
 
@@ -53,24 +78,40 @@ __global__ void pack_stem_cl_kernel(const float4* __restrict__ grid, int n, int 
                                     __nv_bfloat16* __restrict__ out, int fp16, int alpha) {
     const size_t total = (size_t)n * X2 * Y2 * (Z2 + 1) * 8;
     for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
-        const int s = (int)(t & 7);
-        size_t v = t >> 3;
-        const int k = (int)(v % (Z2 + 1)); v /= (Z2 + 1);
-        const int j = (int)(v % Y2); v /= Y2;
-        const int i = (int)(v % X2); const int b = (int)(v / X2);
-        const int half = s >> 2, rx = (s >> 1) & 1, ry = s & 1;
-        const int kk = k - 1 + half;
-        const int x = 2 * i + rx, y = 2 * j + ry, z = 2 * kk;
+        const StemChunk q = stem_chunk(t, X2, Y2, Z2);
         float4 a = make_float4(0.f, 0.f, 0.f, 0.f), c = a;
-        if (kk >= 0 && kk < Z2 && x < X && y < Y) {
-            const float4* p = grid + (((size_t)b * X + x) * Y + y) * Z + z;
-            a = __ldg(p);
-            if (z + 1 < Z) c = __ldg(p + 1);
-            if (alpha) { a.w = density_to_alpha(a.w); if (z + 1 < Z) c.w = density_to_alpha(c.w); }
+        if (q.kk >= 0 && q.kk < Z2 && q.x < X && q.y < Y)
+            stem_load_cl(grid + (((size_t)q.b * X + q.x) * Y + q.y) * Z + q.z, q.z + 1 < Z, alpha, a, c);
+        stem_store(out, t, a, c, fp16);
+    }
+}
+
+// A batch of differently sized scenes packed into the stem input of the batch padded to the element-wise maximum extent
+// (X2, Y2, Z2 of that maximum): each chunk reads its scene's own pointer, extent and memory order; a voxel outside the scene is
+// the reference's zero padding (nerf_rpn.py:140-146) in all four channels -- density_to_alpha is applied to real voxels only.
+struct StemBatch { nrpn_stem_src src[NRPN_STEM_MAX_SCENES]; };
+
+__global__ void pack_stem_batch_kernel(const __grid_constant__ StemBatch B, int n, int X2, int Y2, int Z2, __nv_bfloat16* __restrict__ out,
+                                       int fp16, int alpha) {
+    const size_t total = (size_t)n * X2 * Y2 * (Z2 + 1) * 8;
+    for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
+        const StemChunk q = stem_chunk(t, X2, Y2, Z2);
+        const nrpn_stem_src& S = B.src[q.b];
+        float4 a = make_float4(0.f, 0.f, 0.f, 0.f), c = a;
+        if (q.kk >= 0 && q.z < S.z && q.x < S.x && q.y < S.y) {
+            const size_t vox = ((size_t)q.x * S.y + q.y) * S.z + q.z;
+            const bool second = q.z + 1 < S.z;
+            if (S.channels_last) {
+                stem_load_cl(reinterpret_cast<const float4*>(S.grid) + vox, second, alpha, a, c);
+            } else {
+                float val[8];
+#pragma unroll
+                for (int e = 0; e < 8; ++e) val[e] = 0.f;
+                stem_load_ncdhw(S.grid + vox, (size_t)S.x * S.y * S.z, second, alpha, val);
+                a = make_float4(val[0], val[1], val[2], val[3]); c = make_float4(val[4], val[5], val[6], val[7]);
+            }
         }
-        const uint32_t h0 = pack_act2(a.x, a.y, fp16), h1 = pack_act2(a.z, a.w, fp16);
-        const uint32_t h2 = pack_act2(c.x, c.y, fp16), h3 = pack_act2(c.z, c.w, fp16);
-        *reinterpret_cast<uint4*>(out + (t << 3)) = make_uint4(h0, h1, h2, h3);
+        stem_store(out, t, a, c, fp16);
     }
 }
 
@@ -256,6 +297,25 @@ int nrpn_pack_stem_input_u8(const uint8_t* grid, int n, int x, int y, int z, voi
     const size_t total = (size_t)n * X2 * Y2 * (Z2 + 1) * 8;
     pack_stem_cl_u8_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const uint32_t*>(grid), n, x, y, z, X2, Y2, Z2,
                                                                                   reinterpret_cast<__nv_bfloat16*>(packed), act_fp16 ? 1 : 0);
+    NRPN_LAUNCH_CHECK();
+    return NRPN_OK;
+}
+
+int nrpn_pack_stem_input_batch(const nrpn_stem_src* src, int n, void* packed, int act_fp16, int density_to_alpha, nrpn_stream_t stream) {
+    if (!src || !packed || n < 1 || n > NRPN_STEM_MAX_SCENES) return NRPN_ERR_INVALID;
+    StemBatch B;
+    int x = 0, y = 0, z = 0;
+    for (int i = 0; i < n; ++i) {
+        const nrpn_stem_src& S = src[i];
+        if (!S.grid || S.x < 1 || S.y < 1 || S.z < 1) return NRPN_ERR_INVALID;
+        if (S.channels_last && reinterpret_cast<uintptr_t>(S.grid) % 16 != 0) return NRPN_ERR_INVALID;
+        B.src[i] = S;
+        x = S.x > x ? S.x : x; y = S.y > y ? S.y : y; z = S.z > z ? S.z : z;
+    }
+    const int X2 = (x + 1) / 2, Y2 = (y + 1) / 2, Z2 = (z + 1) / 2;
+    const size_t total = (size_t)n * X2 * Y2 * (Z2 + 1) * 8;
+    pack_stem_batch_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(B, n, X2, Y2, Z2, reinterpret_cast<__nv_bfloat16*>(packed),
+                                                                                  act_fp16 ? 1 : 0, density_to_alpha ? 1 : 0);
     NRPN_LAUNCH_CHECK();
     return NRPN_OK;
 }

@@ -9,6 +9,7 @@
 // IoU arithmetic = iou3d_aabb (utils.py:418-458 order: boxes1 = GT, boxes2 = anchor), anchors outside the padding mask
 // enter the matcher as -1.0 and end with label -1 (rpn.py:260-263, 284-286).
 #include "box_iou.cuh"
+#include "anchor_mask.cuh"
 
 namespace nrpn {
 
@@ -120,6 +121,22 @@ __global__ void __launch_bounds__(kTgtThreads) tgt_match_kernel(TgtDev P) {
     }
 }
 
+// One byte per (scene, flat anchor); the level geometry is shared, the limits are per scene.
+struct MaskParams {
+    AnchorMaskLevel lv[kMaskMaxLevels];
+    int lim[NRPN_STEM_MAX_SCENES][kMaskMaxLevels][3];
+    int n_levels, num_anchors;
+    long long total;
+};
+
+__global__ void anchor_padding_mask_kernel(const __grid_constant__ MaskParams P, int n, uint8_t* __restrict__ mask) {
+    const long long all = (long long)n * P.total;
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < all; e += (long long)gridDim.x * blockDim.x) {
+        const int b = (int)(e / P.total);
+        mask[e] = anchor_mask_value(P.lv, P.lim[b], P.n_levels, P.num_anchors, e - (long long)b * P.total);
+    }
+}
+
 }  // namespace nrpn
 
 using namespace nrpn;
@@ -155,6 +172,39 @@ int nrpn_assign_targets(const float* anchors, int n_anchors, const float* gt, in
     tgt_match_kernel<1><<<blocks, kTgtThreads, 0, st>>>(P);
     NRPN_LAUNCH_CHECK();
     tgt_match_kernel<2><<<blocks, kTgtThreads, 0, st>>>(P);
+    NRPN_LAUNCH_CHECK();
+    return NRPN_OK;
+}
+
+int nrpn_anchor_padding_mask(const int32_t* ori_sizes, int n, int px, int py, int pz, const int32_t* grid_dims, int n_levels, int num_anchors,
+                             uint8_t* mask, nrpn_stream_t stream) {
+    if (!ori_sizes || !grid_dims || !mask || n < 1 || n > NRPN_STEM_MAX_SCENES || n_levels < 1 || n_levels > kMaskMaxLevels || num_anchors < 1)
+        return NRPN_ERR_INVALID;
+    const int pad[3] = {px, py, pz};
+    MaskParams P;
+    P.n_levels = n_levels; P.num_anchors = num_anchors;
+    long long begin = 0;
+    for (int l = 0; l < n_levels; ++l) {
+        P.lv[l].begin = begin;
+        for (int a = 0; a < 3; ++a) {
+            const int g = grid_dims[3 * l + a];
+            if (g < 1 || pad[a] < g) return NRPN_ERR_INVALID;
+            P.lv[l].grid[a] = g;
+        }
+        begin += (long long)num_anchors * P.lv[l].grid[0] * P.lv[l].grid[1] * P.lv[l].grid[2];
+    }
+    P.total = begin;
+    for (int i = 0; i < n; ++i)
+        for (int l = 0; l < n_levels; ++l)
+            for (int a = 0; a < 3; ++a) {
+                const int o = ori_sizes[3 * i + a];
+                if (o < 1 || o > pad[a]) return NRPN_ERR_INVALID;
+                P.lim[i][l][a] = anchor_mask_limit(o, pad[a], P.lv[l].grid[a]);
+            }
+    const long long all = (long long)n * P.total;
+    const long long blocks = (all + 255) / 256;
+    const int cap = num_sms() * 16;
+    anchor_padding_mask_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, (cudaStream_t)stream>>>(P, n, mask);
     NRPN_LAUNCH_CHECK();
     return NRPN_OK;
 }

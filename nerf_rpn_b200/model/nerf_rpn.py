@@ -24,16 +24,20 @@ class _RPNTrainStep(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, eng, grids, targets, *params):
-        n, c, X, Y, Z = grids.shape
-        plan = eng.plan(n, (X, Y, Z))
+        plan = eng.plan_for(grids)
         plan.forward_loss(grids, targets, 1.0, 1.0, 0.0, eval_2d=True)          # the 2-D projection loss is reported like the reference does
-        ctx.eng, ctx.plan = eng, plan
+        ctx.eng, ctx.plan, ctx.forward_count = eng, plan, eng.forward_count
         losses = eng.losses.clone()
         return losses[0].clone(), losses[1].clone(), eng.loss_2d.clone()          # fresh 0-dim tensors (run_rpn.py:385-386 scales them in place)
 
     @staticmethod
     def backward(ctx, g_obj, g_reg, g_2d):
         eng, plan = ctx.eng, ctx.plan
+        if eng.forward_count != ctx.forward_count:
+            # every batch shape trains in the engine's one set of activation buffers: a later forward has overwritten this one's
+            raise RuntimeError("nerf_rpn_b200: another training forward ran on this model before this loss's backward; the CUDA training engine "
+                               "keeps the activations of one forward at a time -- call backward() after each forward (accumulate gradients "
+                               "over several backward() calls instead of summing the losses of several forwards)")
         plan.loss_grad(float(g_obj), float(g_reg), float(g_2d))          # the loss weights arrive as the upstream gradients (run_rpn.py:385-387)
         plan.backward()
         inv = 1.0 / eng.loss_scale
@@ -126,13 +130,12 @@ class NeRFRegionProposalNetwork(nn.Module):
         list and hands every parameter its gradient."""
         if targets is None:
             raise ValueError("targets should not be None")
-        if len({tuple(m.shape) for m in meshes}) != 1:
-            raise NotImplementedError("nerf_rpn_b200: a training batch must hold equally sized meshes (the reference trains with one "
-                                      "scene per rank, train.sh: batch 8 over 8 GPUs)")
         eng = self.train_engine()
         eng.overlap_allreduce = False               # gradients are returned to autograd; a DDP wrapper all-reduces them itself
         eng.sync_parameters()
-        grids = torch.stack([m if m.is_cuda else m.cuda() for m in meshes], 0).float()
+        # meshes of any sizes go to the engine as they are (each in its own memory order): it trains the batch padded to their element-wise
+        # maximum like transform() does, without materialising it -- and without padding the caller's list in place, as transform() would
+        grids = [m if (m.is_cuda and m.dtype == torch.float32) else m.cuda().float() for m in meshes]
         params = list(self.backbone.parameters()) + list(self.rpn.head.parameters())
         l_obj, l_reg, l_2d = _RPNTrainStep.apply(eng, grids, [t for t in targets], *params)
         return [None, None, None], {"loss_objectness": l_obj, "loss_rpn_box_reg": l_reg, "loss_rpn_box_reg_2d": l_2d}, None

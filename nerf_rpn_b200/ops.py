@@ -301,6 +301,55 @@ def pack_stem_input(grid: torch.Tensor, out: Optional[torch.Tensor] = None, dtyp
     return out
 
 
+def padded_extent(grids: Sequence[torch.Tensor]):
+    """Element-wise maximum (X, Y, Z) of the extents of (4,X,Y,Z) scenes: the size the reference pads a batch to (nerf_rpn.py:129-146)."""
+    return tuple(max(int(g.shape[-3 + a]) for g in grids) for a in range(3))
+
+
+def pack_stem_input_batch(grids: Sequence[torch.Tensor], out: Optional[torch.Tensor] = None, dtype=torch.bfloat16,
+                          density_to_alpha: bool = False) -> torch.Tensor:
+    """A list of differently sized (4,X_i,Y_i,Z_i) fp32 scenes -> the packed stem input of the batch zero-padded to the element-wise maximum
+    extent, (N, ceil(X/2), ceil(Y/2), ceil(Z/2)+1, 64), in one launch; the padded fp32 batch is never materialised.  Each scene is
+    contiguous NCDHW or the channels-last view the reference's dataset yields; density_to_alpha maps the real voxels only."""
+    n = len(grids)
+    if n < 1 or n > _lib.STEM_MAX_SCENES:
+        raise ValueError(f"pack_stem_input_batch: 1 to {_lib.STEM_MAX_SCENES} scenes, got {n}")
+    src = (_lib.StemSrc * n)()
+    for i, g in enumerate(grids):
+        if not isinstance(g, torch.Tensor) or not g.is_cuda or g.dtype != torch.float32 or g.dim() != 4 or g.shape[0] != 4:
+            raise RuntimeError("nerf_rpn_b200: every scene must be a (4,X,Y,Z) fp32 CUDA tensor")
+        cl = (not g.is_contiguous()) and g.permute(1, 2, 3, 0).is_contiguous()
+        if not cl and not g.is_contiguous():
+            raise ValueError("nerf_rpn_b200: a scene must be contiguous (4,X,Y,Z) or a permuted view of a contiguous (X,Y,Z,4) array")
+        src[i].grid, src[i].channels_last = g.data_ptr(), int(cl)
+        src[i].x, src[i].y, src[i].z = (int(v) for v in g.shape[1:])
+    x, y, z = padded_extent(grids)
+    shape = (n, (x + 1) // 2, (y + 1) // 2, (z + 1) // 2 + 1, 64)
+    if out is None:
+        out = torch.empty(shape, dtype=dtype, device=grids[0].device)
+    if tuple(out.shape) != shape:
+        raise ValueError(f"pack_stem_input_batch: out must be {shape}, got {tuple(out.shape)}")
+    check(lib().nrpn_pack_stem_input_batch(src, n, _ptr(out), _act16(out, "out"), int(bool(density_to_alpha)), _stream()), "pack_stem_input_batch")
+    return out
+
+
+def anchor_padding_mask(ori_sizes: Sequence[Sequence[int]], padded: Sequence[int], grid_dims: Sequence[Sequence[int]], num_anchors: int,
+                        device=None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """(N, total anchors) uint8 padding masks of a batch padded to `padded` (rpn.py:231-238 order: level, voxel (x,y,z), anchor);
+    1 = the anchor's voxel lies inside the scene's original extent, by the reference's ceil(ori / (padded // grid)) rule."""
+    n, L = len(ori_sizes), len(grid_dims)
+    ori = (ctypes.c_int32 * (3 * n))(*[int(v) for s in ori_sizes for v in s])
+    gd = (ctypes.c_int32 * (3 * L))(*[int(v) for d in grid_dims for v in d])
+    total = num_anchors * sum(int(d[0]) * int(d[1]) * int(d[2]) for d in grid_dims)
+    if out is None:
+        out = torch.empty((n, total), dtype=torch.uint8, device=device)
+    if out.dtype != torch.uint8 or out.numel() != n * total or not out.is_cuda or not out.is_contiguous():
+        raise ValueError(f"anchor_padding_mask: out must be a contiguous ({n}, {total}) uint8 CUDA tensor")
+    check(lib().nrpn_anchor_padding_mask(ori, n, int(padded[0]), int(padded[1]), int(padded[2]), gd, L, int(num_anchors), _ptr(out), _stream()),
+          "anchor_padding_mask")
+    return out
+
+
 def maxpool3d_k3s2(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """(N,X,Y,Z,C) bf16 / fp16 channels-last -> k3 s2 p1 max pool."""
     f16 = _act16(x, "x")

@@ -21,6 +21,7 @@ There is no autograd graph and no eager-PyTorch compute on this path.
 import ctypes
 import os
 import math
+from collections import OrderedDict
 from typing import List, Optional, Sequence
 
 import torch
@@ -31,6 +32,7 @@ from .engine import _down
 
 
 _TRAIN_GRAPH = os.environ.get("NRPN_TRAIN_GRAPH", "1") != "0"          # static launch lists of the training step replayed as CUDA graphs
+PLAN_CACHE = 4          # batch shapes whose per-shape state (launch lists, anchors, CUDA graphs) is kept, least recently used first out
 
 
 
@@ -195,7 +197,16 @@ class RPNTrainEngine:
         self._flatten_parameters()
         self._build_layers()
         self.bucket_elems = int(bucket_mb * (1 << 20) / 4)
-        self._plans = {}
+        # Per-shape plans are few (PLAN_CACHE, LRU); their activation / gradient buffers are views of ONE pool shared by every shape:
+        # the k-th buffer a plan requests is the first bytes of slot k, and every plan requests its buffers in the same order.  Scratch and
+        # workspaces of the backward pass are shared the same way.  A slot (or scratch buffer) only grows -- to the largest batch seen so far --
+        # and growing drops every other cached plan and graph, because they hold the old pointers.
+        self._plans = OrderedDict()
+        self._pool: List[torch.Tensor] = []
+        self._scratch = {}
+        self.pool_growths = 0
+        self.scratch_growths = 0
+        self.forward_count = 0              # training forwards run so far: a backward checks that its activations were not overwritten since
         self._graphs = {}                      # captured static launch lists (repack)
         self.comm_stream = torch.cuda.Stream(device=self.device)
         self._norm = torch.zeros(1, dtype=torch.float32, device=self.device)
@@ -293,19 +304,87 @@ class RPNTrainEngine:
 
     # ------------------------------------------------------------------------------------------------ plan
     def plan(self, n, dims):
-        key = (n, tuple(dims))
+        key = (n, tuple(int(d) for d in dims))
         p = self._plans.get(key)
-        if p is None:
-            p = _TrainPlan(self, n, tuple(dims))
-            self._plans[key] = p
+        if p is not None:
+            self._plans.move_to_end(key)
+            return p
+        p = _TrainPlan(self, n, key[1])
+        self._plans[key] = p
+        while len(self._plans) > PLAN_CACHE:
+            _, old = self._plans.popitem(last=False)
+            if any(st["graph"] is not None for st in old._graphs.values()):
+                torch.cuda.current_stream().synchronize()          # its graphs may still be in flight
+            old.release()
         return p
 
-    # ------------------------------------------------------------------------------------------------ step
-    def forward_backward(self, grids: torch.Tensor, targets: Sequence[torch.Tensor]):
-        """grids (N,4,X,Y,Z) fp32 CUDA, targets: N tensors (G,6|7).  Runs forward, losses, backward (+ the overlapped gradient
-        all-reduce when a process group is active).  Returns the loss tensor (2,) = [loss_objectness, loss_rpn_box_reg] (device)."""
+    def plan_for(self, grids):
+        """The plan of a stacked (N,4,X,Y,Z) batch, or of a list of (4,X_i,Y_i,Z_i) scenes padded to their element-wise maximum."""
+        if isinstance(grids, (list, tuple)):
+            return self.plan(len(grids), ops.padded_extent(grids))
         n, c, X, Y, Z = grids.shape
-        plan = self.plan(n, (X, Y, Z))
+        return self.plan(n, (X, Y, Z))
+
+    def cache_stats(self):
+        """Plans and captured CUDA graphs alive, pool slots and their bytes (the training step's activation / gradient memory), the shared scratch
+        and the cached plans' materialised anchors."""
+        return {"plans": len(self._plans), "graphs": sum(st["graph"] is not None for p in self._plans.values() for st in p._graphs.values()),
+                "pool_slots": len(self._pool), "pool_bytes": sum(t.numel() for t in self._pool), "pool_growths": self.pool_growths,
+                "scratch_bytes": sum(t.numel() * t.element_size() for t in self._scratch.values()), "scratch_growths": self.scratch_growths,
+                "anchor_bytes": sum(p.anchors.numel() * 4 for p in self._plans.values() if p.anchors is not None)}
+
+    def _drop_graphs(self):
+        """A scratch buffer of the backward pass is about to be replaced by a larger one: the launch lists fetch scratch when they run, so the plans
+        stay, but every captured graph holds the old pointer and goes (its plan runs eagerly twice and captures again)."""
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("nerf_rpn_b200: training buffers must not grow during graph capture")
+        self.scratch_growths += 1
+        if any(st["graph"] is not None for p in self._plans.values() for st in p._graphs.values()):
+            torch.cuda.current_stream().synchronize()
+            for p in self._plans.values():
+                p._graphs.clear()
+
+    def _drop_cached(self, keep=None):
+        """A pool slot or scratch buffer is about to be replaced by a larger one: every cached plan but `keep` (and every graph) points at the old
+        memory, so they go; `keep` runs eagerly again until its launch lists are re-captured."""
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("nerf_rpn_b200: training buffers must not grow during graph capture")
+        torch.cuda.current_stream().synchronize()
+        for key in [k for k, p in self._plans.items() if p is not keep]:
+            self._plans.pop(key).release()
+        if keep is not None:
+            keep._graphs.clear()
+        self.pool_growths += 1
+
+    def _pool_view(self, k, shape, dtype, plan):
+        """Request k of a plan under construction: the first numel elements of pool slot k, as `shape`."""
+        numel = math.prod(shape)
+        nbytes = max(numel * torch.empty((), dtype=dtype).element_size(), 1)
+        if k >= len(self._pool) or self._pool[k].numel() < nbytes:
+            if k < len(self._pool):
+                if not plan._grew:                      # once per plan: after that no other plan is left to drop
+                    self._drop_cached(keep=plan)
+                    plan._grew = True
+                self._pool[k] = None                    # nothing else refers to the old slot now: freed before the larger one is allocated
+            slot = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            if k < len(self._pool):
+                self._pool[k] = slot
+            else:
+                self._pool.append(slot)
+        return self._pool[k][:nbytes].view(dtype)[:numel].view(shape)
+
+    def density_to_alpha(self) -> bool:
+        """The model's density_to_alpha_on_device: raw densities in, datasets.py:165-167 applied by the stem packing (training and evaluation alike)."""
+        return bool(getattr(self.model, "density_to_alpha_on_device", False))
+
+    # ------------------------------------------------------------------------------------------------ step
+    def forward_backward(self, grids, targets: Sequence[torch.Tensor]):
+        """grids: (N,4,X,Y,Z) fp32 CUDA, or a list of N (4,X_i,Y_i,Z_i) fp32 CUDA scenes of different sizes (each contiguous or the dataset's
+        channels-last view), trained as the batch zero-padded to their element-wise maximum like the reference does (nerf_rpn.py:129-146,
+        anchors in the padding labelled -1); targets: N tensors (G,6|7).  Runs forward, losses, backward (+ the overlapped gradient
+        all-reduce when a process group is active).  Returns the loss tensor (2,) = [loss_objectness, loss_rpn_box_reg] (device).
+        One step at a time: every shape shares the engine's buffers."""
+        plan = self.plan_for(grids)
         plan.run(grids, targets)
         return self.losses
 
@@ -337,26 +416,31 @@ class _TrainPlan:
         self.bwd: List = []                      # built in forward order, executed reversed
         self.bwd_lo: List[int] = []              # lowest flat-parameter offset whose gradient is final once bwd[i] has run
         self.f16 = eng.f16
-        self._scratch = {}
+        self._scratch = eng._scratch             # shared by every plan (engine-level, grows to the largest batch)
         self._graphs = {}
-        self._ws = None
+        self._grew = False
         X, Y, Z = dims
         L = lib()
+        n_req = [0]
 
-        def buf(d, c, dtype=dt, zero=False):
-            f = torch.zeros if zero else torch.empty
-            return f((n, *d, c), dtype=dtype, device=dev)
+        def req(shape, dtype=dt):
+            t = eng._pool_view(n_req[0], tuple(shape), dtype, self)
+            n_req[0] += 1
+            return t
+
+        def buf(d, c, dtype=dt):
+            return req((n, *d, c), dtype)
 
         self.input = None
         d1 = _down(dims)
-        self.packed = torch.empty((n, d1[0], d1[1], d1[2] + 1, 64), dtype=dt, device=dev)
-        self.fwd.append(lambda: ops.pack_stem_input(self._src, self.packed))
+        self.packed = req((n, d1[0], d1[1], d1[2] + 1, 64))
+        self.fwd.append(self._pack_input)
         y0 = buf(d1, 64); a0 = buf(d1, 64)
         self._conv_fwd(eng.stem, self.packed, (d1[0], d1[1], d1[2] + 1), y0, d1)
         self._bn_fwd(eng.stem_bn, y0, None, a0, True)
         d2 = _down(d1)
         p0 = buf(d2, 64)
-        self.pool_idx = torch.empty((n, *d2, 64), dtype=torch.uint8, device=dev)
+        self.pool_idx = buf(d2, 64, torch.uint8)
         self.fwd.append(lambda: check(L.nrpn_maxpool3d_k3s2_argmax(_p(a0), n, d1[0], d1[1], d1[2], 64, _p(p0), _p(self.pool_idx), self.f16, _stream()), "maxpool_argmax"))
         dp0 = buf(d2, 64)                          # gradient w.r.t. the pooled map
         da0 = buf(d1, 64); dy0 = buf(d1, 64)
@@ -450,10 +534,10 @@ class _TrainPlan:
             for d, v in zip(fdims, vox):
                 out.append(t[o:o + n * v].view(n, *d, t.shape[-1])); o += n * v
             return out
-        hs = [torch.empty((self.total_vox, 256), dtype=dt, device=dev) for _ in eng.hconv]
-        dhs = [torch.empty((self.total_vox, 256), dtype=dt, device=dev) for _ in eng.hconv]
-        self.pred = torch.empty((self.total_vox, 128), dtype=torch.float32, device=dev)
-        self.dpred = torch.zeros((self.total_vox, 128), dtype=dt, device=dev)
+        hs = [req((self.total_vox, 256)) for _ in eng.hconv]
+        dhs = [req((self.total_vox, 256)) for _ in eng.hconv]
+        self.pred = req((self.total_vox, 128), torch.float32)
+        self.dpred = req((self.total_vox, 128))             # zeroed by every loss_grad
         cur = feats
         for k, layer in enumerate(eng.hconv):
             nxt = level_views(hs[k])
@@ -487,17 +571,33 @@ class _TrainPlan:
         self.bwd.append(head_bwd)
         self.bwd_lo.append(min(eng.offsets[id(p_)][0] for p_ in eng.head.parameters()))
         self._src = None
+        self._sizes = None
+        self._alpha = False
+        self.valid = None
         self.anchors = None
+        if self._grew:
+            torch.cuda.empty_cache()            # hand the replaced (smaller) slots back instead of keeping them cached next to the new ones
+
+    def release(self):
+        """Drops everything this plan holds -- pool views, anchors, launch lists, CUDA graphs -- when the engine evicts it or replaces the pool
+        slots it points at.  The launch lists are closures over the plan, so without this the memory would wait for Python's cyclic collector.
+        A released plan cannot run again."""
+        self.__dict__.clear()
+        self.released = True
+
+    def _check_live(self):
+        if getattr(self, "released", False):
+            raise RuntimeError("nerf_rpn_b200: this training plan was released (evicted, or its buffers were replaced by a larger batch)")
 
     # ------------------------------------------------------------------------------------------------ helpers
     def _workspace(self, nbytes):
-        if self._ws is None or self._ws.numel() < nbytes:
-            self._ws = torch.empty(max(int(nbytes), 1 << 20), dtype=torch.uint8, device=self.eng.device)
-        return self._ws
+        return self._scratch_buf("workspace", max(int(nbytes), 1 << 20), torch.uint8)
 
     def _scratch_buf(self, name, numel, dtype):
         t = self._scratch.get(name)
         if t is None or t.numel() < numel or t.dtype != dtype:
+            if t is not None:
+                self.eng._drop_graphs()                     # captured graphs hold the old pointer
             t = torch.empty(int(numel), dtype=dtype, device=self.eng.device)
             self._scratch[name] = t
         return t[:numel]
@@ -648,26 +748,56 @@ class _TrainPlan:
         perm2 = torch.randperm(negative.numel(), device=negative.device, generator=g)[:num_neg]
         return positive[perm1].contiguous(), negative[perm2].contiguous()
 
-    def forward_loss(self, grids, targets, w_obj=1.0, w_reg=None, w_2d=None, eval_2d=False):
-        """Forward launches, target assignment, sampling, losses; fills d(pred) for the weighted sum w_obj * L_obj + w_reg * L_reg (+ w_2d * L_2d)."""
-        eng, n = self.eng, self.n
-        if ops.is_channels_last_grid(grids) or grids.is_contiguous():
-            self._src = grids
+    def _pack_input(self):
+        if self._sizes is not None:
+            ops.pack_stem_input_batch(self._src, self.packed, density_to_alpha=self._alpha)
         else:
-            self._src = grids.contiguous()
+            ops.pack_stem_input(self._src, self.packed, density_to_alpha=self._alpha)
+
+    def _set_input(self, grids):
+        """The caller's batch for the stem packing: a stacked (N,4,X,Y,Z) grid, or a list of scenes whose padded extent is this plan's dims."""
+        self._alpha = self.eng.density_to_alpha()
+        if isinstance(grids, (list, tuple)):
+            if len(grids) != self.n or ops.padded_extent(grids) != tuple(self.dims):
+                raise ValueError(f"nerf_rpn_b200: this plan trains {self.n} scenes padded to {self.dims}")
+            self._src = [g if (g.is_contiguous() or g.permute(1, 2, 3, 0).is_contiguous()) else g.contiguous() for g in grids]
+            self._sizes = [tuple(int(v) for v in g.shape[-3:]) for g in grids]
+            return
+        if self._alpha and grids.dtype == torch.uint8:
+            raise NotImplementedError("density_to_alpha on the device is fused into the fp32 stem packing (uint8 grids hold alphas already)")
+        self._src = grids if (ops.is_channels_last_grid(grids) or grids.is_contiguous()) else grids.contiguous()
+        self._sizes = None
+
+    def padding_masks(self):
+        """(N, anchors) uint8 padding masks of the current batch (None when no scene is padded): AnchorGenerator3D.get_padding_masks."""
+        if self._sizes is None or all(s == tuple(self.dims) for s in self._sizes):
+            return None
+        return ops.anchor_padding_mask(self._sizes, self.dims, self.feat_dims, self.eng.A, device=self.eng.device)
+
+    def forward_loss(self, grids, targets, w_obj=1.0, w_reg=None, w_2d=None, eval_2d=False):
+        """Forward launches, target assignment, sampling, losses; fills d(pred) for the weighted sum w_obj * L_obj + w_reg * L_reg (+ w_2d * L_2d).
+        grids: the stacked batch or the list of differently sized scenes (see RPNTrainEngine.forward_backward)."""
+        self._check_live()
+        eng, n = self.eng, self.n
+        eng.forward_count += 1
+        self._set_input(grids)
         self.fwd[0]()                                               # stem packing reads the caller's grid: its pointer changes from step to step
         _replay_static(self._graphs, "fwd", self.fwd[1:])
         anchors = self._anchors()
+        self.valid = valid = self.padding_masks()
         samples = []
         forced = getattr(self, "forced_samples", None)         # tests: (pos, neg) index tensors per mesh instead of the sampler's draw
         for i in range(n):
             gt = targets[i].to(device=eng.device, dtype=torch.float32).contiguous()
+            vi = None if valid is None else valid[i]
             if gt.numel() == 0:                                     # background mesh (rpn.py:246-250): every anchor is a negative
                 labels = torch.zeros(anchors.shape[0], dtype=torch.float32, device=eng.device)
+                if vi is not None:                                  # ... except those in the padding (rpn.py:283-285): -1
+                    labels = vi.to(torch.float32) - 1.0
                 pos, neg = self._sample(labels)
                 samples.append((pos, neg, torch.zeros((0, 7 if eng.rotated else 6), dtype=torch.float32, device=eng.device)))
                 continue
-            labels, idx = ops.assign_targets(anchors, gt, None, eng.rpn.fg_iou_thresh, eng.rpn.bg_iou_thresh, True)
+            labels, idx = ops.assign_targets(anchors, gt, vi, eng.rpn.fg_iou_thresh, eng.rpn.bg_iou_thresh, True)
             pos, neg = self._sample(labels) if forced is None else (forced[i][0].contiguous(), forced[i][1].contiguous())
             samples.append((pos, neg, gt[idx[pos].clamp(min=0)].contiguous()))
         self.last_samples = samples
@@ -796,6 +926,7 @@ class _TrainPlan:
         """Backward launches in reverse construction order.  Gradients become final from the END of the flat bucket (head, FPN) towards
         its start (stem): every time >= bucket_elems new elements are final their all-reduce is launched on the comm stream, overlapping
         the dgrad / wgrad of the layers below (run_rpn.py:235-236: DDP's bucketed all-reduce during loss.backward())."""
+        self._check_live()
         eng = self.eng
         if not (eng.world > 1 and eng.overlap_allreduce):
             self.allreduce_calls = 0
