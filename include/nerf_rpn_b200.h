@@ -195,11 +195,11 @@ int nrpn_maxpool3d_k2s2_ceil(const void *in, int n, int x, int y, int z, int c, 
  * input rows y = yp-1, yp (56 channels + 8 zero), so that the conv is a 7x4-tap implicit GEMM with K = 64 per tap. */
 int nrpn_pack_stem_input_s1(const float *grid, int n, int x, int y, int z, void *packed, int act_fp16, nrpn_stream_t stream);
 
-/* GroupNorm(32 groups, 256 channels) + optional ReLU, in place, on up to NRPN_CONV_MAX_LEVELS channels-last bf16 tensors
+/* GroupNorm(32 groups, 256 channels) + optional ReLU, in place, on up to NRPN_CONV_MAX_LEVELS channels-last 16-bit tensors
  * (N, voxels, 256) that share gamma/beta (FCOS towers: Conv3d -> GroupNorm -> ReLU, fcos/fcos.py:43-69).  Statistics are
  * per (sample, level, group); reductions run in a fixed order (bit-reproducible). */
 typedef struct {
-    void *x;          /* bf16 (N, voxels, 256), normalised in place */
+    void *x;          /* 16-bit (N, voxels, 256), bf16 or fp16 (act_fp16), normalised in place */
     int32_t voxels;
 } nrpn_gn_level;
 size_t nrpn_groupnorm_workspace_bytes(int n_levels, int n);
@@ -240,10 +240,10 @@ int nrpn_rpn_proposals(const nrpn_rpn_desc *desc /*host*/, float *boxes, float *
                        int32_t *count, void *workspace, size_t workspace_bytes, nrpn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Swin-3D support (SwinTransformer_FPN, feature_extractor.py:382-789). Token grids are channels-last bf16 (N,H,W,D,ld) with
- * C real channels, ld >= C; the Linear layers run through nrpn_conv3d_fprop as 1x1x1 convolutions.
+ * Swin-3D support (SwinTransformer_FPN, feature_extractor.py:382-789). Token grids are channels-last 16-bit (N,H,W,D,ld), bf16
+ * or fp16 as act_fp16 selects, with C real channels, ld >= C; the Linear layers run through nrpn_conv3d_fprop as 1x1x1 convolutions.
  * ---------------------------------------------------------------------------------------------- */
-/* fp32 NCDHW grid (N,4,X,Y,Z) -> bf16 (N, X/4, Y/4, Z/4, 256) patch rows, channel ((c*4+px)*4+py)*4+pz: the patch embedding
+/* fp32 NCDHW grid (N,4,X,Y,Z) -> 16-bit (N, X/4, Y/4, Z/4, 256) patch rows, channel ((c*4+px)*4+py)*4+pz: the patch embedding
  * Conv3d(4, C, kernel 4, stride 4) becomes a 256 -> C GEMM. */
 int nrpn_patch_embed_pack(const float *grid, int n, int x, int y, int z, void *out, int act_fp16, nrpn_stream_t stream);
 /* per-token LayerNorm over the first c channels of each row; rows are ld_in / ld_out elements apart. */

@@ -1,5 +1,5 @@
-// GroupNorm(32, 256) + ReLU on channels-last bf16 activations, in place (FCOS towers: Conv3d -> GroupNorm -> ReLU,
-// nerf_rpn/model/fcos/fcos.py:43-69).  Statistics are per (sample, pyramid level, group) over 8 channels x all voxels.
+// GroupNorm(32, 256) + ReLU on channels-last 16-bit (bf16 or fp16, selected by act_fp16) activations, in place (FCOS towers,
+// Conv3d -> GroupNorm -> ReLU, fcos/fcos.py:43-69).  Statistics are per (sample, pyramid level, group) over 8 channels x all voxels.
 // Two kernels per call, HBM bound: (1) per-CTA partial sums (fp32 per thread, fp64 across threads) written to a scratch
 // array, (2) every CTA first reduces the partials of its (sample, level) in a FIXED order (bit-reproducible), then applies
 // y = relu((x - mean) * rstd * gamma + beta).  One thread owns one 16-byte chunk = the 8 channels of one group of one

@@ -1,11 +1,11 @@
 // Swin-3D support kernels (SwinTransformer_FPN, nerf_rpn/model/feature_extractor.py:382-789). The GEMMs of the transformer
 // (qkv, proj, MLP, patch merging, patch embedding) run on the wgmma implicit-GEMM kernel as 1x1x1 convolutions over
 // channels-last token grids; this file holds what is left around them:
-//   patch_embed_pack      fp32 NCDHW grid -> (X/4, Y/4, Z/4, 256) bf16 patch rows    (Conv3d k4 s4 as a GEMM, :731-733)
+//   patch_embed_pack      fp32 NCDHW grid -> (X/4, Y/4, Z/4, 256) 16-bit patch rows  (Conv3d k4 s4 as a GEMM, :731-733)
 //   layernorm             per-token LayerNorm over C channels                        (:621,634,736)
 //   patch_merge_ln        2x2x2 gather (zero pad on odd extents) + LayerNorm(8C)     (:661-685)
 //   window_attention      4^3 shifted-window multi-head attention, head_dim 32        (:382-497)
-// Activations are (N, H, W, D, ld) bf16 with C real channels and ld >= C (ld a multiple of 64; channels [C, ld) stay zero).
+// Activations are (N, H, W, D, ld) 16-bit -- bf16 or fp16, selected by act_fp16 -- with C real channels and ld >= C.
 #include "common.cuh"
 #include "wgmma.cuh"
 

@@ -430,7 +430,7 @@ def rpn_proposals(desc: RpnDesc, device, out=None, workspace: Optional[torch.Ten
 # ------------------------------------------------------------------------------------------------ FCOS
 def groupnorm_relu_(levels: Sequence[torch.Tensor], gamma: torch.Tensor, beta: torch.Tensor, eps: float = 1e-5, relu: bool = True,
                     groups: int = 32, workspace: Optional[torch.Tensor] = None):
-    """In-place GroupNorm(groups, C) (+ReLU) on channels-last bf16 tensors (N, X, Y, Z, C) that share gamma / beta."""
+    """In-place GroupNorm(groups, C) (+ReLU) on channels-last 16-bit tensors (N, X, Y, Z, C), bf16 or fp16, that share gamma / beta."""
     n, c = levels[0].shape[0], levels[0].shape[-1]
     arr = (GnLevel * len(levels))()
     for i, t in enumerate(levels):
@@ -562,7 +562,7 @@ def patch_embed_pack(grid: torch.Tensor, out: torch.Tensor):
 
 
 def layernorm(x: torch.Tensor, out: torch.Tensor, c: int, gamma: torch.Tensor, beta: torch.Tensor, eps: float = 1e-5):
-    """x, out: (..., ld) bf16 channels-last; normalises the first c channels of every row."""
+    """x, out: (..., ld) 16-bit (bf16 or fp16, both the same) channels-last; normalises the first c channels of every row."""
     tokens = x.numel() // x.shape[-1]
     check(lib().nrpn_layernorm(_ptr(x), int(x.shape[-1]), _ptr(out), int(out.shape[-1]), tokens, int(c), _ptr(gamma), _ptr(beta),
                                float(eps), _act16(x, "x"), _stream()), "layernorm")

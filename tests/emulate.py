@@ -1,5 +1,6 @@
-"""Pure-torch statement of what nrpn_conv3d_fprop / nrpn_pack_stem_input compute (TEST helper, CPU or GPU).
-Used to check the host-side packing logic without a GPU and as the fp32 / float64 references for the CUDA kernels."""
+"""Pure-torch statement of what nrpn_conv3d_fprop / nrpn_pack_stem_input and the Swin-3D / GroupNorm kernels compute (TEST
+helper, CPU or GPU).  Used to check the host-side packing logic without a GPU and as the fp32 / float64 references for the CUDA
+kernels."""
 import math
 
 import torch
@@ -96,6 +97,148 @@ def reference_conv64(x, w, taps, shift, out_dims, stride=1, act=0, res=None):
     elif act == 2:
         ref = 0.5 * ref * (1.0 + torch.erf(ref / math.sqrt(2.0)))
     return ref, mag
+
+
+def _relative_position_index() -> torch.Tensor:
+    """(64 * 64) index into the 343-row relative-position bias table of a 4^3 window, query-major, as the model builds it."""
+    from nerf_rpn_b200.model.feature_extractor import ShiftedWindowAttention
+    return ShiftedWindowAttention(32, [4, 4, 4], [0, 0, 0], 1).relative_position_index.clone()
+
+
+def reference_window_attention64(qkv, qkv_bias, table, heads, shift, fmt, flaw=None):
+    """float64 statement of nrpn_window_attention on the exact operands the kernel reads (CPU or GPU).
+
+    qkv (N,H,W,D,ld) 16-bit holding [q | k | v] in its first 3C columns (C = 32 heads, head-major); qkv_bias (3C) fp32;
+    table (343, heads) fp32; fmt the 16-bit format.  Zero-padded tokens enter the qkv Linear as zeros, so they carry qkv_bias --
+    rounded to fmt, as the kernel packs it (real tokens reach it already rounded by the qkv GEMM).  Pad to multiples of 4,
+    roll by -shift on every axis whose padded extent exceeds 4, split into 4^3 windows, softmax(q.k / sqrt(32) + relative-
+    position bias - 100 between tokens of different shift regions) . v, roll back, crop.
+    Returns (ref, scale), float64 (N,H,W,D,C): scale = sum_j p_j |v_j|, the magnitude the rounding of p scales with.
+    flaw: a deliberate mistake, for the negative controls of tests/test_norm_attention_reference_cpu.py -- "mask_h_omitted"
+    (no region split along H), "mask_unshifted_axes" (regions of the requested shift on every axis), "index_transposed"
+    (bias of j - i instead of i - j), "pad_zero" (padding tokens zero instead of the bias), "no_scale" (no 1/sqrt(32))."""
+    n, H, W, D, _ = qkv.shape
+    C, dev, win = heads * 32, qkv.device, 4
+    PH, PW, PD = (-(-e // win) * win for e in (H, W, D))
+    sh = [0 if win >= e else shift for e in (PH, PW, PD)]
+    bias = qkv_bias.to(dev).to(fmt).double()
+    if flaw == "pad_zero":
+        bias = torch.zeros_like(bias)
+    xp = bias.expand(n, PH, PW, PD, 3 * C).clone()
+    xp[:, :H, :W, :D] = qkv[..., :3 * C].double()
+    xp = torch.roll(xp, shifts=(-sh[0], -sh[1], -sh[2]), dims=(1, 2, 3))
+    nh, nw, nd = PH // win, PW // win, PD // win
+    t = xp.view(n, nh, win, nw, win, nd, win, 3 * C).permute(0, 1, 3, 5, 2, 4, 6, 7).reshape(-1, 64, 3, heads, 32)
+    q, k, v = t.permute(2, 0, 3, 1, 4)                      # (windows, heads, 64, 32) each
+    if flaw != "no_scale":
+        q = q * 32 ** -0.5
+    attn = q @ k.transpose(-2, -1)
+    idx = _relative_position_index()
+    if flaw == "index_transposed":
+        idx = idx.view(64, 64).t().reshape(-1)
+    attn = attn + table.to(dev).double()[idx.to(dev)].view(64, 64, heads).permute(2, 0, 1)
+    if sum(sh) > 0:
+        mask_sh = [shift] * 3 if flaw == "mask_unshifted_axes" else sh
+        labels = []
+        for axis, (P, s) in enumerate(zip((PH, PW, PD), mask_sh)):
+            lab = torch.zeros(P, dtype=torch.float64, device=dev)
+            for r, (lo, hi) in enumerate(((0, -win), (-win, -s), (-s, None))):   # s == 0: (-4, -0) is empty, (-0, None) all
+                lab[lo:hi] = r
+            if flaw == "mask_h_omitted" and axis == 0:
+                lab.zero_()
+            labels.append(lab)
+        region = labels[0].view(-1, 1, 1) * 9 + labels[1].view(1, -1, 1) * 3 + labels[2].view(1, 1, -1)
+        region = region.view(nh, win, nw, win, nd, win).permute(0, 2, 4, 1, 3, 5).reshape(-1, 64)
+        mask = (region[:, :, None] != region[:, None, :]).double() * -100.0
+        attn = (attn.view(n, -1, heads, 64, 64) + mask[None, :, None]).view(-1, heads, 64, 64)
+    p = torch.softmax(attn, dim=-1)
+
+    def unwindow(o):
+        o = o.transpose(1, 2).reshape(n, nh, nw, nd, win, win, win, C).permute(0, 1, 4, 2, 5, 3, 6, 7).reshape(n, PH, PW, PD, C)
+        return torch.roll(o, shifts=tuple(sh), dims=(1, 2, 3))[:, :H, :W, :D].contiguous()
+    return unwindow(p @ v), unwindow(p @ v.abs())
+
+
+def _normalize64(x, dims, eps, unbiased=False, amplify=False):
+    """float64 x normalised over `dims` with the biased variance (the unbiased one only as a negative control).  Returns
+    (x_hat, mag): mag = |x_hat| a + mean|x| / sigma, a = E[x^2] / (var + eps) if amplify else 1 -- what an fp32 statistic's
+    relative error is multiplied by on its way to the output (divided by |gamma|)."""
+    cnt = math.prod(x.shape[d] for d in dims)
+    mu = x.mean(dims, keepdim=True)
+    d = x - mu
+    var = (d * d).sum(dims, keepdim=True) / (cnt - 1 if unbiased else cnt)
+    sigma = torch.sqrt(var + eps)
+    xh = d / sigma
+    a = (x * x).mean(dims, keepdim=True) / (var + eps) if amplify else 1.0
+    return xh, xh.abs() * a + x.abs().mean(dims, keepdim=True) / sigma
+
+
+def reference_layernorm64(x, C, gamma, beta, eps, flaw=None):
+    """float64 statement of nrpn_layernorm: LayerNorm over the first C channels of each row of x (..., ld), 16-bit; the
+    channels [C, ld) are not read.  Returns (ref, scale), float64 (..., C): scale = |gamma| (|x_hat| + mean|x| / sigma) + |beta|,
+    the magnitude the fp32 statistics' and the affine step's rounding scale with.  flaw "unbiased": variance over C - 1."""
+    xh, mag = _normalize64(x[..., :C].double(), (-1,), eps, unbiased=flaw == "unbiased")
+    g, b = gamma.to(x.device).double(), beta.to(x.device).double()
+    return xh * g + b, mag * g.abs() + b.abs()
+
+
+MERGE_PARITY = ((0, 0, 0), (1, 0, 0), (0, 1, 0), (1, 1, 0), (0, 0, 1), (1, 0, 1), (0, 1, 1), (1, 1, 1))
+
+
+def reference_patch_merge64(x, C, gamma, beta, eps, flaw=None):
+    """float64 statement of nrpn_patch_merge_ln: x (N,H,W,D,ld) 16-bit, first C channels read; output token (i,j,k) is the
+    LayerNorm(8C) of the input tokens (2i+a, 2j+b, 2k+c) concatenated in parity order 000,100,010,110,001,101,011,111 (over H,W,D),
+    zero past an odd extent.  Returns (ref, scale) as reference_layernorm64, (N, ceil(H/2), ceil(W/2), ceil(D/2), 8C).
+    flaw: "swap_100_010" (those two parts exchanged), "edge_replicate" (the last plane repeated past an odd extent)."""
+    xs = x[..., :C].double()
+    for axis in (1, 2, 3):
+        if xs.shape[axis] % 2:
+            edge = xs.narrow(axis, xs.shape[axis] - 1, 1)
+            xs = torch.cat([xs, edge if flaw == "edge_replicate" else torch.zeros_like(edge)], axis)
+    order = list(MERGE_PARITY)
+    if flaw == "swap_100_010":
+        order[1], order[2] = order[2], order[1]
+    merged = torch.cat([xs[:, a::2, b::2, c::2] for a, b, c in order], -1)
+    return reference_layernorm64(merged, 8 * C, gamma, beta, eps)
+
+
+def reference_groupnorm64(levels, gamma, beta, eps, relu, flaw=None):
+    """float64 statement of nrpn_groupnorm_relu: levels a list of (N, ..., 256) 16-bit tensors; 32 groups of 8 consecutive
+    channels; mean and biased variance per (sample, level, group) over the group's channels and every voxel; then
+    x_hat gamma + beta, and ReLU if relu.  Returns (refs, scales), lists of float64 (N, ..., 256):
+    scale = |gamma| (|x_hat| E[x^2] / (var + eps) + mean|x| / sigma) + |beta| (before the ReLU) -- the kernel forms the variance
+    as E[x^2] - mean^2, so a relative error of E[x^2] reaches the output multiplied by E[x^2] / var.
+    flaw: "unbiased" (variance over count - 1), "group_mod32" (channel c in group c % 32), "pooled" (statistics over all samples)."""
+    refs, scales = [], []
+    for x in levels:
+        n, shape = x.shape[0], x.shape
+        xs = x.double().reshape(n, -1, 256)
+        if flaw == "group_mod32":
+            g = xs.view(n, -1, 8, 32)                                # group = c % 32: the last index
+            dims = (1, 2)
+        else:
+            g = xs.view(n, -1, 32, 8)                                # group = c // 8
+            dims = (1, 3)
+        if flaw == "pooled":
+            dims = (0,) + dims
+        xh, mag = _normalize64(g, dims, eps, unbiased=flaw == "unbiased", amplify=True)
+        xh, mag = xh.reshape(shape), mag.reshape(shape)
+        ga, be = gamma.to(x.device).double(), beta.to(x.device).double()
+        y = xh * ga + be
+        refs.append(y.clamp_min(0) if relu else y)
+        scales.append(mag * ga.abs() + be.abs())
+    return refs, scales
+
+
+def reference_patch_embed(grid):
+    """nrpn_patch_embed_pack: fp32 (N,4,X,Y,Z) -> float64 (N, X/4, Y/4, Z/4, 256), row (i,j,k) channel ((c*4+px)*4+py)*4+pz =
+    grid[c][4i+px][4j+py][4k+pz] (remainders of X, Y, Z past a multiple of 4 unused) -- the patch embedding Conv3d(4, C, 4,
+    stride 4) as a 256 -> C GEMM with the weight flattened in (c, px, py, pz) order.  Exact: compare it bit for bit after
+    rounding to the 16-bit format."""
+    n, c, X, Y, Z = grid.shape
+    H, W, D = X // 4, Y // 4, Z // 4
+    g = grid[:, :, :4 * H, :4 * W, :4 * D].double().reshape(n, c, H, 4, W, 4, D, 4)
+    return g.permute(0, 2, 4, 6, 1, 3, 5, 7).reshape(n, H, W, D, 256)
 
 
 def emulate_pack_stem_s1(grid: torch.Tensor) -> torch.Tensor:
