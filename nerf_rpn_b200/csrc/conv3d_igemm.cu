@@ -19,10 +19,11 @@
 //     tile list that may span up to 4 pyramid levels sharing the same weights (the RPN head on P2..P5 is ONE launch per
 //     layer).  Prologue (barriers, tensor-map prefetch) runs ahead of griddepcontrol.wait (programmatic dependent launch).
 //   - epilogue (fused): + shift (bias / folded BN), + residual (same shape, or nearest-upsampled coarser level for the FPN
-//     top-down path), ReLU / GELU, convert to bf16 / fp16 / fp32; or -- TMA_EPI variant of the 1^3 layers -- residual tiles
-//     prefetched by TMA into shared memory and output tiles stored with cp.async.bulk.tensor.
-//   - variants: <256,4,1> <128,6,1> <64,8,1> (long reductions; <64,8,1> also for layers with fewer tiles than SMs),
-//     <64,2,3> / <64,2,2,TMA_EPI> (reductions of at most 8 k-blocks).
+//     top-down path), ReLU / GELU, convert to bf16 / fp16 / fp32.  TMA_EPI variants (16-bit output) stage the tile in shared
+//     memory as 128 x 64 sub-tiles and store each with cp.async.bulk.tensor; the short reductions also prefetch a same-shape
+//     residual by TMA.
+//   - variants: <256,4,1> <128,6,1> <64,8,1> (long reductions, each with and without TMA_EPI; <64,8,1> also for layers with
+//     fewer tiles than SMs), <64,2,3> / <64,2,2,TMA_EPI> (reductions of at most 8 k-blocks).
 #include <cstdlib>
 #include <type_traits>
 #include "common.cuh"
@@ -68,6 +69,12 @@ struct ConvMaps {
 
 constexpr int kEpiTileBytes = kBlockM * 64 * 2;      // one 128 x 64 bf16 tile (residual in / output out of the TMA epilogue)
 
+// Shared-memory tiles of the TMA epilogue (see conv3d_igemm_kernel): residual prefetch ring and output staging buffers.
+// The short reductions run 2 CTAs per SM and have room for one staging buffer and a residual ring of 2 (1 with split weights);
+// the long reductions run 1 CTA per SM and double-buffer the staging.
+__host__ __device__ constexpr int epi_res_slots(int min_blocks, bool tma_epi, bool ws) { return tma_epi && min_blocks > 1 ? (ws ? 1 : 2) : 0; }
+__host__ __device__ constexpr int epi_out_slots(int min_blocks, bool tma_epi) { return tma_epi ? (min_blocks > 1 ? 1 : 2) : 0; }
+
 struct TilePos { int l, tix, tiy, tiz, nb; };
 
 __device__ __forceinline__ TilePos tile_pos(const ConvDev& P, int m_tile) {
@@ -88,7 +95,8 @@ struct RowPos { bool valid; size_t vox; const __nv_bfloat16* rrow; };
 
 __device__ __forceinline__ RowPos row_pos(const ConvLevelDev& L, const TilePos& p, int row) {
     RowPos r;
-    const int zi = row % L.bz, yi = (row / L.bz) % L.by, xi = row / (L.bz * L.by);
+    const int lz = __ffs(L.bz) - 1, ly = __ffs(L.by) - 1;             // brick sides are powers of two (choose_brick)
+    const int zi = row & (L.bz - 1), yi = (row >> lz) & (L.by - 1), xi = row >> (lz + ly);
     const int gx = p.tix * L.bx + xi, gy = p.tiy * L.by + yi, gz = p.tiz * L.bz + zi;
     r.valid = gx < L.xo && gy < L.yo && gz < L.zo;
     r.vox = (((size_t)p.nb * L.xo + gx) * L.yo + gy) * L.zo + gz;
@@ -111,10 +119,14 @@ __device__ __forceinline__ float activate(float v, int relu) {
     return v;
 }
 
-// TMA_EPI (N = 64 tiles of the HBM-bound 1^3 layers, bf16 output, Cout % 64 == 0): the epilogue never touches global memory
-// from a register.  The producer warp prefetches the residual tile of a same-shape skip connection into shared memory
-// (2-deep ring) together with the operands; the consumers add it from shared memory, write the 16-bit tile into a
-// swizzled staging buffer and one thread stores it with cp.async.bulk.tensor (hardware clips partial bricks).
+// TMA_EPI (16-bit output): the consumers write the tile, 64 channels at a time, into a swizzled 128 x 64 staging buffer and
+// one thread stores it with cp.async.bulk.tensor (hardware clips partial bricks and channels past Cout).
+//   - short reductions (N = 64 tiles of the HBM-bound 1^3 layers, 2 CTAs / SM, Cout % 64 == 0): the producer warp also
+//     prefetches the residual tile of a same-shape skip connection into shared memory (2-deep ring) with the operands, and
+//     the epilogue never reads global memory from a register.  One staging buffer.
+//   - long reductions (1 CTA / SM): any residual is read from global memory as in the register epilogue.  Two staging
+//     buffers, so that the consumers fill one while the previous sub-tile's store reads the other: the tensor pipe idles
+//     for the shared-memory writes only, not for scattered 4-byte global stores.
 //
 // WS (weight split, the <=1e-3 parity mode of the backbone): every weight is the sum of TWO 16-bit numbers, w = hi + lo with
 // lo = round16(w - hi), packed as (taps, 2, CoutPad, Cin).  One TMA box {64, BLOCK_N, 2} brings both planes of a k-block; the
@@ -122,17 +134,18 @@ __device__ __forceinline__ float activate(float v, int relu) {
 // weights enter the fp32 accumulation with ~22 significant bits and only the activations carry 16-bit rounding error.
 template <int BLOCK_N, int STAGES, int MIN_BLOCKS, bool TMA_EPI = false, bool WS = false>
 __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(const __grid_constant__ ConvMaps maps, const ConvDev P) {
-    static_assert(!TMA_EPI || BLOCK_N == 64, "the TMA epilogue stages 128 x 64 tiles");
     constexpr int kBPlane = BLOCK_N * kBlockK * 2;
     constexpr int kBBytes = kBPlane * (WS ? 2 : 1);
     constexpr int kStageBytes = kABytes + kBBytes;
-    constexpr int RES_SLOTS = (TMA_EPI && WS) ? 1 : 2;              // residual prefetch depth (shared-memory budget of 2 CTAs / SM)
-    constexpr int kEpiBytes = TMA_EPI ? (RES_SLOTS + 1) * kEpiTileBytes : 0;      // residual ring + output staging (1)
+    constexpr bool kResRing = TMA_EPI && MIN_BLOCKS > 1;                // the short reductions' residual prefetch
+    constexpr int RES_SLOTS = epi_res_slots(MIN_BLOCKS, TMA_EPI, WS);
+    constexpr int OUT_SLOTS = epi_out_slots(MIN_BLOCKS, TMA_EPI);
+    constexpr int kEpiBytes = (RES_SLOTS + OUT_SLOTS) * kEpiTileBytes;  // residual ring + output staging
 
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* smem_res = smem + STAGES * kStageBytes;                 // [2][128 rows][128 B], 128B-swizzled (TMA_EPI)
-    uint8_t* smem_out = smem_res + RES_SLOTS * kEpiTileBytes;        // [128 rows][128 B], 128B-swizzled (TMA_EPI)
+    uint8_t* smem_res = smem + STAGES * kStageBytes;                 // [RES_SLOTS][128 rows][128 B], 128B-swizzled
+    uint8_t* smem_out = smem_res + RES_SLOTS * kEpiTileBytes;        // [OUT_SLOTS][128 rows][128 B], 128B-swizzled
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * kStageBytes + kEpiBytes);
     uint64_t* full_bar = bars;
     uint64_t* empty_bar = bars + STAGES;
@@ -146,7 +159,8 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
         for (int a = 0; a < 2; ++a) { ptx::mbar_init(&rfull_bar[a], 1); ptx::mbar_init(&rempty_bar[a], 1); }
         ptx::fence_barrier_init();
         for (int l = 0; l < P.n_levels; ++l) ptx::prefetch_tmap(&maps.x[l]);
-        if (TMA_EPI) for (int l = 0; l < P.n_levels; ++l) { ptx::prefetch_tmap(&maps.y[l]); ptx::prefetch_tmap(&maps.r[l]); }
+        if (TMA_EPI) for (int l = 0; l < P.n_levels; ++l) ptx::prefetch_tmap(&maps.y[l]);
+        if (kResRing) for (int l = 0; l < P.n_levels; ++l) ptx::prefetch_tmap(&maps.r[l]);
         ptx::prefetch_tmap(&maps.w);
     }
     ptx::pdl_trigger();                 // the next layer may start its own prologue as our CTAs retire
@@ -180,7 +194,7 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
                 __syncwarp();
                 if (++stage == STAGES) { stage = 0; phase ^= 1u; }
             }
-            if (TMA_EPI && L.res_tma) {                          // residual tile of this output tile, two tiles ahead of its use
+            if (kResRing && L.res_tma) {                          // residual tile of this output tile, two tiles ahead of its use
                 ptx::mbar_wait(&rempty_bar[rslot], rphase ^ 1u);
                 if (leader) {
                     ptx::mbar_expect_tx(&rfull_bar[rslot], kEpiTileBytes);
@@ -197,6 +211,7 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
     const int t = threadIdx.x & 127, wg = threadIdx.x >> 7;
     int stage = 0; uint32_t phase = 0;
     int rslot = 0; uint32_t rphase = 0;
+    uint32_t n_stores = 0;                                  // bulk stores issued so far: staging buffer n_stores % OUT_SLOTS is next
     float acc[BLOCK_N / 2];
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int n_tile = tile % P.n_tiles_n, m_tile = tile / P.n_tiles_n;
@@ -235,41 +250,65 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
         if (t == 0) ptx::mbar_arrive(&empty_bar[prev]);
 
         if constexpr (TMA_EPI) {
-            // ---- shared-memory epilogue: residual from the TMA-fed ring, output through a swizzled staging tile + TMA store
-            const bool res_smem = L.res_tma != 0;
+            // ---- shared-memory epilogue: output through swizzled 128 x 64 staging sub-tiles + TMA stores
+            const bool res_smem = kResRing && L.res_tma != 0;      // residual from the TMA-fed ring, else from global memory
             if (res_smem) ptx::mbar_wait(&rfull_bar[rslot], rphase);
-            // the staging tile is free once the previous tile's bulk store has finished READING it
-            if (threadIdx.x == 0) ptx::bulk_wait_read0();
-            ptx::named_barrier(1, kConsumerThreads);
             const uint8_t* rsm = smem_res + rslot * kEpiTileBytes;
+            const __nv_bfloat16* rrow[2] = {nullptr, nullptr};            // residual rows read from global memory
+            if (!res_smem && L.res != nullptr) {
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int row = wg * 64 + ptx::frag_row(t, h);
-                const RowPos rp = res_smem ? RowPos{true, 0, nullptr} : row_pos(L, tp, row);
-                const int sw = row & 7;
+                for (int h = 0; h < 2; ++h) rrow[h] = row_pos(L, tp, wg * 64 + ptx::frag_row(t, h)).rrow;
+            }
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {                 // 16-byte chunk j (8 channels) of the 128-byte row
-                    const int col = ptx::frag_col(t, j), ch = n0 + col;
-                    const uint32_t off = (uint32_t)(row * 128 + ((j ^ sw) << 4) + (col & 7) * 2);
-                    const float2 s = __ldg(reinterpret_cast<const float2*>(P.shift + ch));
-                    float v0 = acc[4 * j + 2 * h] + s.x, v1 = acc[4 * j + 2 * h + 1] + s.y;
-                    if (res_smem || rp.rrow != nullptr) {
-                        const uint32_t rv = res_smem ? *reinterpret_cast<const uint32_t*>(rsm + off)
-                                                     : __ldg(reinterpret_cast<const unsigned int*>(rp.rrow + ch));
-                        const float2 f = unpack_act2(rv, P.fp16);
-                        v0 += f.x; v1 += f.y;
-                    }
-                    *reinterpret_cast<uint32_t*>(smem_out + off) = pack_act2(activate(v0, P.relu), activate(v1, P.relu), P.fp16);
+            for (int c = 0; c < BLOCK_N / 64; ++c) {
+                const int c0 = n0 + 64 * c;
+                if (c0 >= P.cout) continue;                       // the same for every thread: nothing of this sub-tile is stored
+                uint8_t* so = smem_out + (OUT_SLOTS == 1 ? 0 : n_stores % OUT_SLOTS) * kEpiTileBytes;
+                if (OUT_SLOTS == 1) {
+                    // the staging tile is free once the previous tile's bulk store has finished READING it
+                    if (threadIdx.x == 0) ptx::bulk_wait_read0();
+                    ptx::named_barrier(1, kConsumerThreads);
                 }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = wg * 64 + ptx::frag_row(t, h);
+                    // 128B swizzle: 16-byte chunk j of the row lands at chunk j ^ (row & 7)
+                    const uint32_t rbase = (uint32_t)(row * 128 + ((row & 7) << 4) + (ptx::frag_col(t, 0) & 7) * 2);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {                 // 16-byte chunk j (8 channels) of the 128-byte row
+                        const int ch = c0 + ptx::frag_col(t, j);
+                        const uint32_t off = rbase ^ (uint32_t)(j << 4);
+                        float v0 = 0.0f, v1 = 0.0f;
+                        if (ch < P.cout) {                        // Cout % 8 == 0: the pair is wholly in or out
+                            const float2 s = __ldg(reinterpret_cast<const float2*>(P.shift + ch));
+                            v0 = acc[4 * (8 * c + j) + 2 * h] + s.x; v1 = acc[4 * (8 * c + j) + 2 * h + 1] + s.y;
+                            if (res_smem || rrow[h] != nullptr) {
+                                const uint32_t rv = res_smem ? *reinterpret_cast<const uint32_t*>(rsm + off)
+                                                             : __ldg(reinterpret_cast<const unsigned int*>(rrow[h] + ch));
+                                const float2 f = unpack_act2(rv, P.fp16);
+                                v0 += f.x; v1 += f.y;
+                            }
+                        }
+                        *reinterpret_cast<uint32_t*>(so + off) = pack_act2(activate(v0, P.relu), activate(v1, P.relu), P.fp16);
+                    }
+                }
+                ptx::fence_proxy_async();                        // generic-proxy smem writes -> visible to the TMA engine
+                // double buffering: once the previous store has read its buffer, the barrier below frees it for the next sub-tile
+                if (OUT_SLOTS > 1 && threadIdx.x == 0) ptx::bulk_wait_read0();
+                ptx::named_barrier(1, kConsumerThreads);
+                if (threadIdx.x == 0) {
+                    // the tile position is recomputed here rather than kept live through the epilogue (register pressure)
+                    const TilePos q = tile_pos(P, tile / P.n_tiles_n);
+                    const ConvLevelDev& Lq = P.lv[q.l];
+                    ptx::tma_store_5d(&maps.y[q.l], so, c0, q.tiz * Lq.bz, q.tiy * Lq.by, q.tix * Lq.bx, q.nb);
+                    ptx::bulk_commit();
+                }
+                ++n_stores;
             }
-            ptx::fence_proxy_async();                            // generic-proxy smem writes -> visible to the TMA engine
-            ptx::named_barrier(1, kConsumerThreads);
-            if (threadIdx.x == 0) {
-                if (res_smem) ptx::mbar_arrive(&rempty_bar[rslot]);
-                ptx::tma_store_5d(&maps.y[tp.l], smem_out, n0, tp.tiz * L.bz, tp.tiy * L.by, tp.tix * L.bx, tp.nb);
-                ptx::bulk_commit();
+            if (res_smem) {
+                if (threadIdx.x == 0) ptx::mbar_arrive(&rempty_bar[rslot]);   // every consumer has passed the last barrier
+                if (++rslot == RES_SLOTS) { rslot = 0; rphase ^= 1u; }
             }
-            if (res_smem && ++rslot == RES_SLOTS) { rslot = 0; rphase ^= 1u; }
             continue;
         }
         // ---- register epilogue: each thread owns 2 channels of every 8-channel group in two rows of the tile
@@ -299,7 +338,8 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
 // ------------------------------------------------------------------------------------------------ host
 template <int BLOCK_N, int STAGES, int MIN_BLOCKS, bool TMA_EPI = false, bool WS = false>
 static int launch_conv(const ConvMaps& maps, const ConvDev& P, int total_tiles, cudaStream_t st) {
-    constexpr int smem = STAGES * (kABytes + BLOCK_N * kBlockK * 2 * (WS ? 2 : 1)) + (TMA_EPI ? ((WS ? 1 : 2) + 1) * kEpiTileBytes : 0) + 1024 + 256;
+    constexpr int smem = STAGES * (kABytes + BLOCK_N * kBlockK * 2 * (WS ? 2 : 1)) +
+                         (epi_res_slots(MIN_BLOCKS, TMA_EPI, WS) + epi_out_slots(MIN_BLOCKS, TMA_EPI)) * kEpiTileBytes + 1024 + 256;
     static_assert((smem + 1024) * MIN_BLOCKS <= 228 * 1024, "shared memory budget");
     static bool attr_set = false;
     if (!attr_set) {
@@ -352,9 +392,9 @@ static int conv_geometry(const nrpn_conv_desc* d, ConvGeom& g) {
         const char* e = getenv("NRPN_CONV_NARROW");
         if (!(e && e[0] == '0')) { g.block_n = 64; g.n_tiles_n = g.cout_pad / 64; }
     }
-    // shared-memory (TMA) epilogue: the HBM-bound short reductions with whole 64-channel bf16 output tiles
+    // shared-memory (TMA) epilogue: 16-bit output; the short reductions also need whole 64-channel output tiles
     { const char* e = getenv("NRPN_CONV_TMA_EPI"); g.tma_epi = !(e && e[0] == '0'); }       // A/B switch for tests and profiling
-    g.tma_epi = g.tma_epi && g.short_k && !d->out_fp32 && d->cout % 64 == 0;
+    g.tma_epi = g.tma_epi && !d->out_fp32 && (!g.short_k || d->cout % 64 == 0);
     for (int l = 0; l < d->n_levels && g.tma_epi; ++l) {
         const nrpn_conv_level& S = d->level[l];
         if (reinterpret_cast<uintptr_t>(S.y) % 16 != 0 || (S.res && reinterpret_cast<uintptr_t>(S.res) % 16 != 0)) g.tma_epi = false;
@@ -436,7 +476,7 @@ int nrpn_conv3d_fprop(const nrpn_conv_desc* d, nrpn_stream_t stream) {
         L.xr = S.res ? S.xr : S.xo; L.yr = S.res ? S.yr : S.yo; L.zr = S.res ? S.zr : S.zo;
         L.rsx = (float)L.xr / (float)S.xo; L.rsy = (float)L.yr / (float)S.yo; L.rsz = (float)L.zr / (float)S.zo;
         L.ldy = S.ldy; L.ldr = S.ldr; L.y = S.y; L.res = reinterpret_cast<const __nv_bfloat16*>(S.res);
-        L.res_tma = (geo.tma_epi && S.res && S.xr == S.xo && S.yr == S.yo && S.zr == S.zo) ? 1 : 0;
+        L.res_tma = (geo.tma_epi && short_k && S.res && S.xr == S.xo && S.yr == S.yo && S.zr == S.zo) ? 1 : 0;
         if (geo.tma_epi) {
             // output / residual tensors (C, Z, Y, X, N) with the row pitch ldy / ldr; one box = one 64-channel brick tile
             cuuint32_t ebox[5] = {64, (cuuint32_t)L.bz, (cuuint32_t)L.by, (cuuint32_t)L.bx, 1};
@@ -489,12 +529,22 @@ int nrpn_conv3d_fprop(const nrpn_conv_desc* d, nrpn_stream_t stream) {
     if (d->wsplit) {
         if (short_k && geo.tma_epi) return launch_conv<64, 2, 2, true, true>(maps, P, total_tiles, st);
         if (short_k) return launch_conv<64, 2, 3, false, true>(maps, P, total_tiles, st);
+        if (geo.tma_epi) {
+            if (block_n == 64) return launch_conv<64, 6, 1, true, true>(maps, P, total_tiles, st);
+            if (block_n == 128) return launch_conv<128, 4, 1, true, true>(maps, P, total_tiles, st);
+            return launch_conv<256, 2, 1, true, true>(maps, P, total_tiles, st);
+        }
         if (block_n == 64) return launch_conv<64, 6, 1, false, true>(maps, P, total_tiles, st);
         if (block_n == 128) return launch_conv<128, 4, 1, false, true>(maps, P, total_tiles, st);
         return launch_conv<256, 2, 1, false, true>(maps, P, total_tiles, st);
     }
     if (short_k && geo.tma_epi) return launch_conv<64, 2, 2, true>(maps, P, total_tiles, st);
     if (short_k) return launch_conv<64, 2, 3>(maps, P, total_tiles, st);
+    if (geo.tma_epi) {
+        if (block_n == 64) return launch_conv<64, 8, 1, true>(maps, P, total_tiles, st);
+        if (block_n == 128) return launch_conv<128, 6, 1, true>(maps, P, total_tiles, st);
+        return launch_conv<256, 4, 1, true>(maps, P, total_tiles, st);
+    }
     if (block_n == 64) return launch_conv<64, 8, 1>(maps, P, total_tiles, st);
     if (block_n == 128) return launch_conv<128, 6, 1>(maps, P, total_tiles, st);
     return launch_conv<256, 4, 1>(maps, P, total_tiles, st);
