@@ -42,7 +42,7 @@ class _RPNTrainStep(torch.autograd.Function):
         plan.backward()
         inv = 1.0 / eng.loss_scale
         grads = []
-        for p in list(eng.bb.parameters()) + list(eng.head.parameters()):
+        for p in (list(eng.bb.parameters()) if not plan.frozen else []) + list(eng.head.parameters()):
             g = eng.grad_of(p).view(p.shape)
             grads.append(g * inv if inv != 1.0 else g.clone())
         return (None, None, None, *grads)
@@ -123,20 +123,29 @@ class NeRFRegionProposalNetwork(nn.Module):
             self._train_engine = RPNTrainEngine(self, **kw)
         return self._train_engine
 
+    def frozen_backbone(self) -> bool:
+        """True when no backbone parameter (FPN included) requires a gradient and every head parameter does: the pattern of run_rpn.py
+        --freeze_backbone, which the training forward runs as the shorter frozen-backbone step.  Read at every training forward."""
+        return not any(p.requires_grad for p in self.backbone.parameters()) and all(p.requires_grad for p in self.rpn.head.parameters())
+
     def _forward_train(self, meshes, targets):
         """Training-mode forward as the reference defines it (nerf_rpn.py:166-217 + rpn.py:514-534): returns losses that carry a
         grad_fn, so the UNMODIFIED loop of run_rpn.py:384-395 (`loss.backward(); clip_grad_norm_; optimizer.step()`) and a DDP
         wrapper drive the CUDA forward / backward kernels: torch.autograd only sees ONE node whose backward runs the engine's launch
-        list and hands every parameter its gradient."""
+        list and hands every parameter its gradient.  A backbone whose every parameter has requires_grad = False under a fully trainable
+        head (run_rpn.py --freeze_backbone) runs the engine's frozen-backbone step: only the head's backward, and only the head's
+        parameters enter the node, so their gradients are all that autograd, clip_grad_norm_, the optimiser and DDP see."""
         if targets is None:
             raise ValueError("targets should not be None")
         eng = self.train_engine()
         eng.overlap_allreduce = False               # gradients are returned to autograd; a DDP wrapper all-reduces them itself
+        eng.freeze_backbone = self.frozen_backbone()
         eng.sync_parameters()
         # meshes of any sizes go to the engine as they are (each in its own memory order): it trains the batch padded to their element-wise
         # maximum like transform() does, without materialising it -- and without padding the caller's list in place, as transform() would
         grids = [m if (m.is_cuda and m.dtype == torch.float32) else m.cuda().float() for m in meshes]
-        params = list(self.backbone.parameters()) + list(self.rpn.head.parameters())
+        head = list(self.rpn.head.parameters())
+        params = head if eng.freeze_backbone else list(self.backbone.parameters()) + head
         l_obj, l_reg, l_2d = _RPNTrainStep.apply(eng, grids, [t for t in targets], *params)
         return [None, None, None], {"loss_objectness": l_obj, "loss_rpn_box_reg": l_reg, "loss_rpn_box_reg_2d": l_2d}, None
 

@@ -76,14 +76,15 @@ def _ru(v, m):
     return (v + m - 1) // m * m
 
 
-def bucket_schedule(bwd_lo: Sequence[int], n_params: int, bucket_elems: int):
+def bucket_schedule(bwd_lo: Sequence[int], n_params: int, bucket_elems: int, lowest: int = 0):
     """All-reduce ranges of the flat gradient bucket, in launch order.  bwd_lo[i] = lowest flat offset that is final once backward stage i
     (construction order: stem, blocks..., FPN, head) has run; stages execute in REVERSE, so gradients become final from the end of the bucket
     towards its start.  A range [lo, hi) is launched after a stage as soon as at least bucket_elems new elements are final (or the bucket is
-    complete).  Returns [(stage index in execution order, lo, hi)]: disjoint, covering [0, n_params) exactly once."""
+    complete down to `lowest`, the start of the part the backward pass produces: the head's offset when the backbone is frozen).
+    Returns [(stage index in execution order, lo, hi)]: disjoint, covering [lowest, n_params) exactly once."""
     out, hi = [], n_params
     for k, lo in enumerate(reversed(list(bwd_lo))):
-        if hi > lo and (hi - lo >= bucket_elems or lo == 0):
+        if hi > lo and (hi - lo >= bucket_elems or lo <= lowest):
             out.append((k, lo, hi))
             hi = lo
     return out
@@ -163,7 +164,7 @@ class RPNTrainEngine:
 
     def __init__(self, model, precision: str = "bf16", lr: float = 1e-4, weight_decay: float = 0.01, betas=(0.9, 0.999), eps: float = 1e-8,
                  clip_grad_norm: float = 0.1, reg_loss_weight: float = 5.0, process_group=None, bucket_mb: float = 32.0,
-                 loss_scale: Optional[float] = None, seed: Optional[int] = None, reg_loss_weight_2d: float = 0.0):
+                 loss_scale: Optional[float] = None, seed: Optional[int] = None, reg_loss_weight_2d: float = 0.0, freeze_backbone: bool = False):
         if precision not in ("bf16", "fp16"):
             raise ValueError("training runs with bf16 (default) or fp16 (with a static loss scale) 16-bit activations / gradients")
         bb, rpn = model.backbone, model.rpn
@@ -215,6 +216,10 @@ class RPNTrainEngine:
         self.losses = torch.zeros(2, dtype=torch.float32, device=self.device)
         self.loss_2d = torch.zeros((), dtype=torch.float32, device=self.device)        # loss_rpn_box_reg_2d (unweighted), when evaluated
         self.overlap_allreduce = True       # False: leave the gradient all-reduce to the caller (DDP wrapping the autograd compat path)
+        # True: run_rpn.py --freeze_backbone.  The backbone (FPN included) keeps training-mode BatchNorm but gets no gradient: the step runs the
+        # head's backward only, and clip, AdamW and the all-reduce cover the head's range [head_lo, n_params) of the flat buffers.  Read when a
+        # step plans its batch and when it updates, so it may change between steps.
+        self.freeze_backbone = bool(freeze_backbone)
         self.gen = None
         if seed is not None:
             self.gen = torch.Generator(device=self.device); self.gen.manual_seed(seed)
@@ -239,6 +244,7 @@ class RPNTrainEngine:
             self.offsets[id(p)] = (off, n)
             off += n
         self.n_params = total
+        self.head_lo = total - sum(p.numel() for p in self.head.parameters())      # the head is the contiguous tail of the flat buffers
         self._params = params
         self._packed_ver = None
 
@@ -252,7 +258,8 @@ class RPNTrainEngine:
             if p.data.data_ptr() != self.flat_p.data_ptr() + 4 * off:
                 self.flat_p[off:off + n].copy_(p.data.reshape(-1)); p.data = self.flat_p[off:off + n].view(p.shape); moved = True
         if moved or ver != self._packed_ver:
-            self.repack()
+            n_bb = len(self._params) - len(list(self.head.parameters()))
+            self.repack(head_only=self.freeze_backbone and not moved and ver[:n_bb] == self._packed_ver[:n_bb])
 
     def grad_of(self, p):
         off, n = self.offsets[id(p)]
@@ -287,13 +294,22 @@ class RPNTrainEngine:
         self.pred_db = torch.zeros(128, dtype=torch.float32, device=self.device)
         self.all_convs = [self.stem] + [e[k] for e in self.blocks for k in ("c1", "c2", "c3", "ds") if e[k] is not None] + self.lat + self.smooth + self.hconv
 
-    def repack(self):
-        """fp32 master weights -> 16-bit GEMM operands (after every optimiser step / checkpoint load)."""
+    def repack(self, head_only: bool = False):
+        """fp32 master weights -> 16-bit GEMM operands (after every optimiser step / checkpoint load); head_only: the head's convs and the
+        fused predictor, when no backbone weight has changed (a frozen backbone's operands are packed once)."""
         self._packed_ver = tuple(p._version for p in self._params)
-        _replay_static(self._graphs, "repack", [self._repack_launches])
+        if head_only:
+            _replay_static(self._graphs, "repack_head", [self._repack_head])
+        else:
+            _replay_static(self._graphs, "repack", [self._repack_launches])
 
     def _repack_launches(self):
-        for c in self.all_convs:
+        for c in self.all_convs[:-len(self.hconv)]:
+            c.repack()
+        self._repack_head()
+
+    def _repack_head(self):
+        for c in self.hconv:
             c.repack()
         hd, A = self.head, self.A
         self.pred_w32[:A].copy_(hd.cls_logits.weight.data.view(A, 256))
@@ -304,12 +320,12 @@ class RPNTrainEngine:
 
     # ------------------------------------------------------------------------------------------------ plan
     def plan(self, n, dims):
-        key = (n, tuple(int(d) for d in dims))
+        key = (n, tuple(int(d) for d in dims), self.freeze_backbone)
         p = self._plans.get(key)
         if p is not None:
             self._plans.move_to_end(key)
             return p
-        p = _TrainPlan(self, n, key[1])
+        p = _TrainPlan(self, n, key[1], key[2])
         self._plans[key] = p
         while len(self._plans) > PLAN_CACHE:
             _, old = self._plans.popitem(last=False)
@@ -389,16 +405,20 @@ class RPNTrainEngine:
         return self.losses
 
     def optimizer_step(self, lr: Optional[float] = None):
-        """clip_grad_norm_(clip) + AdamW on the flat buffers (after the all-reduce has drained), then re-pack the 16-bit operands."""
+        """clip_grad_norm_(clip) + AdamW on the flat buffers (after the all-reduce has drained), then re-pack the 16-bit operands.  With a
+        frozen backbone, norm, update and re-packing cover the head alone, as torch's skip parameters whose .grad is None."""
         torch.cuda.current_stream().wait_stream(self.comm_stream)
         self.step_count += 1
         inv = 1.0 / (self.loss_scale * self.world)
         L = lib()
-        check(L.nrpn_grad_norm(_p(self.flat_g), self.n_params, inv, _p(self._norm), _p(self._norm_ws), self._norm_ws.numel(), _stream()), "grad_norm")
-        check(L.nrpn_adamw_step(_p(self.flat_p), _p(self.flat_g), _p(self.flat_m), _p(self.flat_v), self.n_params, _p(self._norm), float(self.clip),
+        lo = self.head_lo if self.freeze_backbone else 0
+        p, g, m, v = (ctypes.c_void_p(t.data_ptr() + 4 * lo) for t in (self.flat_p, self.flat_g, self.flat_m, self.flat_v))
+        n = self.n_params - lo
+        check(L.nrpn_grad_norm(g, n, inv, _p(self._norm), _p(self._norm_ws), self._norm_ws.numel(), _stream()), "grad_norm")
+        check(L.nrpn_adamw_step(p, g, m, v, n, _p(self._norm), float(self.clip),
                                 inv, float(self.lr if lr is None else lr), self.betas[0], self.betas[1], self.eps, self.wd, self.step_count, _stream()),
               "adamw_step")
-        self.repack()
+        self.repack(head_only=self.freeze_backbone)
 
     def train_step(self, grids, targets, lr: Optional[float] = None):
         losses = self.forward_backward(grids, targets)
@@ -407,10 +427,11 @@ class RPNTrainEngine:
 
 
 class _TrainPlan:
-    """Buffers and the launch lists (forward, backward) for n scenes of one size."""
+    """Buffers and the launch lists (forward, backward) for n scenes of one size.  frozen: the backbone gets no gradient, so the backward list
+    is the head's alone and every backbone activation that only its backward would read lives in a few reused slots."""
 
-    def __init__(self, eng: RPNTrainEngine, n: int, dims):
-        self.eng, self.n, self.dims = eng, n, dims
+    def __init__(self, eng: RPNTrainEngine, n: int, dims, frozen: bool = False):
+        self.eng, self.n, self.dims, self.frozen = eng, n, dims, frozen
         dev, dt = eng.device, eng.act_dtype
         self.fwd: List = []
         self.bwd: List = []                      # built in forward order, executed reversed
@@ -433,72 +454,109 @@ class _TrainPlan:
 
         self.input = None
         d1 = _down(dims)
+        d2 = _down(d1)
+        # the blocks in order: (stage, block, its input dims, its output dims, is the stage's first / last block)
+        geo, xd = [], d2
+        for si, stage in enumerate(eng.bb.layers):
+            for j in range(len(stage)):
+                e = eng.blocks[len(geo)]
+                od = _down(xd) if e["stride"] == 2 else xd
+                geo.append((si, e, xd, od, j == 0, j == len(stage) - 1))
+                xd = od
         self.packed = req((n, d1[0], d1[1], d1[2] + 1, 64))
         self.fwd.append(self._pack_input)
-        y0 = buf(d1, 64); a0 = buf(d1, 64)
+        if frozen:
+            # activations read only by the forward: the stem's y0 / a0 share slots "y" / "a" with the blocks' y3 / yd, every block's y1, y2
+            # share "y1" and a1, a2 share "a1", and the max-pool output and the outputs that are not a stage's last alternate between "x0"
+            # and "x1" (sized alike).  Each slot is requested once, at its largest use.
+            use = {"y": [(d1, 64)], "a": [(d1, 64)], "r": [], "y1": [], "a1": [], "x": [(d2, 64)]}
+            for si, e, xd_, od, first, last in geo:
+                use["y1"].append((od, e["c1"].cout)); use["a1"].append((od, e["c1"].cout)); use["y"].append((od, e["c3"].cout))
+                if e["ds"] is not None:
+                    use["a"].append((od, e["c3"].cout)); use["r"].append((od, e["c3"].cout))
+                if not last:
+                    use["x"].append((od, e["c3"].cout))
+            size = {k: max([n * math.prod(d) * c for d, c in u] + [1]) for k, u in use.items()}
+            slots = {k: req((size[k],)) for k in ("y", "a", "r", "y1", "a1")}
+            slots["x0"], slots["x1"] = req((size["x"],)), req((size["x"],))
+
+            def act(slot, d, c):
+                return slots[slot][:n * math.prod(d) * c].view(n, *d, c)
+        else:
+            def act(slot, d, c):
+                return buf(d, c)
+        y0 = act("y", d1, 64); a0 = act("a", d1, 64)
         self._conv_fwd(eng.stem, self.packed, (d1[0], d1[1], d1[2] + 1), y0, d1)
         self._bn_fwd(eng.stem_bn, y0, None, a0, True)
-        d2 = _down(d1)
-        p0 = buf(d2, 64)
-        self.pool_idx = buf(d2, 64, torch.uint8)
-        self.fwd.append(lambda: check(L.nrpn_maxpool3d_k3s2_argmax(_p(a0), n, d1[0], d1[1], d1[2], 64, _p(p0), _p(self.pool_idx), self.f16, _stream()), "maxpool_argmax"))
-        dp0 = buf(d2, 64)                          # gradient w.r.t. the pooled map
-        da0 = buf(d1, 64); dy0 = buf(d1, 64)
+        p0 = act("x0", d2, 64)
+        if frozen:
+            self.fwd.append(lambda: check(L.nrpn_maxpool3d_k3s2(_p(a0), n, d1[0], d1[1], d1[2], 64, _p(p0), self.f16, _stream()), "maxpool"))
+        else:
+            self.pool_idx = buf(d2, 64, torch.uint8)
+            self.fwd.append(lambda: check(L.nrpn_maxpool3d_k3s2_argmax(_p(a0), n, d1[0], d1[1], d1[2], 64, _p(p0), _p(self.pool_idx), self.f16, _stream()),
+                                          "maxpool_argmax"))
+            dp0 = buf(d2, 64)                          # gradient w.r.t. the pooled map
+            da0 = buf(d1, 64); dy0 = buf(d1, 64)
 
-        # backward of the stem (runs LAST): pool backward -> BN backward -> stem wgrad (on the packed input)
-        def stem_bwd():
-            check(L.nrpn_maxpool3d_k3s2_backward(_p(dp0), _p(self.pool_idx), n, d1[0], d1[1], d1[2], 64, _p(da0), self.f16, _stream()), "maxpool_backward")
-            self._bn_bwd(eng.stem_bn, da0, a0, y0, dy0, None, True)
-            self._wgrad_stem(dy0)
-        self.bwd.append(stem_bwd)
-        self.bwd_lo.append(0)
+            # backward of the stem (runs LAST): pool backward -> BN backward -> stem wgrad (on the packed input)
+            def stem_bwd():
+                check(L.nrpn_maxpool3d_k3s2_backward(_p(dp0), _p(self.pool_idx), n, d1[0], d1[1], d1[2], 64, _p(da0), self.f16, _stream()), "maxpool_backward")
+                self._bn_bwd(eng.stem_bn, da0, a0, y0, dy0, None, True)
+                self._wgrad_stem(dy0)
+            self.bwd.append(stem_bwd)
+            self.bwd_lo.append(0)
 
         # ---- bottom-up
-        x, xd, dx = p0, d2, dp0                    # block input, its dims, and the buffer that receives its gradient
+        x, dx, xs = p0, (None if frozen else dp0), "x0"     # block input, the buffer that receives its gradient, and its slot (frozen)
         c_out = []
-        bi = 0
-        for si, stage in enumerate(eng.bb.layers):
-            for _ in stage:
-                e = eng.blocks[bi]; bi += 1
-                s = e["stride"]
-                od = _down(xd) if s == 2 else xd
-                planes, outc = e["c1"].cout, e["c3"].cout
-                y1, a1 = buf(od, planes), buf(od, planes)
-                y2, a2 = buf(od, planes), buf(od, planes)
-                y3, out = buf(od, outc), buf(od, outc)
-                self._conv_fwd(e["c1"], x, xd, y1, od)
-                self._bn_fwd(e["bn1"], y1, None, a1, True)
-                self._conv_fwd(e["c2"], a1, od, y2, od)
-                self._bn_fwd(e["bn2"], y2, None, a2, True)
-                self._conv_fwd(e["c3"], a2, od, y3, od)
-                if e["ds"] is not None:
-                    yd, r = buf(od, outc), buf(od, outc)
-                    self._conv_fwd(e["ds"], x, xd, yd, od)
-                    self._bn_fwd(e["bnd"], yd, None, r, False)
-                else:
-                    yd, r = None, x
-                self._bn_fwd(e["bn3"], y3, r, out, True)
+        for si, e, xd, od, first, last in geo:
+            s = e["stride"]
+            planes, outc = e["c1"].cout, e["c3"].cout
+            y1, a1 = act("y1", od, planes), act("a1", od, planes)
+            y2, a2 = act("y1", od, planes), act("a1", od, planes)
+            y3 = act("y", od, outc)
+            if frozen and not last:
+                xs = "x1" if xs == "x0" else "x0"
+                out = act(xs, od, outc)
+            else:
+                out = buf(od, outc)                # a stage output (read by its FPN lateral) persists
+            self._conv_fwd(e["c1"], x, xd, y1, od)
+            self._bn_fwd(e["bn1"], y1, None, a1, True)
+            self._conv_fwd(e["c2"], a1, od, y2, od)
+            self._bn_fwd(e["bn2"], y2, None, a2, True)
+            self._conv_fwd(e["c3"], a2, od, y3, od)
+            if e["ds"] is not None:
+                yd, r = act("a", od, outc), act("r", od, outc)
+                self._conv_fwd(e["ds"], x, xd, yd, od)
+                self._bn_fwd(e["bnd"], yd, None, r, False)
+            else:
+                yd, r = None, x
+            self._bn_fwd(e["bn3"], y3, r, out, True)
+            dout = None
+            if not frozen:
                 dout = buf(od, outc)               # gradient w.r.t. the block output (filled by the consumer's backward)
                 # the input of the first block of stages 1..3 is a stage output that also feeds an FPN lateral: fpn_bwd (which runs
                 # earlier in the backward pass) has already written the lateral part into dx, so this block ADDS its data gradient
-                add_lateral = (si > 0 and _ is stage[0])
+                add_lateral = (si > 0 and first)
                 self.bwd.append(self._make_block_bwd(e, x, xd, dx, od, y1, a1, y2, a2, y3, out, yd, dout, s, add_lateral))
                 self.bwd_lo.append(min(eng.offsets[id(p_)][0] for k_ in ("c1", "c2", "c3", "ds") if e[k_] is not None for p_ in [e[k_].weight]))
-                x, xd, dx = out, od, dout
-            c_out.append((x, xd, dx))
+            x, dx = out, dout
+            if last:
+                c_out.append((x, od, dx))
 
         # ---- FPN top-down (feature_extractor.py:224-235)
+        grad = (lambda d, c: None) if frozen else buf      # the FPN's gradient buffers (none when the backbone is frozen)
         (c5, d5, dc5) = c_out[-1]
         q = [None] * 4; dq = [None] * 4; qd = [None] * 4
-        q[0] = buf(d5, 256); dq[0] = buf(d5, 256); qd[0] = d5
+        q[0] = buf(d5, 256); dq[0] = grad(d5, 256); qd[0] = d5
         self._conv_fwd(eng.lat[0], c5, d5, q[0], d5)
         for i in range(1, 4):
             (c, cd, _) = c_out[-1 - i]
-            q[i] = buf(cd, 256); dq[i] = buf(cd, 256); qd[i] = cd
+            q[i] = buf(cd, 256); dq[i] = grad(cd, 256); qd[i] = cd
             self._conv_fwd(eng.lat[i], c, cd, q[i], cd, res=q[i - 1], res_dims=qd[i - 1])
         feats, dfeats, fdims = [q[0]], [dq[0]], [d5]           # P5 = q5 (no smooth conv); its gradient accumulates in dq[0]
         for i, sm in enumerate(eng.smooth):
-            f = buf(qd[i + 1], 256); df = buf(qd[i + 1], 256)
+            f = buf(qd[i + 1], 256); df = grad(qd[i + 1], 256)
             self._conv_fwd(sm, q[i + 1], qd[i + 1], f, qd[i + 1])
             feats.append(f); dfeats.append(df); fdims.append(qd[i + 1])
         feats.reverse(); dfeats.reverse(); fdims.reverse()      # [P2, P3, P4, P5]
@@ -522,8 +580,9 @@ class _TrainPlan:
                 self._conv_bwd(eng.lat[i], c, cd, dq[i], cd, dc, bias=True)      # dc = gradient of the stage output from the lateral branch
         # NOTE: the stage outputs c2..c4 also receive the next stage's data gradient: _make_block_bwd ADDS into dx for the first block
         # of stages 1..3 (flag below), because fpn_bwd (which runs earlier) has already written the lateral part.
-        self.bwd.append(fpn_bwd)
-        self.bwd_lo.append(min(eng.offsets[id(c.weight)][0] for c in eng.lat + eng.smooth))
+        if not frozen:
+            self.bwd.append(fpn_bwd)
+            self.bwd_lo.append(min(eng.offsets[id(c.weight)][0] for c in eng.lat + eng.smooth))
 
         # ---- head: all levels in one launch per layer, activations of all levels in ONE buffer (bias gradients are one reduction)
         vox = [d[0] * d[1] * d[2] for d in fdims]
@@ -566,6 +625,8 @@ class _TrainPlan:
                 self._wgrad(level_views(dhs[k]), xin, layer.taps, 256, 256, eng.grad_of(layer.weight), layout=1)
                 ws = self._workspace(L.nrpn_bias_grad_workspace_bytes(256))
                 check(L.nrpn_bias_grad(_p(dhs[k]), self.total_vox, 256, 256, self.f16, _p(eng.grad_of(layer.bias)), _p(ws), ws.numel(), _stream()), "bias_grad")
+                if k == 0 and frozen:
+                    break                                       # nothing reads the gradient of a frozen backbone's feature maps
                 dst = dfeats if k == 0 else level_views(dhs[k - 1])
                 self._conv_fwd_levels(layer.bwd, layer.bwd_shift, layer.taps, 256, 256, level_views(dhs[k]), dst, fdims, relu=False, run=True)
         self.bwd.append(head_bwd)
@@ -932,7 +993,7 @@ class _TrainPlan:
             self.allreduce_calls = 0
             _replay_static(self._graphs, "bwd", list(reversed(self.bwd)))
             return
-        sched = {k: (lo, hi) for k, lo, hi in bucket_schedule(self.bwd_lo, eng.n_params, eng.bucket_elems)}
+        sched = {k: (lo, hi) for k, lo, hi in bucket_schedule(self.bwd_lo, eng.n_params, eng.bucket_elems, lowest=self.bwd_lo[0])}
         self.allreduce_calls = 0
         order = list(reversed(self.bwd))
         start = 0
