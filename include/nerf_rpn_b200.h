@@ -325,7 +325,7 @@ int nrpn_anchor_padding_mask(const int32_t *ori_sizes /*host, n x 3*/, int n, in
 /* ------------------------------------------------------------------------------------------------ weight gradient
  * dW[tap][co][ci] = sum_v dY[v][co] * X[v + tap_off][ci] of a stride-1 convolution (training, SURVEY.md 8(a) a18) on wgmma.
  * Both operands are read channels-last where they live (MN-major wgmma operands); levels that share the weights (RPN head on
- * P2..P5) accumulate into the same dW.  dw: fp32 in dw_layout's order, overwritten unless accumulate is set.
+ * P2..P5) accumulate into the same dW.  dw: fp32 in dw_layout's order, overwritten.
  * cout % 8 == 0; cin % 32 == 0 with cin <= 256, or cin % 256 == 0; ld_dy / ld_x multiples of 8; any tap offsets.
  * Deterministic (fixed-order reduction of the K-split partial tiles). */
 typedef struct {
@@ -347,7 +347,6 @@ typedef struct {
     size_t workspace_bytes;
     int32_t act_fp16;
     int32_t dw_layout;       /* 0: dw is (taps, Cout, Cin); 1: dw is (Cout, Cin, taps) = nn.Conv3d.weight's own memory order */
-    int32_t accumulate;      /* 1: dw += result (a weight shared by several launches) */
 } nrpn_wgrad_desc;
 
 size_t nrpn_conv3d_wgrad_workspace_bytes(const nrpn_wgrad_desc *desc /*host*/);
@@ -383,10 +382,10 @@ int nrpn_bn_backward(const void *dout, const void *act, const void *y, void *dy,
  * backward as a deterministic gather over the <= 8 windows that contain an input voxel (feature_extractor.py:219). */
 int nrpn_maxpool3d_k3s2_argmax(const void *in, int n, int x, int y, int z, int c, void *out, uint8_t *idx, int act_fp16, nrpn_stream_t stream);
 int nrpn_maxpool3d_k3s2_backward(const void *dy, const uint8_t *idx, int n, int x, int y, int z, int c, void *dx, int act_fp16, nrpn_stream_t stream);
-/* Backward of the FPN top-down merge fine += nearest_upsample(coarse) (feature_extractor.py:211-213): dcoarse (+)= sum of dfine over
+/* Backward of the FPN top-down merge fine += nearest_upsample(coarse) (feature_extractor.py:211-213): dcoarse += sum of dfine over
  * the fine voxels whose source index floor(f * coarse / fine) is the coarse voxel (same float expression as the forward epilogue). */
 int nrpn_upsample_nearest_backward(const void *dfine, int n, int xf, int yf, int zf, int xc, int yc, int zc, int c, void *dcoarse,
-                                   int accumulate, int act_fp16, nrpn_stream_t stream);
+                                   int act_fp16, nrpn_stream_t stream);
 /* Stride-2 1^3 convolutions (first block of ResNet stages 2-4): scatter = 0: dst (ceil/2 extents) = src sub-sampled at even
  * voxels (the wgrad operand); scatter = 1: dst (x,y,z) = src (ceil/2 extents) zero-stuffed (the data gradient). */
 int nrpn_stride2(const void *src, void *dst, int n, int x, int y, int z, int c, int scatter, nrpn_stream_t stream);
@@ -406,9 +405,9 @@ int nrpn_rpn_loss(const nrpn_rpn_desc *desc /*host*/, void *const *dpred /*host 
  * not written (zero-fill the buffers once). */
 int nrpn_pack_weights(const float *w, int cout, int cin, int taps, void *fwd, int fwd_rows, int fwd_cols, void *bwd, int bwd_rows,
                       int bwd_cols, int act_fp16, nrpn_stream_t stream);
-/* out[i] = idx[i] >= 0 ? src[idx[i]] * scale : 0 -- 16-bit (out16) or fp32 (out32): layouts given by a host-built index table
+/* out[i] = idx[i] >= 0 ? src[idx[i]] : 0 -- 16-bit (out16) or fp32 (out32): layouts given by a host-built index table
  * (the space-to-depth stem weights and their gradient). */
-int nrpn_gather_pack(const float *src, const int32_t *idx, size_t n, void *out16, float *out32, float scale, int act_fp16, nrpn_stream_t stream);
+int nrpn_gather_pack(const float *src, const int32_t *idx, size_t n, void *out16, float *out32, int act_fp16, nrpn_stream_t stream);
 /* norm_out[0] = ||g||_2 * inv_scale (fp64 two-stage reduction) */
 size_t nrpn_grad_norm_workspace_bytes(void);
 int nrpn_grad_norm(const float *g, size_t n, float inv_scale, float *norm_out, void *workspace, size_t workspace_bytes, nrpn_stream_t stream);

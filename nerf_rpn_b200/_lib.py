@@ -55,7 +55,7 @@ class WgradDesc(ctypes.Structure):
     _fields_ = [("cin", ctypes.c_int32), ("cout", ctypes.c_int32), ("n_taps", ctypes.c_int32),
                 ("tap_off", (ctypes.c_int8 * 3) * MAX_TAPS), ("n_levels", ctypes.c_int32), ("level", WgradLevel * MAX_LEVELS),
                 ("dw", ctypes.c_void_p), ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_size_t),
-                ("act_fp16", ctypes.c_int32), ("dw_layout", ctypes.c_int32), ("accumulate", ctypes.c_int32)]
+                ("act_fp16", ctypes.c_int32), ("dw_layout", ctypes.c_int32)]
 
 
 class StemSrc(ctypes.Structure):
@@ -172,7 +172,7 @@ _SIGNATURES = {
     "nrpn_maxpool3d_k3s2_backward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                     ctypes.c_int, ctypes.c_void_p, ctypes.c_int, c_stream]),
     "nrpn_upsample_nearest_backward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                                      ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, c_stream]),
+                                                      ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, c_stream]),
     "nrpn_stride2": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                     ctypes.c_int, c_stream]),
     "nrpn_add_inplace": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, c_stream]),
@@ -181,7 +181,7 @@ _SIGNATURES = {
                                      ctypes.c_int, c_stream]),
     "nrpn_pack_weights": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
                                          ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_stream]),
-    "nrpn_gather_pack": (ctypes.c_int, [c_f32p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, c_f32p, ctypes.c_float, ctypes.c_int, c_stream]),
+    "nrpn_gather_pack": (ctypes.c_int, [c_f32p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, c_f32p, ctypes.c_int, c_stream]),
     "nrpn_grad_norm_workspace_bytes": (ctypes.c_size_t, []),
     "nrpn_grad_norm": (ctypes.c_int, [c_f32p, ctypes.c_size_t, ctypes.c_float, c_f32p, ctypes.c_void_p, ctypes.c_size_t, c_stream]),
     "nrpn_adamw_step": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_size_t, c_f32p, ctypes.c_float, ctypes.c_float, ctypes.c_float,

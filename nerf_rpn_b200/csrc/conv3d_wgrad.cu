@@ -38,10 +38,9 @@ __device__ __forceinline__ void store_partial(float* tile, int n_t, int wg, int 
 }
 
 // dW[tap][co][ci] = sum over splits (fixed order) of the partial tiles
-// layout 0: dw (taps, Cout, Cin);  layout 1: dw (Cout, Cin, taps) = nn.Conv3d.weight's own memory order (taps = kx*ky*kz row-major);
-// accumulate: dw += (gradient accumulation of a shared weight over separate launches)
+// layout 0: dw (taps, Cout, Cin);  layout 1: dw (Cout, Cin, taps) = nn.Conv3d.weight's own memory order (taps = kx*ky*kz row-major)
 __global__ void wgrad_reduce_kernel(const float* __restrict__ partial, int n_taps, int m_tiles, int n_tiles, int splits, int n_t, int cout, int cin,
-                                    float* __restrict__ dw, int layout, int accumulate) {
+                                    float* __restrict__ dw, int layout) {
     const size_t total = (size_t)n_taps * cout * cin;
     for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
         const int ci = (int)(t % cin); size_t v = t / cin;
@@ -51,7 +50,7 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ partial, int n_tap
         float s = 0.f;
         for (int sp = 0; sp < splits; ++sp) s += p[(size_t)sp * 128 * n_t];
         const size_t o = layout ? ((size_t)co * cin + ci) * n_taps + tap : t;
-        dw[o] = accumulate ? dw[o] + s : s;
+        dw[o] = s;
     }
 }
 
@@ -320,7 +319,7 @@ static int wgrad_run(const nrpn_wgrad_desc* d, cudaStream_t st) {
     size_t blocks = ceil_div(total, (size_t)256);
     if (blocks > (size_t)num_sms() * 8) blocks = (size_t)num_sms() * 8;
     wgrad_reduce_kernel<<<(unsigned)blocks, 256, 0, st>>>(P.partial, P.n_taps, P.m_tiles, P.n_tiles, P.splits, P.n_t, P.cout, P.cin, d->dw,
-                                                        d->dw_layout ? 1 : 0, d->accumulate ? 1 : 0);
+                                                        d->dw_layout ? 1 : 0);
     NRPN_LAUNCH_CHECK();
     return NRPN_OK;
 }

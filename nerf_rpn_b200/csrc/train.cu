@@ -301,12 +301,12 @@ __global__ void __launch_bounds__(256) maxpool_k3s2_backward_kernel(const __nv_b
 }
 
 // ---------------------------------------------------------------------------------------------- nearest up-sampling, backward
-// Forward (conv epilogue): fine[f] += coarse[min(floor(f * in/out), in-1)].  Backward: dcoarse[cidx] (+)= sum of dfine[f] over the
+// Forward (conv epilogue): fine[f] += coarse[min(floor(f * in/out), in-1)].  Backward: dcoarse[cidx] += sum of dfine[f] over the
 // fine voxels that map to cidx, evaluated with the SAME float expression as the forward epilogue.
 __device__ __forceinline__ int up_src(int g, float rs, int in) { return min((int)floorf((float)g * rs), in - 1); }
 
 __global__ void __launch_bounds__(256) upsample_nearest_backward_kernel(const __nv_bfloat16* __restrict__ dfine, int n, int Xf, int Yf, int Zf, int Xc, int Yc,
-                                                                        int Zc, int C, __nv_bfloat16* __restrict__ dcoarse, int accumulate, int fp16) {
+                                                                        int Zc, int C, __nv_bfloat16* __restrict__ dcoarse, int fp16) {
     const int cg = C >> 3;
     const float rsx = (float)Xc / (float)Xf, rsy = (float)Yc / (float)Yf, rsz = (float)Zc / (float)Zf;
     const size_t total = (size_t)n * Xc * Yc * Zc * cg;
@@ -315,20 +315,16 @@ __global__ void __launch_bounds__(256) upsample_nearest_backward_kernel(const __
         const int z = (int)(v % Zc); v /= Zc;
         const int y = (int)(v % Yc); v /= Yc;
         const int x = (int)(v % Xc); const int b = (int)(v / Xc);
-        float acc[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) acc[q] = 0.f;
-        __nv_bfloat16* dst = dcoarse + ((((size_t)b * Xc + x) * Yc + y) * Zc + z) * C + g * 8;
-        if (accumulate) {
-            const uint4 cur = *reinterpret_cast<const uint4*>(dst);
-            const uint32_t* cw = reinterpret_cast<const uint32_t*>(&cur);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) { const float2 f = unpack_act2(cw[q], fp16); acc[2 * q] = f.x; acc[2 * q + 1] = f.y; }
-        }
         // candidate fine indices: the pre-image of a coarse index under floor(f * in/out) is an interval around x * out/in
         const int fx0 = max(0, (int)((float)x / rsx) - 2), fx1 = min(Xf - 1, (int)((float)(x + 1) / rsx) + 2);
         const int fy0 = max(0, (int)((float)y / rsy) - 2), fy1 = min(Yf - 1, (int)((float)(y + 1) / rsy) + 2);
         const int fz0 = max(0, (int)((float)z / rsz) - 2), fz1 = min(Zf - 1, (int)((float)(z + 1) / rsz) + 2);
+        __nv_bfloat16* dst = dcoarse + t * 8;                  // t enumerates (b, x, y, z, channel group) in dcoarse's order
+        const uint4 cur = *reinterpret_cast<const uint4*>(dst);
+        const uint32_t* cw = reinterpret_cast<const uint32_t*>(&cur);
+        float acc[8];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) { const float2 f = unpack_act2(cw[q], fp16); acc[2 * q] = f.x; acc[2 * q + 1] = f.y; }
         for (int fx = fx0; fx <= fx1; ++fx) {
             if (up_src(fx, rsx, Xc) != x) continue;
             for (int fy = fy0; fy <= fy1; ++fy) {
@@ -526,10 +522,10 @@ __global__ void __launch_bounds__(256) pack_weights_kernel(const float* __restri
 
 // out[i] = idx[i] >= 0 ? src[idx[i]] : 0, converted to 16 bits (stem weight packing through a host-built index table) or kept fp32
 __global__ void gather_pack_kernel(const float* __restrict__ src, const int* __restrict__ idx, size_t n, __nv_bfloat16* __restrict__ out16,
-                                   float* __restrict__ out32, float scale, int fp16) {
+                                   float* __restrict__ out32, int fp16) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         const int k = idx[i];
-        const float v = k >= 0 ? src[k] * scale : 0.f;
+        const float v = k >= 0 ? src[k] : 0.f;
         if (out16) store_act(out16 + i, v, fp16); else out32[i] = v;
     }
 }
@@ -663,13 +659,12 @@ int nrpn_maxpool3d_k3s2_backward(const void* dy, const uint8_t* idx, int n, int 
     return NRPN_OK;
 }
 
-int nrpn_upsample_nearest_backward(const void* dfine, int n, int xf, int yf, int zf, int xc, int yc, int zc, int c, void* dcoarse, int accumulate,
-                                   int act_fp16, nrpn_stream_t stream) {
+int nrpn_upsample_nearest_backward(const void* dfine, int n, int xf, int yf, int zf, int xc, int yc, int zc, int c, void* dcoarse, int act_fp16,
+                                   nrpn_stream_t stream) {
     if (!dfine || !dcoarse || n < 1 || xf < 1 || yf < 1 || zf < 1 || xc < 1 || yc < 1 || zc < 1 || c < 8 || c % 8 != 0) return NRPN_ERR_INVALID;
     const size_t total = (size_t)n * xc * yc * zc * (c / 8);
     upsample_nearest_backward_kernel<<<grid1d(total, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __nv_bfloat16*>(dfine), n, xf, yf, zf, xc, yc, zc, c,
-                                                                                           reinterpret_cast<__nv_bfloat16*>(dcoarse), accumulate ? 1 : 0,
-                                                                                           act_fp16 ? 1 : 0);
+                                                                                           reinterpret_cast<__nv_bfloat16*>(dcoarse), act_fp16 ? 1 : 0);
     NRPN_LAUNCH_CHECK();
     return NRPN_OK;
 }
@@ -724,8 +719,6 @@ int nrpn_pack_weights(const float* w, int cout, int cin, int taps, void* fwd, in
                       int act_fp16, nrpn_stream_t stream) {
     if (!w || !fwd || cout < 1 || cin < 1 || taps < 1 || fwd_rows < cout || fwd_cols < cin) return NRPN_ERR_INVALID;
     if (bwd && (bwd_rows < cin || bwd_cols < cout)) return NRPN_ERR_INVALID;
-    const size_t total = (size_t)cout * cin * taps;
-    (void)total;
     const dim3 grid((unsigned)ceil_div(cin, 16), (unsigned)ceil_div(cout, 16));
     const size_t smem = (size_t)256 * taps * sizeof(float);
     if (grid.y > 65535 || smem > 48 * 1024) return NRPN_ERR_UNSUPPORTED;        // taps <= 48 (3^3 = 27; the 7^3 stem goes through nrpn_gather_pack)
@@ -735,9 +728,9 @@ int nrpn_pack_weights(const float* w, int cout, int cin, int taps, void* fwd, in
     return NRPN_OK;
 }
 
-int nrpn_gather_pack(const float* src, const int32_t* idx, size_t n, void* out16, float* out32, float scale, int act_fp16, nrpn_stream_t stream) {
+int nrpn_gather_pack(const float* src, const int32_t* idx, size_t n, void* out16, float* out32, int act_fp16, nrpn_stream_t stream) {
     if (!src || !idx || n < 1 || ((out16 == nullptr) == (out32 == nullptr))) return NRPN_ERR_INVALID;
-    gather_pack_kernel<<<grid1d(n, 256), 256, 0, (cudaStream_t)stream>>>(src, idx, n, reinterpret_cast<__nv_bfloat16*>(out16), out32, scale, act_fp16 ? 1 : 0);
+    gather_pack_kernel<<<grid1d(n, 256), 256, 0, (cudaStream_t)stream>>>(src, idx, n, reinterpret_cast<__nv_bfloat16*>(out16), out32, act_fp16 ? 1 : 0);
     NRPN_LAUNCH_CHECK();
     return NRPN_OK;
 }

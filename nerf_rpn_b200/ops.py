@@ -218,7 +218,7 @@ def is_channels_last_grid(grid: torch.Tensor) -> bool:
 def wgrad_desc(dys: Sequence[torch.Tensor], xs: Sequence[torch.Tensor], taps: Sequence[Sequence[int]], cout: int, cin: int,
                act_fp16: int) -> WgradDesc:
     """nrpn_wgrad_desc of a stride-1 conv's weight gradient: taps and one level per channels-last 16-bit (dY (N,X,Y,Z,ld_dy), X (N,X',Y',Z',ld_x))
-    pair of the pyramid levels that share the weights.  The caller sets dw, workspace, dw_layout and accumulate."""
+    pair of the pyramid levels that share the weights.  The caller sets dw, workspace and dw_layout."""
     d = WgradDesc()
     d.cout, d.cin, d.n_taps = int(cout), int(cin), len(taps)
     for t, off in enumerate(taps):

@@ -91,23 +91,26 @@ def bucket_schedule(bwd_lo: Sequence[int], n_params: int, bucket_elems: int, low
 
 
 class _TConv:
-    """One trainable convolution: views of the master weight (+ bias), its 16-bit forward / data-gradient operands and tap table."""
+    """One trainable convolution: its fp32 weight (+ bias), their gradient destinations (by default the parameters' views of the flat
+    gradient bucket), its 16-bit forward / data-gradient operands and tap table."""
 
-    def __init__(self, eng, conv: torch.nn.Conv3d, need_dgrad=True, stem=False):
+    def __init__(self, eng, weight, bias, stride=1, need_dgrad=True, stem=False, dw=None, db=None):
         self.eng = eng
-        self.weight, self.bias = conv.weight, conv.bias
-        cout, cin, k = conv.weight.shape[0], conv.weight.shape[1], conv.weight.shape[2]
+        self.weight, self.bias = weight, bias
+        self.dw = eng.grad_of(weight) if dw is None else dw
+        self.db = eng.grad_of(bias) if db is None and bias is not None else db
+        cout, cin, k = weight.shape[0], weight.shape[1], weight.shape[2]
         self.cout, self.cin_real, self.k = cout, cin, k
-        self.stride = conv.stride[0]
+        self.stride = stride
         dt, dev = eng.act_dtype, eng.device
         self.stem = stem
         if stem:
-            probe = torch.arange(1, conv.weight.numel() + 1, dtype=torch.float32).view_as(conv.weight)
+            probe = torch.arange(1, weight.numel() + 1, dtype=torch.float32).view_as(weight)
             wp, taps = packing.pack_stem_weight(probe, None, dtype=torch.float32)                  # (32, 64, 64): source index + 1, 0 = structural zero
             self.taps = taps
             self.cin, self.cout_pad = 64, 64
             self.gather_idx = (wp.reshape(-1).to(torch.int64) - 1).to(torch.int32).to(dev)       # packed position -> master index
-            inv = torch.full((conv.weight.numel(),), -1, dtype=torch.int32)
+            inv = torch.full((weight.numel(),), -1, dtype=torch.int32)
             pos = torch.nonzero(wp.reshape(-1) > 0).reshape(-1)
             inv[(wp.reshape(-1)[pos] - 1).to(torch.int64)] = pos.to(torch.int32)
             assert int((inv < 0).sum()) == 0
@@ -141,7 +144,7 @@ class _TConv:
         f16 = 1 if self.eng.act_dtype == torch.float16 else 0
         L = lib()
         if self.stem:
-            check(L.nrpn_gather_pack(_p(self.weight.data), _p(self.gather_idx), self.gather_idx.numel(), _p(self.fwd), None, 1.0, f16, _stream()),
+            check(L.nrpn_gather_pack(_p(self.weight.data), _p(self.gather_idx), self.gather_idx.numel(), _p(self.fwd), None, f16, _stream()),
                   "gather_pack(stem)")
             return
         taps = len(self.taps)
@@ -267,31 +270,30 @@ class RPNTrainEngine:
 
     def _build_layers(self):
         bb, hd = self.bb, self.head
-        self.stem = _TConv(self, bb.conv1, need_dgrad=False, stem=True)
+
+        def conv(m: torch.nn.Conv3d, **kw):
+            return _TConv(self, m.weight, m.bias, stride=m.stride[0], **kw)
+        self.stem = conv(bb.conv1, need_dgrad=False, stem=True)
         self.stem_bn = _BN(self, bb.bn1)
         self.blocks = []
         for stage in bb.layers:
             for blk in stage:
-                e = dict(c1=_TConv(self, blk.conv1), bn1=_BN(self, blk.bn1), c2=_TConv(self, blk.conv2), bn2=_BN(self, blk.bn2),
-                         c3=_TConv(self, blk.conv3), bn3=_BN(self, blk.bn3), ds=None, bnd=None, stride=blk.stride)
+                e = dict(c1=conv(blk.conv1), bn1=_BN(self, blk.bn1), c2=conv(blk.conv2), bn2=_BN(self, blk.bn2),
+                         c3=conv(blk.conv3), bn3=_BN(self, blk.bn3), ds=None, bnd=None, stride=blk.stride)
                 if blk.downsample is not None:
-                    e["ds"] = _TConv(self, blk.downsample[0]); e["bnd"] = _BN(self, blk.downsample[1])
+                    e["ds"] = conv(blk.downsample[0]); e["bnd"] = _BN(self, blk.downsample[1])
                 self.blocks.append(e)
-        self.lat = [_TConv(self, m) for m in bb.latlayers]
-        self.smooth = [_TConv(self, m) for m in bb.smooths]
-        self.hconv = [_TConv(self, m) for m in hd.conv if isinstance(m, torch.nn.Conv3d)]
-        # fused cls | bbox predictor (anchor.py:196-198): one 1^3 GEMM with 128 (padded) output channels
+        self.lat = [conv(m) for m in bb.latlayers]
+        self.smooth = [conv(m) for m in bb.smooths]
+        self.hconv = [conv(m) for m in hd.conv if isinstance(m, torch.nn.Conv3d)]
+        # fused cls | bbox predictor (anchor.py:196-198): one 1^3 conv with 128 (padded) output channels on fp32 staging copies of the two
+        # layers' weights and biases (_repack_head); its gradients land in staging buffers that head_bwd splits into the two layers' gradients
         self.n_pred = self.A * (1 + self.code)
         if self.n_pred > 128:
             raise ValueError("fused predictor supports at most 128 output channels")
-        dt = self.act_dtype
-        self.pred_fwd = torch.zeros((1, 128, 256), dtype=dt, device=self.device)
-        self.pred_bwd = torch.zeros((1, 256, 128), dtype=dt, device=self.device)
-        self.pred_shift = torch.zeros(128, dtype=torch.float32, device=self.device)
-        self.pred_bwd_shift = torch.zeros(256, dtype=torch.float32, device=self.device)
-        self.pred_w32 = torch.zeros((128, 256), dtype=torch.float32, device=self.device)
-        self.pred_dw = torch.zeros((128, 256), dtype=torch.float32, device=self.device)
-        self.pred_db = torch.zeros(128, dtype=torch.float32, device=self.device)
+        f32 = dict(dtype=torch.float32, device=self.device)
+        self.predictor = _TConv(self, torch.zeros((128, 256, 1, 1, 1), **f32), torch.zeros(128, **f32),
+                                dw=torch.zeros((128, 256), **f32), db=torch.zeros(128, **f32))
         self.all_convs = [self.stem] + [e[k] for e in self.blocks for k in ("c1", "c2", "c3", "ds") if e[k] is not None] + self.lat + self.smooth + self.hconv
 
     def repack(self, head_only: bool = False):
@@ -311,12 +313,11 @@ class RPNTrainEngine:
     def _repack_head(self):
         for c in self.hconv:
             c.repack()
-        hd, A = self.head, self.A
-        self.pred_w32[:A].copy_(hd.cls_logits.weight.data.view(A, 256))
-        self.pred_w32[A:self.n_pred].copy_(hd.bbox_pred.weight.data.view(-1, 256))
-        self.pred_shift[:A].copy_(hd.cls_logits.bias.data); self.pred_shift[A:self.n_pred].copy_(hd.bbox_pred.bias.data)
-        check(lib().nrpn_pack_weights(_p(self.pred_w32), 128, 256, 1, _p(self.pred_fwd), 128, 256, _p(self.pred_bwd), 256, 128, self.f16, _stream()),
-              "pack_weights(pred)")
+        hd, A, pr = self.head, self.A, self.predictor
+        pr.weight[:A].copy_(hd.cls_logits.weight.data)
+        pr.weight[A:self.n_pred].copy_(hd.bbox_pred.weight.data)
+        pr.bias[:A].copy_(hd.cls_logits.bias.data); pr.bias[A:self.n_pred].copy_(hd.bbox_pred.bias.data)
+        pr.repack()
 
     # ------------------------------------------------------------------------------------------------ plan
     def plan(self, n, dims):
@@ -486,7 +487,7 @@ class _TrainPlan:
             def act(slot, d, c):
                 return buf(d, c)
         y0 = act("y", d1, 64); a0 = act("a", d1, 64)
-        self._conv_fwd(eng.stem, self.packed, (d1[0], d1[1], d1[2] + 1), y0, d1)
+        self._conv_fwd(eng.stem, [self.packed], [(d1[0], d1[1], d1[2] + 1)], [y0], [d1])
         self._bn_fwd(eng.stem_bn, y0, None, a0, True)
         p0 = act("x0", d2, 64)
         if frozen:
@@ -510,6 +511,9 @@ class _TrainPlan:
         x, dx, xs = p0, (None if frozen else dp0), "x0"     # block input, the buffer that receives its gradient, and its slot (frozen)
         c_out = []
         for si, e, xd, od, first, last in geo:
+            # a stage's first block -- and only it -- has a downsample, strided in every stage but the first (ResNet_FPN_256._make_layer):
+            # the backward of the first block of stages 1..3 adds its zero-stuffed data gradient to the lateral part fpn_bwd wrote
+            assert (e["ds"] is not None) == first and (e["stride"] == 2) == (first and si > 0), "unexpected ResNet stage layout"
             s = e["stride"]
             planes, outc = e["c1"].cout, e["c3"].cout
             y1, a1 = act("y1", od, planes), act("a1", od, planes)
@@ -520,14 +524,14 @@ class _TrainPlan:
                 out = act(xs, od, outc)
             else:
                 out = buf(od, outc)                # a stage output (read by its FPN lateral) persists
-            self._conv_fwd(e["c1"], x, xd, y1, od)
+            self._conv_fwd(e["c1"], [x], [xd], [y1], [od])
             self._bn_fwd(e["bn1"], y1, None, a1, True)
-            self._conv_fwd(e["c2"], a1, od, y2, od)
+            self._conv_fwd(e["c2"], [a1], [od], [y2], [od])
             self._bn_fwd(e["bn2"], y2, None, a2, True)
-            self._conv_fwd(e["c3"], a2, od, y3, od)
+            self._conv_fwd(e["c3"], [a2], [od], [y3], [od])
             if e["ds"] is not None:
                 yd, r = act("a", od, outc), act("r", od, outc)
-                self._conv_fwd(e["ds"], x, xd, yd, od)
+                self._conv_fwd(e["ds"], [x], [xd], [yd], [od])
                 self._bn_fwd(e["bnd"], yd, None, r, False)
             else:
                 yd, r = None, x
@@ -535,10 +539,7 @@ class _TrainPlan:
             dout = None
             if not frozen:
                 dout = buf(od, outc)               # gradient w.r.t. the block output (filled by the consumer's backward)
-                # the input of the first block of stages 1..3 is a stage output that also feeds an FPN lateral: fpn_bwd (which runs
-                # earlier in the backward pass) has already written the lateral part into dx, so this block ADDS its data gradient
-                add_lateral = (si > 0 and first)
-                self.bwd.append(self._make_block_bwd(e, x, xd, dx, od, y1, a1, y2, a2, y3, out, yd, dout, s, add_lateral))
+                self.bwd.append(self._make_block_bwd(e, x, xd, dx, od, y1, a1, y2, a2, y3, out, yd, dout, s))
                 self.bwd_lo.append(min(eng.offsets[id(p_)][0] for k_ in ("c1", "c2", "c3", "ds") if e[k_] is not None for p_ in [e[k_].weight]))
             x, dx = out, dout
             if last:
@@ -549,15 +550,15 @@ class _TrainPlan:
         (c5, d5, dc5) = c_out[-1]
         q = [None] * 4; dq = [None] * 4; qd = [None] * 4
         q[0] = buf(d5, 256); dq[0] = grad(d5, 256); qd[0] = d5
-        self._conv_fwd(eng.lat[0], c5, d5, q[0], d5)
+        self._conv_fwd(eng.lat[0], [c5], [d5], [q[0]], [d5])
         for i in range(1, 4):
             (c, cd, _) = c_out[-1 - i]
             q[i] = buf(cd, 256); dq[i] = grad(cd, 256); qd[i] = cd
-            self._conv_fwd(eng.lat[i], c, cd, q[i], cd, res=q[i - 1], res_dims=qd[i - 1])
+            self._conv_fwd(eng.lat[i], [c], [cd], [q[i]], [cd], res=q[i - 1], res_dims=qd[i - 1])
         feats, dfeats, fdims = [q[0]], [dq[0]], [d5]           # P5 = q5 (no smooth conv); its gradient accumulates in dq[0]
         for i, sm in enumerate(eng.smooth):
             f = buf(qd[i + 1], 256); df = grad(qd[i + 1], 256)
-            self._conv_fwd(sm, q[i + 1], qd[i + 1], f, qd[i + 1])
+            self._conv_fwd(sm, [q[i + 1]], [qd[i + 1]], [f], [qd[i + 1]])
             feats.append(f); dfeats.append(df); fdims.append(qd[i + 1])
         feats.reverse(); dfeats.reverse(); fdims.reverse()      # [P2, P3, P4, P5]
         self.features, self.feat_dims = feats, fdims
@@ -567,19 +568,21 @@ class _TrainPlan:
             # dfeats = [dP2, dP3, dP4, dP5(=dq[0])]
             for i in (2, 1, 0):                                 # smooth[i] acts on q[i+1]; finest level first
                 lvl_feat = 2 - i                                # index into feats / dfeats ([P2,P3,P4,P5]): smooth[2]->P2, [1]->P3, [0]->P4
-                self._conv_bwd(eng.smooth[i], q[i + 1], qd[i + 1], dfeats[lvl_feat], qd[i + 1], dq[i + 1], bias=True)
+                self._param_grad(eng.smooth[i], [dfeats[lvl_feat]], [q[i + 1]])
+                self._dgrad(eng.smooth[i], [dfeats[lvl_feat]], [dq[i + 1]], [qd[i + 1]])
                 if i < 2:                                       # the finer level's merged map took up(q[i+1]) as its residual
                     fd, cd_ = qd[i + 2], qd[i + 1]
-                    check(L.nrpn_upsample_nearest_backward(_p(dq[i + 2]), n, fd[0], fd[1], fd[2], cd_[0], cd_[1], cd_[2], 256, _p(dq[i + 1]), 1, self.f16, _stream()),
+                    check(L.nrpn_upsample_nearest_backward(_p(dq[i + 2]), n, fd[0], fd[1], fd[2], cd_[0], cd_[1], cd_[2], 256, _p(dq[i + 1]), self.f16, _stream()),
                           "upsample_backward")
             fd, cd_ = qd[1], qd[0]
-            check(L.nrpn_upsample_nearest_backward(_p(dq[1]), n, fd[0], fd[1], fd[2], cd_[0], cd_[1], cd_[2], 256, _p(dq[0]), 1, self.f16, _stream()),
+            check(L.nrpn_upsample_nearest_backward(_p(dq[1]), n, fd[0], fd[1], fd[2], cd_[0], cd_[1], cd_[2], 256, _p(dq[0]), self.f16, _stream()),
                   "upsample_backward")
             for i in range(4):
                 (c, cd, dc) = c_out[-1 - i]
-                self._conv_bwd(eng.lat[i], c, cd, dq[i], cd, dc, bias=True)      # dc = gradient of the stage output from the lateral branch
+                self._param_grad(eng.lat[i], [dq[i]], [c])
+                self._dgrad(eng.lat[i], [dq[i]], [dc], [cd])    # dc = gradient of the stage output from the lateral branch
         # NOTE: the stage outputs c2..c4 also receive the next stage's data gradient: _make_block_bwd ADDS into dx for the first block
-        # of stages 1..3 (flag below), because fpn_bwd (which runs earlier) has already written the lateral part.
+        # of stages 1..3, because fpn_bwd (which runs earlier) has already written the lateral part.
         if not frozen:
             self.bwd.append(fpn_bwd)
             self.bwd_lo.append(min(eng.offsets[id(c.weight)][0] for c in eng.lat + eng.smooth))
@@ -597,38 +600,29 @@ class _TrainPlan:
         dhs = [req((self.total_vox, 256)) for _ in eng.hconv]
         self.pred = req((self.total_vox, 128), torch.float32)
         self.dpred = req((self.total_vox, 128))             # zeroed by every loss_grad
+        self.pred_levels, self.dpred_levels = level_views(self.pred), level_views(self.dpred)
+        h_lv, dh_lv = [level_views(h) for h in hs], [level_views(h) for h in dhs]
         cur = feats
-        for k, layer in enumerate(eng.hconv):
-            nxt = level_views(hs[k])
-            self._conv_fwd_levels(layer.fwd, layer.shift, layer.taps, 256, 256, cur, nxt, fdims, relu=True)
+        for layer, nxt in zip(eng.hconv, h_lv):
+            self._conv_fwd(layer, cur, fdims, nxt, fdims, relu=True)
             cur = nxt
-        self._conv_fwd_levels(eng.pred_fwd, eng.pred_shift, [(0, 0, 0)], 256, 128, cur, level_views(self.pred), fdims, relu=False, out_fp32=True)
-        self.pred_levels = level_views(self.pred)
-        self.dbg = dict(hs=[level_views(h) for h in hs], dhs=[level_views(h) for h in dhs], dfeats=dfeats, q=q, dq=dq, c_out=c_out)   # tools/debug_train.py
-        self.dpred_levels = level_views(self.dpred)
+        self._conv_fwd(eng.predictor, cur, fdims, self.pred_levels, fdims, out_fp32=True)
+        self.dbg = dict(hs=h_lv, dhs=dh_lv, dfeats=dfeats, q=q, dq=dq, c_out=c_out)   # tools/debug_train.py
         self.strides = [tuple(dims[k] // d[k] for k in range(3)) for d in fdims]
+        # the head's layers with the input and the output of each, all levels, and their gradients
+        layers, ins, dins, douts = eng.hconv + [eng.predictor], [feats] + h_lv, [dfeats] + dh_lv, dh_lv + [self.dpred_levels]
 
         def head_bwd():
-            h_last = level_views(hs[-1])
-            # predictor: wgrad / bias grad into scratch (cls and bbox rows are separate parameters), dgrad -> dh4
-            self._wgrad(self.dpred_levels, h_last, [(0, 0, 0)], 128, 256, eng.pred_dw, layout=0)
-            ws = self._workspace(L.nrpn_bias_grad_workspace_bytes(128))
-            check(L.nrpn_bias_grad(_p(self.dpred), self.total_vox, 128, 128, self.f16, _p(eng.pred_db), _p(ws), ws.numel(), _stream()), "bias_grad")
-            A, hd = eng.A, eng.head
-            eng.grad_of(hd.cls_logits.weight).copy_(eng.pred_dw[:A].reshape(-1)); eng.grad_of(hd.bbox_pred.weight).copy_(eng.pred_dw[A:eng.n_pred].reshape(-1))
-            eng.grad_of(hd.cls_logits.bias).copy_(eng.pred_db[:A]); eng.grad_of(hd.bbox_pred.bias).copy_(eng.pred_db[A:eng.n_pred])
-            self._conv_fwd_levels(eng.pred_bwd, eng.pred_bwd_shift, [(0, 0, 0)], 128, 256, self.dpred_levels, level_views(dhs[-1]), fdims, relu=False, run=True)
-            for k in range(len(eng.hconv) - 1, -1, -1):
-                layer = eng.hconv[k]
-                check(L.nrpn_relu_backward(_p(dhs[k]), _p(hs[k]), dhs[k].numel(), self.f16, _stream()), "relu_backward")
-                xin = feats if k == 0 else level_views(hs[k - 1])
-                self._wgrad(level_views(dhs[k]), xin, layer.taps, 256, 256, eng.grad_of(layer.weight), layout=1)
-                ws = self._workspace(L.nrpn_bias_grad_workspace_bytes(256))
-                check(L.nrpn_bias_grad(_p(dhs[k]), self.total_vox, 256, 256, self.f16, _p(eng.grad_of(layer.bias)), _p(ws), ws.numel(), _stream()), "bias_grad")
+            for k in range(len(layers) - 1, -1, -1):
+                self._param_grad(layers[k], douts[k], ins[k])
                 if k == 0 and frozen:
                     break                                       # nothing reads the gradient of a frozen backbone's feature maps
-                dst = dfeats if k == 0 else level_views(dhs[k - 1])
-                self._conv_fwd_levels(layer.bwd, layer.bwd_shift, layer.taps, 256, 256, level_views(dhs[k]), dst, fdims, relu=False, run=True)
+                self._dgrad(layers[k], douts[k], dins[k], fdims)
+                if k > 0:                                       # the input of layer k is the ReLU output of layer k - 1
+                    check(L.nrpn_relu_backward(_p(dhs[k - 1]), _p(hs[k - 1]), dhs[k - 1].numel(), self.f16, _stream()), "relu_backward")
+            A, hd, pr = eng.A, eng.head, eng.predictor          # the fused predictor's gradients: cls and bbox rows are separate parameters
+            eng.grad_of(hd.cls_logits.weight).copy_(pr.dw[:A].reshape(-1)); eng.grad_of(hd.bbox_pred.weight).copy_(pr.dw[A:eng.n_pred].reshape(-1))
+            eng.grad_of(hd.cls_logits.bias).copy_(pr.db[:A]); eng.grad_of(hd.bbox_pred.bias).copy_(pr.db[A:eng.n_pred])
         self.bwd.append(head_bwd)
         self.bwd_lo.append(min(eng.offsets[id(p_)][0] for p_ in eng.head.parameters()))
         self._src = None
@@ -663,22 +657,14 @@ class _TrainPlan:
             self._scratch[name] = t
         return t[:numel]
 
-    def _conv_call(self, w, shift, taps, cin, cout, levels, stride=1, relu=False, out_fp32=False):
-        ops.conv3d_fprop(levels, w, shift, cin, cout, taps, stride=stride, relu=relu, out_fp32=out_fp32)
-
-    def _conv_fwd(self, layer: _TConv, x, xd, y, od, res=None, res_dims=None, relu=False):
-        n = self.n
-        args = [ops.ConvLevelArgs(x, y, n, xd, od, y.shape[-1], res=res, res_dims=res_dims, ldr=0 if res is None else res.shape[-1])]
-        self.fwd.append(lambda: self._conv_call(layer.fwd, layer.shift, layer.taps, layer.cin, y.shape[-1], args, stride=layer.stride, relu=relu))
-
-    def _conv_fwd_levels(self, w, shift, taps, cin, cout, xs, ys, dims_l, relu, out_fp32=False, run=False):
-        n = self.n
-        args = [ops.ConvLevelArgs(xs[i], ys[i], n, dims_l[i], dims_l[i], ys[i].shape[-1]) for i in range(len(xs))]
-        f = lambda: self._conv_call(w, shift, taps, cin, cout, args, relu=relu, out_fp32=out_fp32)
-        if run:
-            f()
-        else:
-            self.fwd.append(f)
+    def _conv_fwd(self, layer: _TConv, xs, xds, ys, yds, res=None, res_dims=None, relu=False, out_fp32=False):
+        """Records one launch of `layer`'s forward over the levels xs[i] (dims xds[i]) -> ys[i] (dims yds[i]); res: one level's residual added
+        in the epilogue, read at res_dims (up-sampled when coarser)."""
+        args = [ops.ConvLevelArgs(x, y, self.n, xd, yd, y.shape[-1], res=res, res_dims=res_dims, ldr=0 if res is None else res.shape[-1])
+                for x, xd, y, yd in zip(xs, xds, ys, yds)]
+        cout = ys[0].shape[-1]
+        self.fwd.append(lambda: ops.conv3d_fprop(args, layer.fwd, layer.shift, layer.cin, cout, layer.taps, stride=layer.stride, relu=relu,
+                                                 out_fp32=out_fp32))
 
     def _bn_fwd(self, bn: _BN, y, res, out, relu):
         rows = y.numel() // bn.c
@@ -699,10 +685,10 @@ class _TrainPlan:
         check(lib().nrpn_bn_backward(_p(dout), _p(act), _p(y), _p(dy), _p(dres), rows, bn.c, _p(bn.stats), _p(bn.m.weight.data), _p(sums), int(relu),
                                      self.f16, _p(ws), ws.numel(), _stream()), "bn_backward")
 
-    def _wgrad(self, dys, xs, taps, cout, cin, dw, layout, accumulate=False):
+    def _wgrad(self, dys, xs, taps, cout, cin, dw, layout):
         """dW of a stride-1 'same' conv from per-level channels-last (dY, X) pairs, written to `dw` (fp32) in `layout`."""
         d = ops.wgrad_desc(dys, xs, taps, cout, cin, self.f16)
-        d.dw_layout, d.accumulate = int(layout), int(bool(accumulate))
+        d.dw_layout = int(layout)
         need = lib().nrpn_conv3d_wgrad_workspace_bytes(ctypes.byref(d))
         if need == 0:
             raise ValueError(f"conv3d_wgrad: unsupported shape cout={cout} cin={cin}")
@@ -710,42 +696,45 @@ class _TrainPlan:
         d.dw, d.workspace, d.workspace_bytes = dw.data_ptr(), ws.data_ptr(), ws.numel()
         check(lib().nrpn_conv3d_wgrad(ctypes.byref(d), _stream()), "conv3d_wgrad")
 
+    def _param_grad(self, layer: _TConv, dys, xs):
+        """layer.dw (nn.Conv3d's layout) from per-level (dY, X) pairs, and layer.db when the layer has a bias.  The levels of dY are consecutive
+        rows of one buffer."""
+        self._wgrad(dys, xs, layer.taps, layer.cout, layer.cin_real, layer.dw, layout=1)
+        if layer.db is not None:
+            L = lib()
+            ws = self._workspace(L.nrpn_bias_grad_workspace_bytes(layer.cout))
+            rows = sum(dy.numel() for dy in dys) // layer.cout
+            check(L.nrpn_bias_grad(_p(dys[0]), rows, layer.cout, layer.cout, self.f16, _p(layer.db), _p(ws), ws.numel(), _stream()), "bias_grad")
+
+    def _dgrad(self, layer: _TConv, dys, dxs, dims, res=None):
+        """Data gradient of a stride-1 layer: its mirrored / transposed operand run forward over the levels dys[i] -> dxs[i] (both dims[i]),
+        + res (one level) in the epilogue."""
+        args = [ops.ConvLevelArgs(dy, dx, self.n, d, d, dx.shape[-1], res=res, ldr=0 if res is None else res.shape[-1]) for dy, dx, d in zip(dys, dxs, dims)]
+        ops.conv3d_fprop(args, layer.bwd, layer.bwd_shift, layer.bwd_cols, dxs[0].shape[-1], layer.taps)
+
     def _wgrad_stem(self, dy0):
-        eng = self.eng
-        st = eng.stem
+        st = self.eng.stem
         dwp = self._scratch_buf("stem_dw", len(st.taps) * 64 * 64, torch.float32)
         self._wgrad([dy0], [self.packed], st.taps, 64, 64, dwp, layout=0)
-        g = eng.grad_of(st.weight)
-        check(lib().nrpn_gather_pack(_p(dwp), _p(st.scatter_idx), g.numel(), None, _p(g), 1.0, self.f16, _stream()), "gather_pack(stem grad)")
+        check(lib().nrpn_gather_pack(_p(dwp), _p(st.scatter_idx), st.dw.numel(), None, _p(st.dw), self.f16, _stream()), "gather_pack(stem grad)")
 
-    def _conv_bwd(self, layer: _TConv, x, xd, dy, od, dx, bias=False, dx_res=None, accumulate_dx=False):
-        """wgrad (+ bias grad) of a stride-1 layer and its data gradient into dx (optionally + dx_res through the conv epilogue)."""
+    def _make_block_bwd(self, e, x, xd, dx, od, y1, a1, y2, a2, y3, out, yd, dout, s):
         eng, L, n = self.eng, lib(), self.n
-        self._wgrad([dy], [x], layer.taps, layer.cout, layer.cin_real, eng.grad_of(layer.weight), layout=1)
-        if bias:
-            ws = self._workspace(L.nrpn_bias_grad_workspace_bytes(layer.cout))
-            rows = dy.numel() // layer.cout
-            check(L.nrpn_bias_grad(_p(dy), rows, layer.cout, layer.cout, self.f16, _p(eng.grad_of(layer.bias)), _p(ws), ws.numel(), _stream()), "bias_grad")
-        if dx is not None:
-            args = [ops.ConvLevelArgs(dy, dx, n, od, xd, dx.shape[-1], res=dx_res, res_dims=None if dx_res is None else xd,
-                                      ldr=0 if dx_res is None else dx_res.shape[-1])]
-            self._conv_call(layer.bwd, layer.bwd_shift, layer.taps, layer.bwd_cols, dx.shape[-1], args)
-
-    def _make_block_bwd(self, e, x, xd, dx, od, y1, a1, y2, a2, y3, out, yd, dout, s, add_lateral):
-        eng, L, n = self.eng, lib(), self.n
-        planes, outc, cin = e["c1"].cout, e["c3"].cout, e["c1"].cin_real
-        dt, dev = eng.act_dtype, eng.device
+        cin = e["c1"].cin_real
+        dt = eng.act_dtype
 
         def f():
             g = self._scratch_buf("g_skip", out.numel(), dt).view_as(out)        # masked gradient of the block output = skip-branch gradient
             dy3 = self._scratch_buf("dy3", y3.numel(), dt).view_as(y3)
             self._bn_bwd(e["bn3"], dout, out, y3, dy3, g, True)
             da2 = self._scratch_buf("da2", a2.numel(), dt).view_as(a2)
-            self._conv_bwd(e["c3"], a2, od, dy3, od, da2)
+            self._param_grad(e["c3"], [dy3], [a2])
+            self._dgrad(e["c3"], [dy3], [da2], [od])
             dy2 = self._scratch_buf("dy2", y2.numel(), dt).view_as(y2)
             self._bn_bwd(e["bn2"], da2, a2, y2, dy2, None, True)
             da1 = self._scratch_buf("da1", a1.numel(), dt).view_as(a1)
-            self._conv_bwd(e["c2"], a1, od, dy2, od, da1)
+            self._param_grad(e["c2"], [dy2], [a1])
+            self._dgrad(e["c2"], [dy2], [da1], [od])
             dy1 = self._scratch_buf("dy1", y1.numel(), dt).view_as(y1)
             self._bn_bwd(e["bn1"], da1, a1, y1, dy1, None, True)
             if s == 1:
@@ -753,34 +742,25 @@ class _TrainPlan:
             else:                                                               # stride-2 1^3 convs read the even voxels of x
                 xs = self._scratch_buf("x_s2", n * od[0] * od[1] * od[2] * cin, dt).view(n, *od, cin)
                 check(L.nrpn_stride2(_p(x), _p(xs), n, xd[0], xd[1], xd[2], cin, 0, _stream()), "stride2 gather")
-            # dx accumulates: [lateral branch, already written by fpn_bwd for stage outputs] + skip / downsample branch + conv1 branch
-            if e["ds"] is None:
-                # identity skip: dx = dgrad_c1(dy1) + g   (stride 1 always)
-                self._wgrad([dy1], [xs], e["c1"].taps, planes, cin, eng.grad_of(e["c1"].weight), layout=1)
-                tgt = dx if not add_lateral else self._scratch_buf("dx_tmp", dx.numel(), dt).view_as(dx)
-                args = [ops.ConvLevelArgs(dy1, tgt, n, od, od, cin, res=g, res_dims=od, ldr=outc)]
-                self._conv_call(e["c1"].bwd, e["c1"].bwd_shift, e["c1"].taps, e["c1"].bwd_cols, cin, args)
-                if add_lateral:
-                    check(L.nrpn_add_inplace(_p(dx), _p(tgt), dx.numel(), self.f16, _stream()), "add_inplace")
-            else:
-                dyd = self._scratch_buf("dyd", yd.numel(), dt).view_as(yd)
-                self._bn_bwd(e["bnd"], g, None, yd, dyd, None, False)
-                self._wgrad([dy1], [xs], e["c1"].taps, planes, cin, eng.grad_of(e["c1"].weight), layout=1)
-                self._wgrad([dyd], [xs], e["ds"].taps, outc, cin, eng.grad_of(e["ds"].weight), layout=1)
-                t1 = self._scratch_buf("t1", n * od[0] * od[1] * od[2] * cin, dt).view(n, *od, cin)
-                args = [ops.ConvLevelArgs(dy1, t1, n, od, od, cin)]
-                self._conv_call(e["c1"].bwd, e["c1"].bwd_shift, e["c1"].taps, e["c1"].bwd_cols, cin, args)
-                direct = (s == 1 and not add_lateral)
-                t2 = dx if direct else self._scratch_buf("t2", n * od[0] * od[1] * od[2] * cin, dt).view(n, *od, cin)
-                args = [ops.ConvLevelArgs(dyd, t2, n, od, od, cin, res=t1, res_dims=od, ldr=cin)]
-                self._conv_call(e["ds"].bwd, e["ds"].bwd_shift, e["ds"].taps, e["ds"].bwd_cols, cin, args)
-                if s == 2:
-                    full = dx if not add_lateral else self._scratch_buf("dx_tmp", dx.numel(), dt).view_as(dx)
-                    check(L.nrpn_stride2(_p(t2), _p(full), n, xd[0], xd[1], xd[2], cin, 1, _stream()), "stride2 scatter")
-                    if add_lateral:
-                        check(L.nrpn_add_inplace(_p(dx), _p(full), dx.numel(), self.f16, _stream()), "add_inplace")
-                elif add_lateral:
-                    check(L.nrpn_add_inplace(_p(dx), _p(t2), dx.numel(), self.f16, _stream()), "add_inplace")
+            if e["ds"] is None:                                                 # identity skip (not a stage's first block): dx = dgrad_c1(dy1) + g
+                self._param_grad(e["c1"], [dy1], [xs])
+                self._dgrad(e["c1"], [dy1], [dx], [od], res=g)
+                return
+            dyd = self._scratch_buf("dyd", yd.numel(), dt).view_as(yd)
+            self._bn_bwd(e["bnd"], g, None, yd, dyd, None, False)
+            self._param_grad(e["c1"], [dy1], [xs])
+            self._param_grad(e["ds"], [dyd], [xs])
+            t1 = self._scratch_buf("t1", n * od[0] * od[1] * od[2] * cin, dt).view(n, *od, cin)
+            self._dgrad(e["c1"], [dy1], [t1], [od])
+            if s == 1:                                                          # stage 0: dx = dgrad_ds(dyd) + dgrad_c1(dy1)
+                self._dgrad(e["ds"], [dyd], [dx], [od], res=t1)
+                return
+            # stages 1..3: the sum, zero-stuffed to x's grid, is added to the lateral part fpn_bwd has already written into dx
+            t2 = self._scratch_buf("t2", n * od[0] * od[1] * od[2] * cin, dt).view(n, *od, cin)
+            self._dgrad(e["ds"], [dyd], [t2], [od], res=t1)
+            full = self._scratch_buf("dx_tmp", dx.numel(), dt).view_as(dx)
+            check(L.nrpn_stride2(_p(t2), _p(full), n, xd[0], xd[1], xd[2], cin, 1, _stream()), "stride2 scatter")
+            check(L.nrpn_add_inplace(_p(dx), _p(full), dx.numel(), self.f16, _stream()), "add_inplace")
         return f
 
     # ------------------------------------------------------------------------------------------------ run
@@ -898,6 +878,15 @@ class _TrainPlan:
                 deltas[m] = p[i].reshape(-1, 128)[vox[m].view(-1, 1), cols[m]]
         return deltas, level, vox, cols
 
+    def _put_dpred(self, i, level, vox, cols, g, add):
+        """Writes the per-positive gradient rows g (n_pos, code) of mesh i to where _gather_deltas found the deltas in d(pred): assigned (g already
+        in d(pred)'s dtype), or with add=True added to what is there in fp32 and rounded once."""
+        for l, dp in enumerate(self.dpred_levels):
+            m = level == l
+            if m.any():
+                view, rows = dp[i].reshape(-1, 128), vox[m].view(-1, 1)
+                view[rows, cols[m]] = (view[rows, cols[m]].float() + g[m]).to(view.dtype) if add else g[m]
+
     def _proj2d_loss(self, w_2d):
         """loss_rpn_box_reg_2d (rpn.py:421-453): the sampled positives' DECODED boxes and their matched ground truth, two points each, projected into
         four cameras, smooth-L1 / positives / max mesh dimension (model/proj2d.py); with a non-zero weight its gradient w.r.t. the deltas (autograd
@@ -923,13 +912,7 @@ class _TrainPlan:
                     (g,) = torch.autograd.grad(loss, d)
             total = total + loss.detach()
             if w_2d != 0.0:
-                g = g * (w_2d * eng.loss_scale)
-                for l, dp in enumerate(self.dpred_levels):
-                    m = level == l
-                    if m.any():
-                        view = dp[i].reshape(-1, 128)
-                        rows = vox[m].view(-1, 1)
-                        view[rows, cols[m]] = (view[rows, cols[m]].float() + g[m]).to(view.dtype)
+                self._put_dpred(i, level, vox, cols, g * (w_2d * eng.loss_scale), add=True)
         eng.loss_2d.copy_(total)
 
     # ---- IoU-type regression losses (RotatedIOULoss, rpn.py:133-165: "iou", "linear_iou", "giou", "diou") on the <= 128 sampled positives per mesh
@@ -948,19 +931,12 @@ class _TrainPlan:
         from .model.coder_torch import decode_obb
         from .model.rotated_iou.oriented_iou_loss import cal_diou_3d, cal_giou_3d, cal_iou_3d
         eng = self.eng
-        A, code = eng.A, 8
         anchors = self._anchors()
         total = torch.zeros((), dtype=torch.float32, device=eng.device)
         for i, (pos, neg, gtp) in enumerate(self.last_samples):
             if pos.numel() == 0:
                 continue
-            level, vox, a = self._split_anchor_index(pos)
-            cols = (A + a * code).view(-1, 1) + torch.arange(code, device=pos.device).view(1, -1)
-            deltas = torch.empty((pos.numel(), code), dtype=torch.float32, device=eng.device)
-            for l, p in enumerate(self.pred_levels):
-                m = level == l
-                if m.any():
-                    deltas[m] = p[i].reshape(-1, 128)[vox[m].view(-1, 1), cols[m]]
+            deltas, level, vox, cols = self._gather_deltas(i, pos)
             with torch.enable_grad():
                 d = deltas.detach().requires_grad_(True)
                 boxes = decode_obb(anchors[pos], d)
@@ -976,11 +952,7 @@ class _TrainPlan:
                 (g,) = torch.autograd.grad(loss, d)
             total = total + loss.detach()
             if w_reg != 0.0:
-                g = (g * (w_reg * eng.loss_scale)).to(self.dpred.dtype)
-                for l, dp in enumerate(self.dpred_levels):
-                    m = level == l
-                    if m.any():
-                        dp[i].reshape(-1, 128)[vox[m].view(-1, 1), cols[m]] = g[m]
+                self._put_dpred(i, level, vox, cols, (g * (w_reg * eng.loss_scale)).to(self.dpred.dtype), add=False)
         eng.losses[1] = total
 
     def backward(self):

@@ -34,7 +34,7 @@ def test_host_only_queries():
     assert L.nrpn_nms_workspace_bytes(0) > 0
 
 
-def test_ctypes_struct_layouts_match_c():
+def test_ctypes_struct_layouts_match_header():
     code = r'''
 #include <stdio.h>
 #include <stddef.h>
@@ -45,7 +45,7 @@ int main(void) {
          offsetof(nrpn_conv_desc, w), offsetof(nrpn_conv_desc, level), sizeof(nrpn_rpn_level), sizeof(nrpn_rpn_desc),
          offsetof(nrpn_rpn_desc, cell_anchors), offsetof(nrpn_rpn_desc, nms_thresh), offsetof(nrpn_rpn_desc, valid));
   printf("%zu %zu %zu %zu %zu %zu\n", sizeof(nrpn_wgrad_level), sizeof(nrpn_wgrad_desc), offsetof(nrpn_wgrad_desc, level),
-         offsetof(nrpn_wgrad_desc, dw), offsetof(nrpn_wgrad_desc, workspace_bytes), offsetof(nrpn_wgrad_desc, accumulate));
+         offsetof(nrpn_wgrad_desc, dw), offsetof(nrpn_wgrad_desc, workspace_bytes), offsetof(nrpn_wgrad_desc, dw_layout));
   return 0; }'''
     with tempfile.TemporaryDirectory() as d:
         src, exe = os.path.join(d, "t.c"), os.path.join(d, "t")
@@ -55,7 +55,7 @@ int main(void) {
     C, R, W = _lib.ConvDesc, _lib.RpnDesc, _lib.WgradDesc
     mine = [C.act_fp16.offset, C.wsplit.offset, ctypes.sizeof(_lib.ConvLevel), ctypes.sizeof(C), C.stride.offset, C.w.offset, C.level.offset,
             ctypes.sizeof(_lib.RpnLevel), ctypes.sizeof(R), R.cell_anchors.offset, R.nms_thresh.offset, R.valid.offset,
-            ctypes.sizeof(_lib.WgradLevel), ctypes.sizeof(W), W.level.offset, W.dw.offset, W.workspace_bytes.offset, W.accumulate.offset]
+            ctypes.sizeof(_lib.WgradLevel), ctypes.sizeof(W), W.level.offset, W.dw.offset, W.workspace_bytes.offset, W.dw_layout.offset]
     assert mine == vals
 
 

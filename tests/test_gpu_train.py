@@ -101,14 +101,14 @@ def test_maxpool_argmax_and_backward_vs_autograd(L, dims, c, dtype):
 
 
 @pytest.mark.parametrize("fine,coarse", [((13, 9, 7), (7, 5, 4)), ((40, 64, 64), (20, 32, 32)), ((25, 25, 17), (13, 13, 9))])
-def test_upsample_nearest_backward_vs_autograd(L, fine, coarse):
+def test_upsample_nearest_backward_adds_vs_autograd(L, fine, coarse):
     from nerf_rpn_b200._lib import check
     g = torch.Generator(device="cuda").manual_seed(sum(fine))
     n, c = 1, 64
     df = torch.randn(n, *fine, c, device="cuda", generator=g).to(torch.bfloat16)
     dc = torch.randn(n, *coarse, c, device="cuda", generator=g).to(torch.bfloat16)
     base = dc.clone()
-    check(L.nrpn_upsample_nearest_backward(_p(df), n, *fine, *coarse, c, _p(dc), 1, 0, _s()), "upsample_backward")
+    check(L.nrpn_upsample_nearest_backward(_p(df), n, *fine, *coarse, c, _p(dc), 0, _s()), "upsample_backward")
     torch.cuda.synchronize()
     cz = torch.zeros(n, c, *coarse, device="cuda", requires_grad=True)
     F.interpolate(cz, size=fine, mode="nearest").backward(df.float().permute(0, 4, 1, 2, 3))
@@ -147,7 +147,7 @@ def test_wgrad_general_shapes_vs_autograd(L, cout, cin, k):
     taps = [(a - k // 2, b - k // 2, c - k // 2) for a in range(k) for b in range(k) for c in range(k)]
     plan = T._TrainPlan.__new__(T._TrainPlan)
     plan.eng = type("E", (), {"device": torch.device("cuda")})()
-    plan._scratch, plan._ws, plan.f16, plan.n = {}, None, 0, 1
+    plan._scratch, plan.f16, plan.n = {}, 0, 1
     dw = torch.full((cout, cin, k, k, k), float("nan"), device="cuda")
     plan._wgrad([dy], [x], taps, cout, cin, dw, layout=1)
     torch.cuda.synchronize()
