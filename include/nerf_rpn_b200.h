@@ -350,6 +350,11 @@ typedef struct {
 } nrpn_wgrad_desc;
 
 size_t nrpn_conv3d_wgrad_workspace_bytes(const nrpn_wgrad_desc *desc /*host*/);
+/* Name of the kernel instance and plan nrpn_conv3d_wgrad would run for this descriptor: "wgrad<NT,NACC>/m<M>/t<T>/s<S>" = input
+ * channels per accumulator, accumulators per work item, Cout slices per item, taps per item, K-splits ("wgrad<128,2>/m1/t2/s3");
+ * "invalid" / "unsupported" when it would be rejected.  Pure host logic: pointers inside the descriptor are not dereferenced.  The
+ * split count depends on the current device's SM count.  The returned string is valid until the calling thread's next call. */
+const char *nrpn_conv3d_wgrad_variant(const nrpn_wgrad_desc *desc /*host*/);
 int nrpn_conv3d_wgrad(const nrpn_wgrad_desc *desc /*host*/, nrpn_stream_t stream);
 
 /* Pointwise pieces of a conv + bias + ReLU layer's backward pass (training building blocks):

@@ -120,6 +120,7 @@ _SIGNATURES = {
     "nrpn_conv3d_variant": (ctypes.c_char_p, [ctypes.POINTER(ConvDesc)]),
     "nrpn_conv3d_fprop": (ctypes.c_int, [ctypes.POINTER(ConvDesc), c_stream]),
     "nrpn_conv3d_wgrad_workspace_bytes": (ctypes.c_size_t, [ctypes.POINTER(WgradDesc)]),
+    "nrpn_conv3d_wgrad_variant": (ctypes.c_char_p, [ctypes.POINTER(WgradDesc)]),
     "nrpn_conv3d_wgrad": (ctypes.c_int, [ctypes.POINTER(WgradDesc), c_stream]),
     "nrpn_bias_grad_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int]),
     "nrpn_bias_grad": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_long, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, ctypes.c_void_p,

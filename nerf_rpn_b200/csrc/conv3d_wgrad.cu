@@ -11,6 +11,7 @@
 // (n_t input channels x 64 voxels).  Work item = (tap group, Cout slice(s), Cin slice, K-split); every item streams its share of the voxel bricks
 // of all pyramid levels that share the weights (the RPN head on P2..P5) and writes fp32 partial tiles; a second kernel sums them in a fixed order
 // (bit-reproducible) into dW (taps, Cout, Cin) or nn.Conv3d.weight's own (Cout, Cin, taps) order.
+#include <cstdio>
 #include <cstring>
 #include <type_traits>
 #include "common.cuh"
@@ -328,6 +329,18 @@ size_t nrpn_conv3d_wgrad_workspace_bytes(const nrpn_wgrad_desc* d) {
     WgDev P;
     if (wgrad_plan(d, P) != NRPN_OK) return 0;
     return (size_t)P.n_taps * P.m_tiles * P.n_tiles * P.splits * 128 * P.n_t * sizeof(float) + 256;
+}
+
+// "wgrad<NT,NACC>/m<m_pair>/t<t_group>/s<splits>": the instance wgrad_run's switch launches (NT = 64 b_boxes, NACC = m_pair t_group)
+// and the plan it runs with.  Pure host logic; the name lives in a per-thread buffer until this thread's next call.
+const char* nrpn_conv3d_wgrad_variant(const nrpn_wgrad_desc* d) {
+    static thread_local char name[64];
+    WgDev P;
+    const int rc = wgrad_plan(d, P);
+    if (rc == NRPN_ERR_UNSUPPORTED) return "unsupported";
+    if (rc != NRPN_OK) return "invalid";
+    snprintf(name, sizeof(name), "wgrad<%d,%d>/m%d/t%d/s%d", 64 * P.b_boxes, P.m_pair * P.t_group, P.m_pair, P.t_group, P.splits);
+    return name;
 }
 
 int nrpn_conv3d_wgrad(const nrpn_wgrad_desc* d, nrpn_stream_t stream) {

@@ -234,6 +234,13 @@ def wgrad_desc(dys: Sequence[torch.Tensor], xs: Sequence[torch.Tensor], taps: Se
     return d
 
 
+def conv3d_wgrad_variant(dys: Sequence[torch.Tensor], xs: Sequence[torch.Tensor], taps: Sequence[Sequence[int]], cout: int, cin: int,
+                         act_fp16: int) -> str:
+    """Which instance and plan nrpn_conv3d_wgrad runs for these operands ("wgrad<NT,NACC>/m<M>/t<T>/s<S>"; host-side query, no launch)."""
+    d = wgrad_desc(dys, xs, taps, cout, cin, act_fp16)
+    return lib().nrpn_conv3d_wgrad_variant(ctypes.byref(d)).decode()
+
+
 def conv3d_wgrad(dys: Sequence[torch.Tensor], xs: Sequence[torch.Tensor], taps: Sequence[Sequence[int]]) -> torch.Tensor:
     """dW (taps, Cout, Cin) fp32 of a stride-1 'same' conv from channels-last 16-bit dY (N,X,Y,Z,Cout) and X (N,X,Y,Z,Cin), one pair per
     pyramid level that shares the weights.  The tensors are read where they live (MN-major wgmma operands)."""

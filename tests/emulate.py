@@ -1,4 +1,4 @@
-"""Pure-torch statement of what nrpn_conv3d_fprop / nrpn_pack_stem_input and the Swin-3D / GroupNorm kernels compute (TEST
+"""Pure-torch statement of what nrpn_conv3d_fprop / nrpn_conv3d_wgrad / nrpn_pack_stem_input and the Swin-3D / GroupNorm kernels compute (TEST
 helper, CPU or GPU).  Used to check the host-side packing logic without a GPU and as the fp32 / float64 references for the CUDA
 kernels."""
 import math
@@ -96,6 +96,34 @@ def reference_conv64(x, w, taps, shift, out_dims, stride=1, act=0, res=None):
         ref = ref.clamp_min(0)
     elif act == 2:
         ref = 0.5 * ref * (1.0 + torch.erf(ref / math.sqrt(2.0)))
+    return ref, mag
+
+
+def reference_wgrad64(dys, xs, taps, x_dims=None):
+    """float64 statement of nrpn_conv3d_wgrad on the exact operands the kernel reads (CPU or GPU):
+        dW[tap][co][ci] = sum over levels, samples and voxels v of dY   dY[v][co] * X[v + tap][ci],   X zero outside its grid.
+
+    dys / xs: one (N,X,Y,Z,Cout) / (N,X',Y',Z',Cin) 16-bit tensor per level (the real channels: slice away any row padding).
+    x_dims: per level, the extent of X when it differs from dY's (the descriptor's xx / xy / xz); without it X must have dY's extent.
+    Returns (ref, mag), float64 (taps, Cout, Cin): mag is the same sum over |dY| |X| -- the scale of the rounding error of a float
+    accumulation."""
+    cout, cin = dys[0].shape[-1], xs[0].shape[-1]
+    P = max(max(abs(int(v)) for v in t) for t in taps)
+    ref = torch.zeros((len(taps), cout, cin), dtype=torch.float64, device=dys[0].device)
+    mag = torch.zeros_like(ref)
+    for i, (dy, x) in enumerate(zip(dys, xs)):
+        ext, xext = tuple(dy.shape[1:4]), tuple(x.shape[1:4])
+        want = ext if x_dims is None else tuple(x_dims[i])
+        assert xext == want and dy.shape[0] == x.shape[0], f"level {i}: X extent {xext}, expected {want}"
+        d = dy.double().reshape(-1, cout)
+        da = d.abs()
+        hi = [max(0, P + e - xe) for e, xe in zip(ext, xext)]
+        xp = F.pad(x.double(), (0, 0, P, hi[2], P, hi[1], P, hi[0]))
+        xa = xp.abs()
+        for t, (dx, dy_, dz) in enumerate(taps):
+            sl = (slice(None), slice(P + dx, P + dx + ext[0]), slice(P + dy_, P + dy_ + ext[1]), slice(P + dz, P + dz + ext[2]))
+            ref[t] += d.t() @ xp[sl].reshape(-1, cin)
+            mag[t] += da.t() @ xa[sl].reshape(-1, cin)
     return ref, mag
 
 

@@ -271,33 +271,6 @@ def test_conv_data_gradient_runs_on_the_forward_kernel(ops, dims, cin, cout, k):
     assert (dx - ref).abs().max().item() <= 2e-3 * ref.abs().max().item(), _diagnose(dx, ref, "dgrad")
 
 
-@pytest.mark.parametrize("level_dims,cin,cout,k,dtype", [
-    ([(8, 8, 16)], 64, 128, 3, torch.bfloat16),
-    ([(9, 12, 10), (5, 6, 5)], 128, 256, 3, torch.bfloat16),        # two levels sharing the weights, ragged bricks
-    ([(6, 7, 9)], 256, 128, 1, torch.float16),
-])
-def test_conv_weight_gradient_vs_autograd(ops, level_dims, cin, cout, k, dtype):
-    """dW of a stride-1 'same' Conv3d on wgmma (K = voxels; channels-last tensors as MN-major operands) against torch.autograd on the
-    rounded operands."""
-    g = torch.Generator(device="cuda").manual_seed(61)
-    w = torch.zeros((cout, cin, k, k, k), device="cuda", requires_grad=True)
-    dys, xs, ref = [], [], torch.zeros_like(w)
-    for dims in level_dims:
-        x = torch.randn((2, *dims, cin), device="cuda", generator=g).to(dtype)
-        dy = torch.randn((2, *dims, cout), device="cuda", generator=g).to(dtype)
-        y = F.conv3d(x.float().permute(0, 4, 1, 2, 3), w, padding=k // 2)
-        (gw,) = torch.autograd.grad(y, w, dy.float().permute(0, 4, 1, 2, 3))
-        ref += gw
-        xs.append(x); dys.append(dy)
-    taps = [(a - k // 2, b - k // 2, c - k // 2) for a in range(k) for b in range(k) for c in range(k)]
-    dw = ops.conv3d_wgrad(dys, xs, taps)
-    torch.cuda.synchronize()
-    refp = ref.permute(2, 3, 4, 0, 1).reshape(len(taps), cout, cin)
-    assert not torch.isnan(dw).any()
-    assert (dw - refp).abs().max().item() <= 2e-3 * refp.abs().max().item(), _diagnose(dw, refp, "wgrad")
-    assert torch.equal(dw, ops.conv3d_wgrad(dys, xs, taps)), "weight gradients must be bit-reproducible"
-
-
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 def test_bias_grad_and_relu_backward(ops, dtype):
     g = torch.Generator(device="cuda").manual_seed(71)
