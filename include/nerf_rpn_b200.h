@@ -143,8 +143,9 @@ typedef struct {
 
 /* Padding granularity of the output-channel axis for this cout (64, 128 or 256): w / shift must be padded to a multiple. */
 int nrpn_conv3d_block_n(int cout);
-/* Name of the kernel variant nrpn_conv3d_fprop would launch for this descriptor ("slab<4x16x8,N64>", "igemm<256,4,1>", ...;
- * "invalid" / "unsupported" when it would be rejected).  Pure host logic: pointers inside the descriptor are not dereferenced. */
+/* Name of the kernel instance nrpn_conv3d_fprop would launch for this descriptor ("slab<4x16x8,N64>", "igemm<256,4,1>",
+ * "igemm<256,4,1,tma-epilogue>", ...; "unsupported" when it would return NRPN_ERR_UNSUPPORTED, "invalid" when it would reject
+ * the descriptor otherwise).  Pure host logic, no device needed: pointers inside the descriptor are not dereferenced. */
 const char *nrpn_conv3d_variant(const nrpn_conv_desc *desc);
 int nrpn_conv3d_fprop(const nrpn_conv_desc *desc /*host*/, nrpn_stream_t stream);
 

@@ -22,8 +22,9 @@
 //     top-down path), ReLU / GELU, convert to bf16 / fp16 / fp32.  TMA_EPI variants (16-bit output) stage the tile in shared
 //     memory as 128 x 64 sub-tiles and store each with cp.async.bulk.tensor; the short reductions also prefetch a same-shape
 //     residual by TMA.
-//   - variants: <256,4,1> <128,6,1> <64,8,1> (long reductions, each with and without TMA_EPI; <64,8,1> also for layers with
-//     fewer tiles than SMs), <64,2,3> / <64,2,2,TMA_EPI> (reductions of at most 8 k-blocks).
+//   - instances (kConvInstances, which also holds the names nrpn_conv3d_variant reports): <256,4,1> <128,6,1> <64,8,1> (long
+//     reductions, each with and without TMA_EPI; <64,8,1> also for layers with fewer tiles than SMs), <64,2,3> /
+//     <64,2,2,TMA_EPI> (reductions of at most 8 k-blocks); with WS the long ones are <256,2,1> <128,4,1> <64,6,1>.
 #include <cstdlib>
 #include <type_traits>
 #include "common.cuh"
@@ -337,7 +338,7 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
 
 // ------------------------------------------------------------------------------------------------ host
 template <int BLOCK_N, int STAGES, int MIN_BLOCKS, bool TMA_EPI = false, bool WS = false>
-static int launch_conv(const ConvMaps& maps, const ConvDev& P, int total_tiles, cudaStream_t st) {
+static int launch_conv(const ConvMaps& maps, const ConvDev& P, cudaStream_t st) {
     constexpr int smem = STAGES * (kABytes + BLOCK_N * kBlockK * 2 * (WS ? 2 : 1)) +
                          (epi_res_slots(MIN_BLOCKS, TMA_EPI, WS) + epi_out_slots(MIN_BLOCKS, TMA_EPI)) * kEpiTileBytes + 1024 + 256;
     static_assert((smem + 1024) * MIN_BLOCKS <= 228 * 1024, "shared memory budget");
@@ -347,12 +348,35 @@ static int launch_conv(const ConvMaps& maps, const ConvDev& P, int total_tiles, 
                                            cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         attr_set = true;
     }
+    const int total_tiles = P.total_m_tiles * P.n_tiles_n;
     const int slots = num_sms() * MIN_BLOCKS;
     const int grid = total_tiles < slots ? total_tiles : slots;
     NRPN_CUDA_TRY(launch_pdl(conv3d_igemm_kernel<BLOCK_N, STAGES, MIN_BLOCKS, TMA_EPI, WS>, dim3(grid), dim3(kConvThreads), smem, st, total_tiles <= 2 * slots, maps, P));
     NRPN_LAUNCH_CHECK();
     return NRPN_OK;
 }
+
+// Every instance nrpn_conv3d_fprop launches, under the name nrpn_conv3d_variant reports for it.  Index:
+// 8 wsplit + 2 (0 for a short reduction, else 1 + log2(BLOCK_N / 64)) + TMA epilogue.
+struct ConvInstance { const char* name; int (*launch)(const ConvMaps&, const ConvDev&, cudaStream_t); };
+static const ConvInstance kConvInstances[16] = {
+    {"igemm<64,2,3>", launch_conv<64, 2, 3>},
+    {"igemm<64,2,2,tma-epilogue>", launch_conv<64, 2, 2, true>},
+    {"igemm<64,8,1>", launch_conv<64, 8, 1>},
+    {"igemm<64,8,1,tma-epilogue>", launch_conv<64, 8, 1, true>},
+    {"igemm<128,6,1>", launch_conv<128, 6, 1>},
+    {"igemm<128,6,1,tma-epilogue>", launch_conv<128, 6, 1, true>},
+    {"igemm<256,4,1>", launch_conv<256, 4, 1>},
+    {"igemm<256,4,1,tma-epilogue>", launch_conv<256, 4, 1, true>},
+    {"igemm<64,2,3,wsplit>", launch_conv<64, 2, 3, false, true>},
+    {"igemm<64,2,2,tma-epilogue,wsplit>", launch_conv<64, 2, 2, true, true>},
+    {"igemm<64,6,1,wsplit>", launch_conv<64, 6, 1, false, true>},
+    {"igemm<64,6,1,tma-epilogue,wsplit>", launch_conv<64, 6, 1, true, true>},
+    {"igemm<128,4,1,wsplit>", launch_conv<128, 4, 1, false, true>},
+    {"igemm<128,4,1,tma-epilogue,wsplit>", launch_conv<128, 4, 1, true, true>},
+    {"igemm<256,2,1,wsplit>", launch_conv<256, 2, 1, false, true>},
+    {"igemm<256,2,1,tma-epilogue,wsplit>", launch_conv<256, 2, 1, true, true>},
+};
 
 static void choose_brick(int xo, int yo, int zo, int& bx, int& by, int& bz) {
     long best = -1;
@@ -367,41 +391,86 @@ static void choose_brick(int xo, int yo, int zo, int& bx, int& by, int& bz) {
     }
 }
 
-struct ConvGeom { int pad_n, cout_pad, block_n, kblocks, m_tiles, n_tiles_n; bool short_k, tma_epi; };
+struct ConvPlan {
+    const ConvInstance* inst;   // nullptr: the halo-slab kernel (conv3d_slab.cu)
+    int block_n, cout_pad;      // N tile of the instance; Cout padded to nrpn_conv3d_block_n(cout)
+    bool tma_epi;               // shared-memory (TMA-store) epilogue
+    ConvDev P;
+};
 
-static int conv_geometry(const nrpn_conv_desc* d, ConvGeom& g) {
-    g.pad_n = nrpn_conv3d_block_n(d->cout);
-    g.cout_pad = ceil_div(d->cout, g.pad_n) * g.pad_n;
-    g.kblocks = d->n_taps * (d->cin / kBlockK);
-    g.short_k = g.kblocks <= 8;
-    g.block_n = g.short_k ? 64 : g.pad_n;
-    g.n_tiles_n = g.cout_pad / g.block_n;
+// Validates a descriptor and decides what nrpn_conv3d_fprop launches for it.  Host logic only: pointers are checked and
+// compared, never dereferenced.  The A/B switches NRPN_CONV_NARROW, NRPN_CONV_TMA_EPI (and NRPN_CONV_SLAB) are read on every call.
+static int conv_plan(const nrpn_conv_desc* d, ConvPlan& p) {
+    if (!d || !d->w || !d->shift) return NRPN_ERR_INVALID;
+    if (d->cin < 64 || d->cin % 64 != 0 || d->cout < 8 || d->cout % 8 != 0) return NRPN_ERR_UNSUPPORTED;
+    if (d->n_taps < 1 || d->n_taps > NRPN_CONV_MAX_TAPS || d->n_levels < 1 || d->n_levels > NRPN_CONV_MAX_LEVELS)
+        return NRPN_ERR_INVALID;
+    if (d->stride != 1 && d->stride != 2) return NRPN_ERR_UNSUPPORTED;
+    if (d->stride == 2) {       // strided access is expressed through a sub-sampled tensor map: taps must not move
+        for (int t = 0; t < d->n_taps; ++t)
+            if (d->tap_off[t][0] || d->tap_off[t][1] || d->tap_off[t][2]) return NRPN_ERR_UNSUPPORTED;
+    }
+    if (!conv_pairs_aligned(d)) return NRPN_ERR_INVALID;
+    for (int l = 0; l < d->n_levels; ++l) {
+        const nrpn_conv_level& S = d->level[l];
+        if (!S.x || !S.y || S.n < 1 || S.xi < 1 || S.yi < 1 || S.zi < 1 || S.xo < 1 || S.yo < 1 || S.zo < 1) return NRPN_ERR_INVALID;
+        if (S.ldy < d->cout || S.ldy % 8 != 0) return NRPN_ERR_INVALID;
+        if (S.res && (S.ldr < d->cout || S.ldr % 8 != 0 || S.xr < 1 || S.yr < 1 || S.zr < 1)) return NRPN_ERR_INVALID;
+        if (d->stride == 2 && (S.xo != (S.xi + 1) / 2 || S.yo != (S.yi + 1) / 2 || S.zo != (S.zi + 1) / 2)) return NRPN_ERR_INVALID;
+    }
+    p.inst = nullptr;
+    if (!d->wsplit && conv3d_slab_eligible(d)) return NRPN_OK;
+
+    ConvDev& P = p.P;
+    memset(&P, 0, sizeof(P));
+    P.n_levels = d->n_levels; P.n_taps = d->n_taps; P.kc_blocks = d->cin / kBlockK;
+    P.cout = d->cout; P.relu = d->relu; P.out_fp32 = d->out_fp32; P.shift = d->shift; P.fp16 = d->act_fp16 ? 1 : 0;
+    for (int t = 0; t < d->n_taps; ++t) { P.tap[t][0] = d->tap_off[t][0]; P.tap[t][1] = d->tap_off[t][1]; P.tap[t][2] = d->tap_off[t][2]; P.tap[t][3] = 0; }
     int tiles = 0;
     for (int l = 0; l < d->n_levels; ++l) {
         const nrpn_conv_level& S = d->level[l];
-        if (S.n < 1 || S.xo < 1 || S.yo < 1 || S.zo < 1) return NRPN_ERR_INVALID;
-        int bx, by, bz;
-        choose_brick(S.xo, S.yo, S.zo, bx, by, bz);
-        tiles += S.n * ceil_div(S.xo, bx) * ceil_div(S.yo, by) * ceil_div(S.zo, bz);
+        ConvLevelDev& L = P.lv[l];
+        L.n = S.n; L.xo = S.xo; L.yo = S.yo; L.zo = S.zo;
+        choose_brick(S.xo, S.yo, S.zo, L.bx, L.by, L.bz);
+        L.tx = ceil_div(S.xo, L.bx); L.ty = ceil_div(S.yo, L.by); L.tz = ceil_div(S.zo, L.bz);
+        L.tile_begin = tiles;
+        tiles += S.n * L.tx * L.ty * L.tz;
+        L.xr = S.res ? S.xr : S.xo; L.yr = S.res ? S.yr : S.yo; L.zr = S.res ? S.zr : S.zo;
+        L.rsx = (float)L.xr / (float)S.xo; L.rsy = (float)L.yr / (float)S.yo; L.rsz = (float)L.zr / (float)S.zo;
+        L.ldy = S.ldy; L.ldr = S.ldr; L.y = S.y; L.res = reinterpret_cast<const __nv_bfloat16*>(S.res);
     }
-    g.m_tiles = tiles;
+    P.total_m_tiles = tiles;
+
+    // Weights are padded to nrpn_conv3d_block_n(cout) (a multiple of 64). Long reductions (3^3 taps) use the widest N tile
+    // that fits, one CTA per SM, deep smem ring: tensor-pipe bound.  Short reductions (1^3 convs: at most 8 k-blocks) are
+    // HBM / epilogue-latency bound: they run N = 64 tiles with 3 CTAs per SM so that 3x more loads/stores are in flight.
+    const int pad_n = nrpn_conv3d_block_n(d->cout);
+    p.cout_pad = ceil_div(d->cout, pad_n) * pad_n;
+    const bool short_k = d->n_taps * P.kc_blocks <= 8;
+    p.block_n = short_k ? 64 : pad_n;
     // Late ResNet stages (5x8x8 .. 10x16x16 voxels, K up to 13 824): a handful of 128 x 256 tiles leaves most SMs idle while each
     // tile runs a long reduction.  When even 64-wide tiles fit in one wave, they are used instead: 4x the CTAs (same reduction
     // order per output element, bit-identical results).
-    if (!g.short_k && g.block_n > 64 && tiles * (g.cout_pad / 64) <= num_sms()) {
+    if (!short_k && p.block_n > 64 && tiles * (p.cout_pad / 64) <= num_sms()) {
         const char* e = getenv("NRPN_CONV_NARROW");
-        if (!(e && e[0] == '0')) { g.block_n = 64; g.n_tiles_n = g.cout_pad / 64; }
+        if (!(e && e[0] == '0')) p.block_n = 64;
     }
+    P.n_tiles_n = p.cout_pad / p.block_n;
     // shared-memory (TMA) epilogue: 16-bit output; the short reductions also need whole 64-channel output tiles
-    { const char* e = getenv("NRPN_CONV_TMA_EPI"); g.tma_epi = !(e && e[0] == '0'); }       // A/B switch for tests and profiling
-    g.tma_epi = g.tma_epi && !d->out_fp32 && (!g.short_k || d->cout % 64 == 0);
-    for (int l = 0; l < d->n_levels && g.tma_epi; ++l) {
+    { const char* e = getenv("NRPN_CONV_TMA_EPI"); p.tma_epi = !(e && e[0] == '0'); }       // A/B switch for tests and profiling
+    p.tma_epi = p.tma_epi && !d->out_fp32 && (!short_k || d->cout % 64 == 0);
+    for (int l = 0; l < d->n_levels; ++l) {
         const nrpn_conv_level& S = d->level[l];
-        if (reinterpret_cast<uintptr_t>(S.y) % 16 != 0 || (S.res && reinterpret_cast<uintptr_t>(S.res) % 16 != 0)) g.tma_epi = false;
+        const ConvLevelDev& L = P.lv[l];
+        if (reinterpret_cast<uintptr_t>(S.y) % 16 != 0 || (S.res && reinterpret_cast<uintptr_t>(S.res) % 16 != 0)) p.tma_epi = false;
         // a nearest-upsampled residual (FPN top-down) is gathered per row from registers: the pipelined register epilogue
         // with 3 CTAs per SM is faster for it (measured: lat3+up 0.207 ms vs 0.275 ms)
-        if (S.res && (S.xr != S.xo || S.yr != S.yo || S.zr != S.zo)) g.tma_epi = false;
+        if (L.xr != L.xo || L.yr != L.yo || L.zr != L.zo) p.tma_epi = false;
     }
+    // once tma_epi holds, every residual has the output's extent: the short reductions prefetch it through maps.r
+    for (int l = 0; l < d->n_levels; ++l) P.lv[l].res_tma = (p.tma_epi && short_k && d->level[l].res) ? 1 : 0;
+    const int tile_kind = short_k ? 0 : (p.block_n == 64 ? 1 : (p.block_n == 128 ? 2 : 3));
+    p.inst = &kConvInstances[8 * (d->wsplit ? 1 : 0) + 2 * tile_kind + (p.tma_epi ? 1 : 0)];
     return NRPN_OK;
 }
 
@@ -415,85 +484,36 @@ extern "C" {
 int nrpn_conv3d_block_n(int cout) { return cout <= 64 ? 64 : (cout <= 128 ? 128 : 256); }
 
 const char* nrpn_conv3d_variant(const nrpn_conv_desc* d) {
-    if (!d || d->n_taps < 1 || d->n_taps > NRPN_CONV_MAX_TAPS || d->n_levels < 1 || d->n_levels > NRPN_CONV_MAX_LEVELS) return "invalid";
-    if (d->cin < 64 || d->cin % 64 != 0 || d->cout < 8 || d->cout % 8 != 0 || (d->stride != 1 && d->stride != 2)) return "unsupported";
-    if (!conv_pairs_aligned(d)) return "invalid";
-    if (!d->wsplit && conv3d_slab_eligible(d)) return "slab<4x16x8,N64>";
-    ConvGeom g;
-    if (conv_geometry(d, g) != NRPN_OK) return "invalid";
-    if (d->wsplit) {
-        if (g.short_k) return g.tma_epi ? "igemm<64,2,2,tma-epilogue,wsplit>" : "igemm<64,2,3,wsplit>";
-        return g.block_n == 64 ? "igemm<64,6,1,wsplit>" : (g.block_n == 128 ? "igemm<128,4,1,wsplit>" : "igemm<256,2,1,wsplit>");
-    }
-    if (g.short_k) return g.tma_epi ? "igemm<64,2,2,tma-epilogue>" : "igemm<64,2,3>";
-    return g.block_n == 64 ? "igemm<64,8,1>" : (g.block_n == 128 ? "igemm<128,6,1>" : "igemm<256,4,1>");
+    ConvPlan p;
+    const int rc = conv_plan(d, p);
+    if (rc == NRPN_ERR_UNSUPPORTED) return "unsupported";
+    if (rc != NRPN_OK) return "invalid";
+    return p.inst ? p.inst->name : "slab<4x16x8,N64>";
 }
 
 int nrpn_conv3d_fprop(const nrpn_conv_desc* d, nrpn_stream_t stream) {
-    if (!d || !d->w || !d->shift) return NRPN_ERR_INVALID;
-    if (d->cin < 64 || d->cin % 64 != 0 || d->cout < 8 || d->cout % 8 != 0) return NRPN_ERR_UNSUPPORTED;
-    if (d->n_taps < 1 || d->n_taps > NRPN_CONV_MAX_TAPS || d->n_levels < 1 || d->n_levels > NRPN_CONV_MAX_LEVELS)
-        return NRPN_ERR_INVALID;
-    if (d->stride != 1 && d->stride != 2) return NRPN_ERR_UNSUPPORTED;
-    if (d->stride == 2) {       // strided access is expressed through a sub-sampled tensor map: taps must not move
-        for (int t = 0; t < d->n_taps; ++t)
-            if (d->tap_off[t][0] || d->tap_off[t][1] || d->tap_off[t][2]) return NRPN_ERR_UNSUPPORTED;
-    }
-    if (!conv_pairs_aligned(d)) return NRPN_ERR_INVALID;
-    EncodeTiledFn encode = get_encode();
-    if (!encode) return NRPN_ERR_NO_DEVICE;
-    if (!d->wsplit && conv3d_slab_eligible(d)) return conv3d_slab_launch(d, (cudaStream_t)stream);
+    ConvPlan p;
+    { const int rc = conv_plan(d, p); if (rc) return rc; }
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!p.inst) return conv3d_slab_launch(d, st);
 
-    // Weights are padded to nrpn_conv3d_block_n(cout) (a multiple of 64). Long reductions (3^3 taps) use the widest N tile
-    // that fits, one CTA per SM, deep smem ring: tensor-pipe bound.  Short reductions (1^3 convs: at most 8 k-blocks) are
-    // HBM / epilogue-latency bound: they run N = 64 tiles with 3 CTAs per SM so that 3x more loads/stores are in flight.
-    ConvGeom geo;
-    { const int rc = conv_geometry(d, geo); if (rc) return rc; }
-    const int cout_pad = geo.cout_pad;
-    const bool short_k = geo.short_k;
-    const int block_n = geo.block_n;
     ConvMaps maps;
-    ConvDev P;
-    memset(&P, 0, sizeof(P));
-    P.n_levels = d->n_levels; P.n_taps = d->n_taps; P.kc_blocks = d->cin / kBlockK; P.n_tiles_n = cout_pad / block_n;
-    P.cout = d->cout; P.relu = d->relu; P.out_fp32 = d->out_fp32; P.shift = d->shift; P.fp16 = d->act_fp16 ? 1 : 0;
-    for (int t = 0; t < d->n_taps; ++t) { P.tap[t][0] = d->tap_off[t][0]; P.tap[t][1] = d->tap_off[t][1]; P.tap[t][2] = d->tap_off[t][2]; P.tap[t][3] = 0; }
-
-    int tiles = 0;
     const int s = d->stride;
     for (int l = 0; l < d->n_levels; ++l) {
         const nrpn_conv_level& S = d->level[l];
-        ConvLevelDev& L = P.lv[l];
-        if (!S.x || !S.y || S.n < 1 || S.xi < 1 || S.yi < 1 || S.zi < 1 || S.xo < 1 || S.yo < 1 || S.zo < 1) return NRPN_ERR_INVALID;
-        if (S.ldy < d->cout || S.ldy % 8 != 0) return NRPN_ERR_INVALID;
-        if (S.res && (S.ldr < d->cout || S.ldr % 8 != 0 || S.xr < 1 || S.yr < 1 || S.zr < 1)) return NRPN_ERR_INVALID;
-        if (s == 2 && (S.xo != (S.xi + 1) / 2 || S.yo != (S.yi + 1) / 2 || S.zo != (S.zi + 1) / 2)) return NRPN_ERR_INVALID;
-        L.n = S.n; L.xo = S.xo; L.yo = S.yo; L.zo = S.zo;
-        choose_brick(S.xo, S.yo, S.zo, L.bx, L.by, L.bz);
-        L.tx = ceil_div(S.xo, L.bx); L.ty = ceil_div(S.yo, L.by); L.tz = ceil_div(S.zo, L.bz);
-        L.tile_begin = tiles;
-        tiles += S.n * L.tx * L.ty * L.tz;
-        L.xr = S.res ? S.xr : S.xo; L.yr = S.res ? S.yr : S.yo; L.zr = S.res ? S.zr : S.zo;
-        L.rsx = (float)L.xr / (float)S.xo; L.rsy = (float)L.yr / (float)S.yo; L.rsz = (float)L.zr / (float)S.zo;
-        L.ldy = S.ldy; L.ldr = S.ldr; L.y = S.y; L.res = reinterpret_cast<const __nv_bfloat16*>(S.res);
-        L.res_tma = (geo.tma_epi && short_k && S.res && S.xr == S.xo && S.yr == S.yo && S.zr == S.zo) ? 1 : 0;
-        if (geo.tma_epi) {
+        const ConvLevelDev& L = p.P.lv[l];
+        if (p.tma_epi) {
             // output / residual tensors (C, Z, Y, X, N) with the row pitch ldy / ldr; one box = one 64-channel brick tile
             cuuint32_t ebox[5] = {64, (cuuint32_t)L.bz, (cuuint32_t)L.by, (cuuint32_t)L.bx, 1};
-            cuuint32_t eone[5] = {1, 1, 1, 1, 1};
             cuuint64_t ydim[5] = {(cuuint64_t)d->cout, (cuuint64_t)S.zo, (cuuint64_t)S.yo, (cuuint64_t)S.xo, (cuuint64_t)S.n};
             cuuint64_t ystr[4] = {(cuuint64_t)S.ldy * 2, (cuuint64_t)S.zo * S.ldy * 2, (cuuint64_t)S.yo * S.zo * S.ldy * 2,
                                   (cuuint64_t)S.xo * S.yo * S.zo * S.ldy * 2};
-            CUresult ry = encode(&maps.y[l], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, S.y, ydim, ystr, ebox, eone, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (ry != CUDA_SUCCESS) { g_last_cuda_error = (int)ry; return NRPN_ERR_CUDA; }
+            { const int rc = encode_tmap(&maps.y[l], S.y, ydim, ystr, ebox); if (rc) return rc; }
             if (L.res_tma) {
                 cuuint64_t rstr[4] = {(cuuint64_t)S.ldr * 2, (cuuint64_t)S.zo * S.ldr * 2, (cuuint64_t)S.yo * S.zo * S.ldr * 2,
                                       (cuuint64_t)S.xo * S.yo * S.zo * S.ldr * 2};
-                CUresult rr = encode(&maps.r[l], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(S.res), ydim, rstr, ebox, eone,
-                                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-                if (rr != CUDA_SUCCESS) { g_last_cuda_error = (int)rr; return NRPN_ERR_CUDA; }
+                const int rc = encode_tmap(&maps.r[l], S.res, ydim, rstr, ebox);
+                if (rc) return rc;
             } else maps.r[l] = maps.y[l];
         }
 
@@ -503,51 +523,20 @@ int nrpn_conv3d_fprop(const nrpn_conv_desc* d, nrpn_stream_t stream) {
         cuuint64_t gstr[4] = {cin * 2 * s, (cuuint64_t)S.zi * cin * 2 * s, (cuuint64_t)S.yi * S.zi * cin * 2 * s,
                               (cuuint64_t)S.xi * S.yi * S.zi * cin * 2};
         cuuint32_t box[5] = {(cuuint32_t)kBlockK, (cuuint32_t)L.bz, (cuuint32_t)L.by, (cuuint32_t)L.bx, 1};
-        cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-        CUresult r = encode(&maps.x[l], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(S.x), gdim, gstr, box, estr,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { g_last_cuda_error = (int)r; return NRPN_ERR_CUDA; }
+        { const int rc = encode_tmap(&maps.x[l], S.x, gdim, gstr, box); if (rc) return rc; }
     }
     for (int l = d->n_levels; l < NRPN_CONV_MAX_LEVELS; ++l) { maps.x[l] = maps.x[0]; maps.y[l] = maps.y[0]; maps.r[l] = maps.r[0]; }
-    if (!geo.tma_epi) for (int l = 0; l < NRPN_CONV_MAX_LEVELS; ++l) { maps.y[l] = maps.x[0]; maps.r[l] = maps.x[0]; }
+    if (!p.tma_epi) for (int l = 0; l < NRPN_CONV_MAX_LEVELS; ++l) { maps.y[l] = maps.x[0]; maps.r[l] = maps.x[0]; }
     {
         // wsplit: (taps, 2, CoutPad, cin) -- the hi and lo planes of a tap are consecutive slices, one box of depth 2 fetches both
         const int planes = d->wsplit ? 2 : 1;
-        cuuint64_t gdim[3] = {(cuuint64_t)d->cin, (cuuint64_t)cout_pad, (cuuint64_t)d->n_taps * planes};
-        cuuint64_t gstr[2] = {(cuuint64_t)d->cin * 2, (cuuint64_t)cout_pad * d->cin * 2};
-        cuuint32_t box[3] = {(cuuint32_t)kBlockK, (cuuint32_t)block_n, (cuuint32_t)planes};
-        cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = encode(&maps.w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(d->w), gdim, gstr, box, estr,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { g_last_cuda_error = (int)r; return NRPN_ERR_CUDA; }
+        cuuint64_t gdim[3] = {(cuuint64_t)d->cin, (cuuint64_t)p.cout_pad, (cuuint64_t)d->n_taps * planes};
+        cuuint64_t gstr[2] = {(cuuint64_t)d->cin * 2, (cuuint64_t)p.cout_pad * d->cin * 2};
+        cuuint32_t box[3] = {(cuuint32_t)kBlockK, (cuuint32_t)p.block_n, (cuuint32_t)planes};
+        const int rc = encode_tmap(&maps.w, d->w, gdim, gstr, box);
+        if (rc) return rc;
     }
-    P.total_m_tiles = tiles;
-    const int total_tiles = tiles * P.n_tiles_n;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (d->wsplit) {
-        if (short_k && geo.tma_epi) return launch_conv<64, 2, 2, true, true>(maps, P, total_tiles, st);
-        if (short_k) return launch_conv<64, 2, 3, false, true>(maps, P, total_tiles, st);
-        if (geo.tma_epi) {
-            if (block_n == 64) return launch_conv<64, 6, 1, true, true>(maps, P, total_tiles, st);
-            if (block_n == 128) return launch_conv<128, 4, 1, true, true>(maps, P, total_tiles, st);
-            return launch_conv<256, 2, 1, true, true>(maps, P, total_tiles, st);
-        }
-        if (block_n == 64) return launch_conv<64, 6, 1, false, true>(maps, P, total_tiles, st);
-        if (block_n == 128) return launch_conv<128, 4, 1, false, true>(maps, P, total_tiles, st);
-        return launch_conv<256, 2, 1, false, true>(maps, P, total_tiles, st);
-    }
-    if (short_k && geo.tma_epi) return launch_conv<64, 2, 2, true>(maps, P, total_tiles, st);
-    if (short_k) return launch_conv<64, 2, 3>(maps, P, total_tiles, st);
-    if (geo.tma_epi) {
-        if (block_n == 64) return launch_conv<64, 8, 1, true>(maps, P, total_tiles, st);
-        if (block_n == 128) return launch_conv<128, 6, 1, true>(maps, P, total_tiles, st);
-        return launch_conv<256, 4, 1, true>(maps, P, total_tiles, st);
-    }
-    if (block_n == 64) return launch_conv<64, 8, 1>(maps, P, total_tiles, st);
-    if (block_n == 128) return launch_conv<128, 6, 1>(maps, P, total_tiles, st);
-    return launch_conv<256, 4, 1>(maps, P, total_tiles, st);
+    return p.inst->launch(maps, p.P, st);
 }
 
 #pragma GCC visibility pop

@@ -270,10 +270,6 @@ int conv3d_slab_launch(const nrpn_conv_desc* d, cudaStream_t st) {
     memset(&P, 0, sizeof(P));
     if (!slab_plan(d, P)) return NRPN_ERR_UNSUPPORTED;
     const nrpn_conv_level& S = d->level[0];
-    if (!S.x || !S.y || S.n < 1 || S.xo < 1 || S.yo < 1 || S.zo < 1) return NRPN_ERR_INVALID;
-    if (S.ldy < d->cout || S.ldy % 8 != 0 || !conv_pairs_aligned(d)) return NRPN_ERR_INVALID;
-    EncodeTiledFn encode = get_encode();
-    if (!encode) return NRPN_ERR_NO_DEVICE;
     P.n = S.n; P.xo = S.xo; P.yo = S.yo; P.zo = S.zo;
     P.tx = ceil_div(S.xo, kSlabAcc); P.ty = ceil_div(S.yo, kSlabTileY); P.tz = ceil_div(S.zo, kSlabTileZ);
     P.total_tiles = S.n * P.tx * P.ty * P.tz;
@@ -285,21 +281,15 @@ int conv3d_slab_launch(const nrpn_conv_desc* d, cudaStream_t st) {
         cuuint64_t gdim[5] = {64, (cuuint64_t)S.zi, (cuuint64_t)S.yi, (cuuint64_t)S.xi, (cuuint64_t)S.n};
         cuuint64_t gstr[4] = {128, (cuuint64_t)S.zi * 128, (cuuint64_t)S.yi * S.zi * 128, (cuuint64_t)S.xi * S.yi * S.zi * 128};
         cuuint32_t box[5] = {64, (cuuint32_t)kSlabTileZ, (cuuint32_t)(P.plane_bytes / 1024), 1, 1};
-        cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-        CUresult r = encode(&maps.x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(S.x), gdim, gstr, box, estr,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { g_last_cuda_error = (int)r; return NRPN_ERR_CUDA; }
+        const int rc = encode_tmap(&maps.x, S.x, gdim, gstr, box);
+        if (rc) return rc;
     }
     {   // weights (Cin, CoutPad = 64, taps)
         cuuint64_t gdim[3] = {64, 64, (cuuint64_t)d->n_taps};
         cuuint64_t gstr[2] = {128, 64 * 128};
         cuuint32_t box[3] = {64, 64, 1};
-        cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = encode(&maps.w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(d->w), gdim, gstr, box, estr,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { g_last_cuda_error = (int)r; return NRPN_ERR_CUDA; }
+        const int rc = encode_tmap(&maps.w, d->w, gdim, gstr, box);
+        if (rc) return rc;
     }
     const int smem = 1024 + P.slots * P.plane_bytes + kSlabBStages * kSlabBBytes + 512;
     static int smem_set = 0;

@@ -273,14 +273,11 @@ static int wgrad_plan(const nrpn_wgrad_desc* d, WgDev& P) {
 static int wgrad_run(const nrpn_wgrad_desc* d, cudaStream_t st) {
     WgDev P;
     { const int rc = wgrad_plan(d, P); if (rc) return rc; }
-    EncodeTiledFn encode = get_encode();
-    if (!encode) return NRPN_ERR_NO_DEVICE;
     WgMaps maps;
     const CUtensorMapDataType dt = d->act_fp16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     for (int l = 0; l < d->n_levels; ++l) {
         const nrpn_wgrad_level& S = d->level[l];
         const WgLevel& L = P.lv[l];
-        cuuint32_t one[5] = {1, 1, 1, 1, 1};
         cuuint32_t box[5] = {64, (cuuint32_t)L.bz, (cuuint32_t)L.by, (cuuint32_t)L.bx, 1};
         // dY: (cout, Z, Y, X, N) with the extents of the OUTPUT grid; X: the input grid (its own extents when they differ)
         const int xz = S.xz > 0 ? S.xz : S.z, xy = S.xy > 0 ? S.xy : S.y, xx = S.xx > 0 ? S.xx : S.x;
@@ -288,17 +285,15 @@ static int wgrad_run(const nrpn_wgrad_desc* d, cudaStream_t st) {
             cuuint64_t gdim[5] = {(cuuint64_t)d->cout, (cuuint64_t)S.z, (cuuint64_t)S.y, (cuuint64_t)S.x, (cuuint64_t)S.n};
             const cuuint64_t e = (cuuint64_t)S.ld_dy * 2;
             cuuint64_t gstr[4] = {e, e * S.z, e * S.z * S.y, e * S.z * S.y * S.x};
-            CUresult r = encode(&maps.dy[l], dt, 5, const_cast<void*>(S.dy_cl), gdim, gstr, box, one, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (r != CUDA_SUCCESS) { g_last_cuda_error = (int)r; return NRPN_ERR_CUDA; }
+            const int rc = encode_tmap(&maps.dy[l], S.dy_cl, gdim, gstr, box, dt);
+            if (rc) return rc;
         }
         {
             cuuint64_t gdim[5] = {(cuuint64_t)d->cin, (cuuint64_t)xz, (cuuint64_t)xy, (cuuint64_t)xx, (cuuint64_t)S.n};
             const cuuint64_t e = (cuuint64_t)S.ld_x * 2;
             cuuint64_t gstr[4] = {e, e * xz, e * xz * xy, e * xz * xy * xx};
-            CUresult r = encode(&maps.x[l], dt, 5, const_cast<void*>(S.x_cl), gdim, gstr, box, one, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (r != CUDA_SUCCESS) { g_last_cuda_error = (int)r; return NRPN_ERR_CUDA; }
+            const int rc = encode_tmap(&maps.x[l], S.x_cl, gdim, gstr, box, dt);
+            if (rc) return rc;
         }
     }
     for (int l = d->n_levels; l < NRPN_CONV_MAX_LEVELS; ++l) { maps.dy[l] = maps.dy[0]; maps.x[l] = maps.x[0]; }

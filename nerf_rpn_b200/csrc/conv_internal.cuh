@@ -1,4 +1,4 @@
-// Internal (not exported) declarations shared by the two convolution translation units.
+// Internal (not exported) declarations shared by the convolution translation units (igemm, halo-slab, weight gradient).
 #pragma once
 #include <cuda.h>
 #include <cstdlib>
@@ -24,6 +24,22 @@ inline EncodeTiledFn get_encode() {
             fn = reinterpret_cast<EncodeTiledFn>(p);
     }
     return fn;
+}
+
+// Encodes a tiled tensor map with the settings every convolution map shares: 128B swizzle, 256B L2 promotion, out-of-bounds
+// elements read as zero (no NaN fill), unit element strides.  The bf16 default moves fp16 data just as well: TMA copies bytes.
+// NRPN_ERR_NO_DEVICE without the driver entry point; NRPN_ERR_CUDA (and nrpn_last_cuda_error) when the driver refuses the map.
+template <int RANK>
+inline int encode_tmap(CUtensorMap* map, const void* base, const cuuint64_t (&dims)[RANK], const cuuint64_t (&strides)[RANK - 1],
+                       const cuuint32_t (&box)[RANK], CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
+    EncodeTiledFn encode = get_encode();
+    if (!encode) return NRPN_ERR_NO_DEVICE;
+    cuuint32_t estr[RANK];
+    for (int i = 0; i < RANK; ++i) estr[i] = 1;
+    const CUresult r = encode(map, dt, RANK, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { g_last_cuda_error = (int)r; return NRPN_ERR_CUDA; }
+    return NRPN_OK;
 }
 
 // Launch with programmatic stream serialization (the kernel must call ptx::pdl_wait() before reading its inputs): the
@@ -55,7 +71,8 @@ inline bool conv_pairs_aligned(const nrpn_conv_desc* d) {
 }
 
 // conv3d_slab.cu: halo-slab kernel for 64 -> (<=64)-channel stride-1 convolutions with a full box of filter taps.
-// Returns true when the descriptor is of that shape (the caller then launches it with conv3d_slab_launch).
+// Returns true when the descriptor is of that shape (the caller then launches it with conv3d_slab_launch, on a descriptor
+// nrpn_conv3d_fprop has validated).
 bool conv3d_slab_eligible(const nrpn_conv_desc* d);
 int conv3d_slab_launch(const nrpn_conv_desc* d, cudaStream_t st);
 

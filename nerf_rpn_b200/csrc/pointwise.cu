@@ -348,7 +348,7 @@ int nrpn_pack_stem_input_s1(const float* grid, int n, int x, int y, int z, void*
     return NRPN_OK;
 }
 
-int nrpn_version(void) { return 104; }
+int nrpn_version(void) { return 105; }
 
 const char* nrpn_status_string(int status) {
     switch (status) {

@@ -34,6 +34,29 @@ def test_host_only_queries():
     assert L.nrpn_nms_workspace_bytes(0) > 0
 
 
+def test_conv_variant_query_needs_no_device():
+    """nrpn_conv3d_variant names the exact instance nrpn_conv3d_fprop launches (the epilogue included) and refuses what it refuses."""
+    L = _lib.lib()
+    d = _lib.ConvDesc()
+    d.cin, d.cout, d.stride, d.n_levels = 256, 256, 1, 1
+    taps = [(a, b, c) for a in (-1, 0, 1) for b in (-1, 0, 1) for c in (-1, 0, 1)]
+    d.n_taps = len(taps)
+    for t, off in enumerate(taps):
+        d.tap_off[t][0], d.tap_off[t][1], d.tap_off[t][2] = off
+    d.w, d.shift = 1 << 32, 2 << 32                                 # pointers are checked, never dereferenced
+    lv = d.level[0]
+    lv.x, lv.y, lv.n, lv.ldy = 3 << 32, 4 << 32, 1, 256
+    lv.xi, lv.yi, lv.zi = lv.xo, lv.yo, lv.zo = (40, 48, 64)
+    name = lambda: L.nrpn_conv3d_variant(ctypes.byref(d)).decode()
+    assert name() == "igemm<256,4,1,tma-epilogue>"
+    d.out_fp32 = 1
+    assert name() == "igemm<256,4,1>"
+    d.stride = 2                                                    # strided taps must not move
+    assert name() == "unsupported"
+    d.stride, lv.x = 1, 0
+    assert name() == "invalid"
+
+
 def test_ctypes_struct_layouts_match_header():
     code = r'''
 #include <stdio.h>

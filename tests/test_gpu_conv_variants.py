@@ -1,7 +1,8 @@
-"""Every kernel variant nrpn_conv3d_fprop can launch, against the float64 reference (tests/emulate.py:reference_conv64).
+"""Every kernel instance nrpn_conv3d_fprop can launch, against the float64 reference (tests/emulate.py:reference_conv64).
 
-One table: each row names the exact variant it expects, so that a change of the tile rule cannot move a row to another kernel
-unnoticed.  Every row checks the same things:
+One table: each row names the exact instance it expects, so that a change of the tile or epilogue rule cannot move a row to
+another kernel unnoticed, and every launchable instance has a row (test_rows_cover_every_instance).  Every row checks the same
+things:
   - nothing unwritten, nothing over-written: y is NaN-filled with ldy = cout + 8 and guard elements before and after it; the
     weight rows and shift entries cout..CoutPad are NaN (and so are residual columns cout..ldr).  Afterwards every column below
     cout is finite and every other element is still the NaN it was, bit for bit;
@@ -11,8 +12,12 @@ unnoticed.  Every row checks the same things:
     Rows marked `exact` draw every operand from a coarse grid, so that every product and partial sum is exact in fp32 and the
     only error left is the epilogue's: their bound is  r |ref| + 2^-21 |pre-activation| + 2^-24, the fp32 GELU's error with
     room to spare, which a wrong GELU constant or any other epilogue slip exceeds;
-  - the bit-identities the code claims: TMA versus register epilogue (NRPN_CONV_TMA_EPI=0), narrow versus wide long-K tiles
+  - the bit-identities the code claims: TMA versus register epilogue (NRPN_CONV_TMA_EPI=0 turns a `,tma-epilogue` instance
+    into its register-epilogue twin and leaves every other row on its instance), narrow versus wide long-K tiles
     (NRPN_CONV_NARROW=0), and a 4-level launch versus its levels launched one at a time.
+The TMA-store epilogue stages 128 x 64 sub-tiles in shared memory and stores them with cp.async.bulk.tensor, which clips partial
+bricks and the channels past Cout; the `fallback` rows are cases it does not take (fp32 output, y not 16-byte aligned, a
+nearest-upsampled residual).
 Run with -s to see the worst err / bound of every row."""
 import dataclasses
 import math
@@ -50,7 +55,11 @@ class Row:
     levels: Optional[tuple] = None           # multi-level launch: the (X, Y, Z) of each level (dims unused)
     narrow: bool = False                     # long-K layer narrowed to 64-wide tiles: bit-identical to the wide tiles
     exact: bool = False                      # operands on a coarse grid: the fp32 accumulation is exact (see Case)
+    # elements in front of y, moving its base address; not part of the seed, so a shifted row draws the same operands
+    y_offset: int = dataclasses.field(default=0, repr=False)
 
+
+LEVELS = ((16, 16, 32), (8, 8, 16), (5, 6, 7), (3, 2, 2))
 
 ROWS = {
     # ---- short reductions (1^3), TMA epilogue: 16-bit output, cout % 64 == 0, same-extent or no residual
@@ -64,21 +73,47 @@ ROWS = {
     "reg_fp16_up_13_9": Row("igemm<64,2,3>", (13, 9, 4), 256, 256, k=1, dtype="fp16", res=(7, 5, 2)),
     "reg_bf16_relu_res_wrap": Row("igemm<64,2,3>", (16, 24, 40), 64, 120, k=1, relu=1, res="same", wrap=True),
     # ---- long reductions (3^3 taps)
-    "long64_bf16_relu_wrap": Row("igemm<64,8,1>", (12, 16, 48), 128, 40, relu=1, wrap=True),
-    "long64_narrow_fp16_gelu_k13824": Row("igemm<64,8,1>", (5, 8, 8), 512, 200, dtype="fp16", relu=2, n=1, narrow=True),
+    "long64_bf16_relu_wrap": Row("igemm<64,8,1,tma-epilogue>", (12, 16, 48), 128, 40, relu=1, wrap=True),
+    "long64_narrow_fp16_gelu_k13824": Row("igemm<64,8,1,tma-epilogue>", (5, 8, 8), 512, 200, dtype="fp16", relu=2, n=1,
+                                          narrow=True),
+    "long64_narrow_bf16_res_c200": Row("igemm<64,8,1,tma-epilogue>", (5, 8, 8), 512, 200, relu=1, res="same", n=1, narrow=True),
     "long128_bf16_f32_res_wrap": Row("igemm<128,6,1>", (10, 16, 60), 64, 120, out_fp32=True, res="same", wrap=True),
+    "long128_fp16_relu_res_c120_wrap": Row("igemm<128,6,1,tma-epilogue>", (10, 16, 60), 64, 120, dtype="fp16", relu=1,
+                                           res="same", wrap=True),
+    "long128_bf16_4_levels": Row("igemm<128,6,1,tma-epilogue>", None, 64, 128, relu=1, n=1, levels=LEVELS),
     "long256_fp16_relu_up_wrap": Row("igemm<256,4,1>", (12, 16, 96), 64, 200, dtype="fp16", relu=1, res=(7, 9, 55), n=1,
                                      wrap=True),
+    # 128 x 256 tiles: Cout 200 leaves the last 64-channel sub-tile 8 channels wide; z = 95 leaves partial bricks
+    "long256_bf16_relu_c200_wrap": Row("igemm<256,4,1,tma-epilogue>", (12, 16, 95), 64, 200, relu=1, n=1, wrap=True),
+    "long256_fp16_gelu_4_levels": Row("igemm<256,4,1,tma-epilogue>", None, 64, 136, dtype="fp16", relu=2, n=1, levels=LEVELS),
+    "long256_bf16_res_wrap": Row("igemm<256,4,1,tma-epilogue>", (12, 16, 96), 64, 256, res="same", n=1, wrap=True),
+    # ---- long reductions the TMA store does not take: the register epilogue
+    "fallback_long256_f32_out": Row("igemm<256,4,1>", (12, 16, 40), 64, 200, out_fp32=True, relu=1, n=1),
+    "fallback_long256_y_not_16B_aligned": Row("igemm<256,4,1>", (12, 16, 40), 64, 200, relu=1, n=1, y_offset=2),
+    "fallback_long128_upsampled_res": Row("igemm<128,6,1>", (12, 16, 48), 64, 128, dtype="fp16", relu=1, res=(6, 9, 21), n=1),
     # ---- weight split (hi + lo planes)
     "ws_tma_fp16_res_wrap": Row("igemm<64,2,2,tma-epilogue,wsplit>", (16, 24, 32), 64, 256, k=1, dtype="fp16", relu=1,
                                 res="same", n=1, wsplit=True, wrap=True),             # the fp16_w2 bottleneck c3 convolution
+    "ws_tma_fp16_4_levels": Row("igemm<64,2,2,tma-epilogue,wsplit>", None, 128, 64, k=1, dtype="fp16", relu=1, res="same", n=1,
+                                wsplit=True, levels=((8, 8, 16), (5, 6, 7), (1, 4, 30), (3, 2, 2))),   # one-slot residual ring
     "ws_reg_fp16_gelu_up": Row("igemm<64,2,3,wsplit>", (13, 9, 2), 256, 120, k=1, dtype="fp16", relu=2, res=(7, 5, 1),
                                wsplit=True),
-    "ws_long64_narrow_fp16": Row("igemm<64,6,1,wsplit>", (5, 8, 8), 256, 256, dtype="fp16", relu=1, n=1, wsplit=True,
-                                 narrow=True),
+    "ws_long64_narrow_fp16": Row("igemm<64,6,1,tma-epilogue,wsplit>", (5, 8, 8), 256, 256, dtype="fp16", relu=1, n=1,
+                                 wsplit=True, narrow=True),
+    "ws_long64_fp16_c40_wrap": Row("igemm<64,6,1,tma-epilogue,wsplit>", (12, 16, 48), 128, 40, dtype="fp16", relu=1,
+                                   wsplit=True, wrap=True),                          # Cout <= 64: 64-wide without narrowing
+    "ws_long64_narrow_fp16_f32": Row("igemm<64,6,1,wsplit>", (5, 8, 8), 256, 256, dtype="fp16", out_fp32=True, relu=1, n=1,
+                                     wsplit=True, narrow=True),
     "ws_long128_f32_wrap": Row("igemm<128,4,1,wsplit>", (16, 24, 48), 128, 128, dtype="fp16", out_fp32=True, n=1,
                                wsplit=True, wrap=True),
-    "ws_long256_bf16_gelu_wrap": Row("igemm<256,2,1,wsplit>", (12, 16, 96), 64, 256, relu=2, n=1, wsplit=True, wrap=True),
+    "ws_long128_fp16_4_levels": Row("igemm<128,4,1,tma-epilogue,wsplit>", None, 64, 96, dtype="fp16", relu=2, n=1, wsplit=True,
+                                    levels=LEVELS),
+    "ws_long256_bf16_gelu_wrap": Row("igemm<256,2,1,tma-epilogue,wsplit>", (12, 16, 96), 64, 256, relu=2, n=1, wsplit=True,
+                                     wrap=True),
+    "ws_long256_fp16_relu_c248_wrap": Row("igemm<256,2,1,tma-epilogue,wsplit>", (12, 16, 95), 64, 248, dtype="fp16", relu=1,
+                                          n=1, wsplit=True, wrap=True),
+    "ws_long256_fp16_relu_up_wrap": Row("igemm<256,2,1,wsplit>", (12, 16, 96), 64, 256, dtype="fp16", relu=1, res=(7, 9, 55),
+                                        n=1, wsplit=True, wrap=True),
     # ---- halo-slab kernel: 64 -> (<= 64) channels, stride 1, full box of taps, 16-bit output, no residual
     "slab_fp16_gelu_c24_wrap": Row("slab<4x16x8,N64>", (40, 33, 17), 64, 24, dtype="fp16", relu=2, wrap=True),
     "slab_bf16_relu_y1": Row("slab<4x16x8,N64>", (5, 1, 9), 64, 48, relu=1),
@@ -87,6 +122,20 @@ ROWS = {
                                       exact=True),
     "exact_long64_fp16_f32_gelu_res": Row("igemm<64,8,1>", (6, 9, 10), 128, 64, dtype="fp16", out_fp32=True, relu=2, res="same",
                                           exact=True),
+}
+
+# Every instance nrpn_conv3d_fprop can launch (conv3d_igemm.cu:kConvInstances and the halo-slab kernel), written out so that
+# an instance without a row in ROWS fails test_rows_cover_every_instance.
+LAUNCHABLE = {
+    "slab<4x16x8,N64>",
+    "igemm<64,2,3>", "igemm<64,2,2,tma-epilogue>",
+    "igemm<64,8,1>", "igemm<64,8,1,tma-epilogue>",
+    "igemm<128,6,1>", "igemm<128,6,1,tma-epilogue>",
+    "igemm<256,4,1>", "igemm<256,4,1,tma-epilogue>",
+    "igemm<64,2,3,wsplit>", "igemm<64,2,2,tma-epilogue,wsplit>",
+    "igemm<64,6,1,wsplit>", "igemm<64,6,1,tma-epilogue,wsplit>",
+    "igemm<128,4,1,wsplit>", "igemm<128,4,1,tma-epilogue,wsplit>",
+    "igemm<256,2,1,wsplit>", "igemm<256,2,1,tma-epilogue,wsplit>",
 }
 
 
@@ -113,7 +162,7 @@ def _nan_bits(dtype, device):
 class Case:
     """The operands of one row: NaN weight / shift padding, residuals with NaN columns cout..ldr, NaN-filled outputs."""
 
-    def __init__(self, ops, row, device="cuda", y_offset=0):
+    def __init__(self, ops, row, device="cuda"):
         from nerf_rpn_b200 import packing
         self.ops, self.row = ops, row
         dt = _dtype(row)
@@ -147,7 +196,7 @@ class Case:
                 res = draw((row.n, *rdims, cout + 8), 1.0).to(dt)                                    # ldr = cout + 8
                 res[..., cout:] = float("nan")
             self.levels.append(dict(x=x, dims=dims, od=od, res=res, rdims=rdims))
-        self.y_offset = y_offset
+        self.y_offset = row.y_offset
 
     def args(self, ys):
         row = self.row
@@ -229,6 +278,10 @@ def _items_and_slots(case, variant):
     return math.ceil(voxels / 128) * (case.cpad // block_n), sms * min_blocks
 
 
+def _same_bits(a, b):
+    return all(torch.equal(x.view(INT_VIEW[x.element_size()]), y.view(INT_VIEW[y.element_size()])) for x, y in zip(a, b))
+
+
 def _report(name, variant, worst, extra=""):
     print(f"\n[conv variant] {name:34s} {variant:36s} worst err/bound {worst:.3g}{extra}")
 
@@ -240,11 +293,17 @@ def ops():
     return _ops
 
 
+def test_rows_cover_every_instance():
+    assert {row.variant for row in ROWS.values()} == LAUNCHABLE
+
+
 @pytest.mark.parametrize("name", list(ROWS))
 def test_conv_variant_row(ops, monkeypatch, name):
     row = ROWS[name]
     case = Case(ops, row)
     probe = [y for _, y in case.outputs()]
+    if row.y_offset:
+        assert probe[0].data_ptr() % 16 != 0
     variant = case.variant(probe)
     assert variant == row.variant, f"{name}: the tile rule now picks {variant}"
     items, slots = _items_and_slots(case, variant)
@@ -254,32 +313,29 @@ def test_conv_variant_row(ops, monkeypatch, name):
     worst = case.check(bufs, f"{name} [{variant}]")
     _report(name, variant, worst, f"  ({items}+ work items, {slots} resident CTAs)" if row.wrap else "")
 
-    if "tma-epilogue" in variant:                # the register epilogue performs the same fp32 operations in the same order
-        monkeypatch.setenv("NRPN_CONV_TMA_EPI", "0")
-        reg = variant.replace(",2,2,tma-epilogue", ",2,3")
-        assert case.variant(probe) == reg
-        assert all(torch.equal(a.view(torch.int16), b.view(torch.int16)) for a, b in zip(bufs, case.run())), \
-            f"{name}: {reg} differs from {variant}"
-        monkeypatch.delenv("NRPN_CONV_TMA_EPI")
+    # the register epilogue performs the same fp32 operations in the same order as the TMA store; a row that does not take the
+    # TMA store keeps its instance
+    monkeypatch.setenv("NRPN_CONV_TMA_EPI", "0")
+    reg = variant.replace(",2,2,tma-epilogue", ",2,3").replace(",tma-epilogue", "")
+    assert case.variant(probe) == reg
+    assert _same_bits(bufs, case.run()), f"{name}: {reg} differs from {variant}"
+    monkeypatch.delenv("NRPN_CONV_TMA_EPI")
     if row.narrow:                               # 64-wide tiles keep the reduction order of every output element
         monkeypatch.setenv("NRPN_CONV_NARROW", "0")
         wide = case.variant(probe)
         assert wide != variant and "igemm<64," not in wide, wide
-        assert all(torch.equal(a.view(INT_VIEW[a.element_size()]), b.view(INT_VIEW[b.element_size()]))
-                   for a, b in zip(bufs, case.run())), f"{name}: {wide} differs from {variant}"
+        assert _same_bits(bufs, case.run()), f"{name}: {wide} differs from {variant}"
         monkeypatch.delenv("NRPN_CONV_NARROW")
     if row.levels:                               # one launch over 4 levels == the 4 levels launched one at a time
         for i in range(len(row.levels)):
-            sub = case.run(levels=[i])[0]
-            assert torch.equal(sub.view(INT_VIEW[sub.element_size()]), bufs[i].view(INT_VIEW[sub.element_size()])), \
-                f"{name}: level {i} launched alone differs"
+            assert _same_bits(case.run(levels=[i]), [bufs[i]]), f"{name}: level {i} launched alone differs"
 
 
 def test_conv_rejects_misaligned_pointers(ops):
     """y must be aligned to one output pair (4 bytes for 16-bit output), shift to 8 bytes: otherwise the launch is refused before
     it starts and the variant query says so."""
     row = Row("igemm<64,2,2,tma-epilogue>", (4, 5, 6), 64, 64, k=1)
-    case = Case(ops, row, y_offset=1)                                       # a 16-bit y at a 2-byte offset
+    case = Case(ops, dataclasses.replace(row, y_offset=1))                 # a 16-bit y at a 2-byte offset
     _, y = case.outputs()[0]
     assert y.data_ptr() % 4 == 2
     assert case.variant([y]) == "invalid"
@@ -301,7 +357,7 @@ def test_conv_fp32_output_needs_only_pair_alignment(ops):
     on an aligned y bit for bit."""
     row = Row("igemm<64,8,1>", (5, 8, 8), 512, 256, out_fp32=True, relu=1, res="same", n=1)
     aligned = Case(ops, row)
-    shifted = Case(ops, row, y_offset=2)                                     # fp32 y at an 8-byte offset
+    shifted = Case(ops, dataclasses.replace(row, y_offset=2))                # fp32 y at an 8-byte offset
     _, y = shifted.outputs()[0]
     assert y.data_ptr() % 16 == 8
     assert shifted.variant([y]) == row.variant
