@@ -15,9 +15,14 @@
 //   - warps 0-7 = two consumer warpgroups (rows 0-63 / 64-127 of the tile: m64nNk16 wgmma into register accumulators,
 //     then the epilogue straight from those registers), warp 8 = TMA producer (one elect.sync lane issues the loads).  smem
 //     ring of 2-8 stages (full/empty mbarriers); a stage is released once the MMAs that read it have retired (wait_group 1),
-//     so the producer streams the next tile's operands while the consumers run the epilogue.  Persistent CTAs walk a static
-//     tile list that may span up to 4 pyramid levels sharing the same weights (the RPN head on P2..P5 is ONE launch per
-//     layer).  Prologue (barriers, tensor-map prefetch) runs ahead of griddepcontrol.wait (programmatic dependent launch).
+//     so the producer streams the next tile's operands while the consumers run the epilogue.  Persistent CTAs (grid = min(tiles,
+//     resident slots)) take tiles from a list that may span up to 4 pyramid levels sharing the same weights (the RPN head on
+//     P2..P5 is ONE launch per layer).  Tiles are handed out dynamically: CTA b starts with tile b, then its producer claims the
+//     next one from a per-launch counter (g_conv_sched) and passes each index to both consumer warpgroups through a 4-deep
+//     shared-memory ring with its own full/empty mbarriers; an index past the last tile ends the loop.  A CTA that starts late
+//     (its SM still busy with other streams' kernels) or runs slow thus does fewer tiles instead of setting the layer's end.
+//     Every tile runs all its k-blocks in the same order on whichever CTA claims it: results do not depend on the schedule.
+//     Prologue (barriers, tensor-map prefetch) runs ahead of griddepcontrol.wait (programmatic dependent launch, every launch).
 //   - epilogue (fused): + shift (bias / folded BN), + residual (same shape, or nearest-upsampled coarser level for the FPN
 //     top-down path), ReLU / GELU, convert to bf16 / fp16 / fp32.  TMA_EPI variants (16-bit output) stage the tile in shared
 //     memory as 128 x 64 sub-tiles and store each with cp.async.bulk.tensor; the short reductions also prefetch a same-shape
@@ -25,6 +30,7 @@
 //   - instances (kConvInstances, which also holds the names nrpn_conv3d_variant reports): <256,4,1> <128,6,1> <64,8,1> (long
 //     reductions, each with and without TMA_EPI; <64,8,1> also for layers with fewer tiles than SMs), <64,2,3> /
 //     <64,2,2,TMA_EPI> (reductions of at most 8 k-blocks); with WS the long ones are <256,2,1> <128,4,1> <64,6,1>.
+#include <atomic>
 #include <cstdlib>
 #include <type_traits>
 #include "common.cuh"
@@ -56,6 +62,7 @@ struct ConvLevelDev {
 struct ConvDev {
     int n_levels, n_taps, kc_blocks, n_tiles_n, cout, relu, out_fp32, fp16;
     int total_m_tiles;
+    int sched_slot;          // g_conv_sched pair of this launch
     signed char tap[NRPN_CONV_MAX_TAPS][4];
     const float* shift;
     ConvLevelDev lv[NRPN_CONV_MAX_LEVELS];
@@ -69,6 +76,15 @@ struct ConvMaps {
 };
 
 constexpr int kEpiTileBytes = kBlockM * 64 * 2;      // one 128 x 64 bf16 tile (residual in / output out of the TMA epilogue)
+constexpr int kTileRing = 4;                         // tile indices handed from the producer warp to the consumers
+
+// Dynamic tile scheduler: {claim, done} counter pairs, one pair per launch in flight.  A launch takes the next pair round
+// robin (g_conv_sched_next, shared by every instance), so launches on concurrent streams use different pairs unless
+// kSchedSlots launches apart.  Every pair is zero between launches: the last CTA of a launch to stop claiming resets it
+// (conv3d_igemm_kernel).
+constexpr int kSchedSlots = 1024;
+__device__ unsigned int g_conv_sched[kSchedSlots][2];
+static std::atomic<unsigned int> g_conv_sched_next{0};
 
 // Shared-memory tiles of the TMA epilogue (see conv3d_igemm_kernel): residual prefetch ring and output staging buffers.
 // The short reductions run 2 CTAs per SM and have room for one staging buffer and a residual ring of 2 (1 with split weights);
@@ -152,12 +168,16 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
     uint64_t* empty_bar = bars + STAGES;
     uint64_t* rfull_bar = bars + 2 * STAGES;
     uint64_t* rempty_bar = bars + 2 * STAGES + 2;
+    uint64_t* tfull_bar = bars + 2 * STAGES + 4;
+    uint64_t* tempty_bar = tfull_bar + kTileRing;
+    int* tile_ring = reinterpret_cast<int*>(tempty_bar + kTileRing);
 
     const int warp = threadIdx.x >> 5;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 2); }   // one arrival per consumer warpgroup
         for (int a = 0; a < 2; ++a) { ptx::mbar_init(&rfull_bar[a], 1); ptx::mbar_init(&rempty_bar[a], 1); }
+        for (int s = 0; s < kTileRing; ++s) { ptx::mbar_init(&tfull_bar[s], 1); ptx::mbar_init(&tempty_bar[s], kConsumerThreads); }
         ptx::fence_barrier_init();
         for (int l = 0; l < P.n_levels; ++l) ptx::prefetch_tmap(&maps.x[l]);
         if (TMA_EPI) for (int l = 0; l < P.n_levels; ++l) ptx::prefetch_tmap(&maps.y[l]);
@@ -174,9 +194,18 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
     if (warp == kConsumerThreads / 32) {
         // ------------------------------------------------------------------ TMA producer (whole warp walks, one elected lane issues)
         const bool leader = ptx::elect_one();
+        const int leader_lane = __ffs(__ballot_sync(0xffffffffu, leader)) - 1;
+        unsigned int* sched = g_conv_sched[P.sched_slot];
         int stage = 0; uint32_t phase = 0;
         int rslot = 0; uint32_t rphase = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        int tslot = 0; uint32_t tphase = 0;
+        for (int tile = blockIdx.x;;) {
+            // hand the tile to the consumers; total_tiles (past the last tile) ends their loop
+            ptx::mbar_wait(&tempty_bar[tslot], tphase ^ 1u);
+            if (leader) { tile_ring[tslot] = tile; ptx::mbar_arrive(&tfull_bar[tslot]); }
+            __syncwarp();
+            if (++tslot == kTileRing) { tslot = 0; tphase ^= 1u; }
+            if (tile >= total_tiles) break;
             const int n_tile = tile % P.n_tiles_n, m_tile = tile / P.n_tiles_n;
             const TilePos tp = tile_pos(P, m_tile);
             const ConvLevelDev& L = P.lv[tp.l];
@@ -204,6 +233,17 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
                 __syncwarp();
                 if (++rslot == RES_SLOTS) { rslot = 0; rphase ^= 1u; }
             }
+            // Claim the next tile once this one's loads are issued: a CTA that started late, or shares its SM with other
+            // work, simply claims fewer tiles.  A launch with one tile per CTA claims nothing.
+            int next = total_tiles;
+            if (leader && (int)gridDim.x < total_tiles) next = (int)gridDim.x + (int)atomicAdd(&sched[0], 1u);
+            tile = __shfl_sync(0xffffffffu, next, leader_lane);
+        }
+        // The claim that came back past the last tile was this CTA's last: once every CTA has made it, the last one to
+        // count itself done zeroes the pair for the next launch that takes it.
+        if (leader && (int)gridDim.x < total_tiles) {
+            __threadfence();
+            if (atomicAdd(&sched[1], 1u) == gridDim.x - 1) { atomicExch(&sched[0], 0u); atomicExch(&sched[1], 0u); }
         }
         return;
     }
@@ -212,9 +252,17 @@ __global__ void __launch_bounds__(kConvThreads, MIN_BLOCKS) conv3d_igemm_kernel(
     const int t = threadIdx.x & 127, wg = threadIdx.x >> 7;
     int stage = 0; uint32_t phase = 0;
     int rslot = 0; uint32_t rphase = 0;
+    int tslot = 0; uint32_t tphase = 0;
     uint32_t n_stores = 0;                                  // bulk stores issued so far: staging buffer n_stores % OUT_SLOTS is next
     float acc[BLOCK_N / 2];
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    auto next_tile = [&]() {                                // the producer's next tile index (total_tiles: no more)
+        ptx::mbar_wait(&tfull_bar[tslot], tphase);
+        const int tile = tile_ring[tslot];
+        ptx::mbar_arrive(&tempty_bar[tslot]);
+        if (++tslot == kTileRing) { tslot = 0; tphase ^= 1u; }
+        return tile;
+    };
+    for (int tile = next_tile(); tile < total_tiles; tile = next_tile()) {
         const int n_tile = tile % P.n_tiles_n, m_tile = tile / P.n_tiles_n;
         const TilePos tp = tile_pos(P, m_tile);
         const ConvLevelDev& L = P.lv[tp.l];
@@ -342,16 +390,20 @@ static int launch_conv(const ConvMaps& maps, const ConvDev& P, cudaStream_t st) 
     constexpr int smem = STAGES * (kABytes + BLOCK_N * kBlockK * 2 * (WS ? 2 : 1)) +
                          (epi_res_slots(MIN_BLOCKS, TMA_EPI, WS) + epi_out_slots(MIN_BLOCKS, TMA_EPI)) * kEpiTileBytes + 1024 + 256;
     static_assert((smem + 1024) * MIN_BLOCKS <= 228 * 1024, "shared memory budget");
+    static_assert((2 * STAGES + 4 + 2 * kTileRing) * 8 + kTileRing * 4 <= 256, "barriers and tile ring");
     static bool attr_set = false;
     if (!attr_set) {
         NRPN_CUDA_TRY(cudaFuncSetAttribute(conv3d_igemm_kernel<BLOCK_N, STAGES, MIN_BLOCKS, TMA_EPI, WS>,
                                            cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         attr_set = true;
     }
+    ConvDev Q = P;
+    Q.sched_slot = (int)(g_conv_sched_next.fetch_add(1u, std::memory_order_relaxed) % kSchedSlots);
     const int total_tiles = P.total_m_tiles * P.n_tiles_n;
     const int slots = num_sms() * MIN_BLOCKS;
     const int grid = total_tiles < slots ? total_tiles : slots;
-    NRPN_CUDA_TRY(launch_pdl(conv3d_igemm_kernel<BLOCK_N, STAGES, MIN_BLOCKS, TMA_EPI, WS>, dim3(grid), dim3(kConvThreads), smem, st, total_tiles <= 2 * slots, maps, P));
+    // No CTA owns a fixed tile set, so every launch may start its prologue on SMs that the previous layer's CTAs leave.
+    NRPN_CUDA_TRY(launch_pdl(conv3d_igemm_kernel<BLOCK_N, STAGES, MIN_BLOCKS, TMA_EPI, WS>, dim3(grid), dim3(kConvThreads), smem, st, true, maps, Q));
     NRPN_LAUNCH_CHECK();
     return NRPN_OK;
 }

@@ -44,8 +44,9 @@ inline int encode_tmap(CUtensorMap* map, const void* base, const cuuint64_t (&di
 
 // Launch with programmatic stream serialization (the kernel must call ptx::pdl_wait() before reading its inputs): the
 // prologue of layer i+1 (barrier init, tensor-map prefetch) overlaps the tail of layer i, also inside a captured CUDA graph.
-// NRPN_PDL=0 falls back to ordinary stream-ordered launches.  It is applied only to latency-bound launches of at most 2 tiles
-// per SM slot (`small`); NRPN_PDL=2 forces it on for every launch.
+// NRPN_PDL=0 falls back to ordinary stream-ordered launches.  It is applied only where the caller passes `small`: every
+// implicit-GEMM launch (dynamically scheduled tiles), and latency-bound halo-slab launches of at most 2 tiles per SM; NRPN_PDL=2
+// forces it on for every launch.
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool small, Args&&... args) {
     static const int mode = [] { const char* e = getenv("NRPN_PDL"); return e ? (e[0] - '0') : 1; }();
