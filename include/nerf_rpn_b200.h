@@ -153,37 +153,30 @@ int nrpn_conv3d_fprop(const nrpn_conv_desc *desc /*host*/, nrpn_stream_t stream)
  * Bandwidth-bound helpers around the convolutions.
  * ---------------------------------------------------------------------------------------------- */
 
-/* Stem input packing: fp32 NCDHW grid (4, X, Y, Z) as the reference feeds the backbone (datasets.py:55-57,
- * nerf_rpn.py:210) -> bf16 (ceil(X/2), ceil(Y/2), ceil(Z/2)+1, 64): a 2x2x2 space-to-depth block (32 ch)
- * of voxel (i,j,k-1) followed by the block of voxel (i,j,k), k in [0, ceil(Z/2)] (so the packed Z extent is
- * ceil(Z/2)+1); turns the 7^3 stride-2 stem conv (feature_extractor.py:163) into a 4x4x2-tap stride-1
- * implicit GEMM with K = 64 per tap. */
-int nrpn_pack_stem_input(const float *grid, int n, int x, int y, int z, void *packed, int act_fp16,
-                         int channels_last /* 0: grid is (N,4,X,Y,Z); 1: (N,X,Y,Z,4) as stored on disk, datasets.py:49-57 */,
-                         nrpn_stream_t stream);
-
-/* Same, with density_to_alpha = 1 applying the reference dataset's --normalize_density map to the last channel on the device:
- * alpha = clip(1 - exp(-exp(sigma) / 100), 0, 1) (datasets.py:50-52,165-167), fused into the read of the grid. */
-int nrpn_pack_stem_input_ex(const float *grid, int n, int x, int y, int z, void *packed, int act_fp16, int channels_last,
-                            int density_to_alpha, nrpn_stream_t stream);
-
-/* Same packing from a raw uint8 grid in its on-disk order (N,X,Y,Z,4): bytes are normalised by / 255 on the device, as
- * datasets.py:59-61 does on the host (.float() / 255.0); a quarter of the fp32 host-to-device traffic. */
-int nrpn_pack_stem_input_u8(const uint8_t *grid_xyzc, int n, int x, int y, int z, void *packed, int act_fp16, nrpn_stream_t stream);
-
-/* Same packing for a batch of differently sized fp32 scenes (the reference pads a training batch to its element-wise maximum,
- * nerf_rpn.py:129-146): scene i is read through its own pointer, extent and memory order and written, in ONE launch, into slot i
- * of the packed padded batch (n, ceil(X/2), ceil(Y/2), ceil(Z/2)+1, 64), (X, Y, Z) = element-wise maximum of the extents.
- * Voxels outside a scene's extent are exactly 0 in all four channels; the padded fp32 batch is never materialised.
- * density_to_alpha = 1 maps the real voxels only: the reference's dataset maps the densities before the batch is padded. */
+/* Stem input packing: n RGB-sigma scenes (4, X_i, Y_i, Z_i) as the reference feeds the backbone (datasets.py:55-57,
+ * nerf_rpn.py:210) -> 16-bit (n, ceil(X/2), ceil(Y/2), ceil(Z/2)+1, 64), bf16 or fp16 (act_fp16), (X, Y, Z) = element-wise maximum
+ * of the extents: row (i,j,k) is the 2x2x2 space-to-depth block (32 ch) of voxel (i,j,k-1) followed by the block of voxel (i,j,k),
+ * k in [0, ceil(Z/2)] (so the packed Z extent is ceil(Z/2)+1); turns the 7^3 stride-2 stem conv (feature_extractor.py:163) into a
+ * 4x4x2-tap stride-1 implicit GEMM with K = 64 per tap.
+ * Scene i is read in place through its own pointer, extent and layout and written into slot i.  A stacked batch is n scenes of one
+ * extent; differently sized scenes give the padded batch the reference builds for training (nerf_rpn.py:129-146): voxels outside a
+ * scene's extent are exactly 0 in all four channels, and the padded input is never materialised.
+ * density_to_alpha = 1 applies the reference dataset's --normalize_density map to the last channel of the real voxels, fused into
+ * the read: alpha = clip(1 - exp(-exp(sigma) / 100), 0, 1) (datasets.py:50-52,165-167; the dataset maps the densities before the
+ * batch is padded).  It is refused (NRPN_ERR_INVALID) when any scene is uint8.
+ * One launch per NRPN_STEM_MAX_SCENES scenes. */
 #define NRPN_STEM_MAX_SCENES 32
+#define NRPN_STEM_F32_NCDHW 0 /* fp32, contiguous (4,x,y,z) */
+#define NRPN_STEM_F32_XYZC 1  /* fp32, the (4,x,y,z) view of a contiguous (x,y,z,4) array as stored on disk (datasets.py:49-57); 16-byte aligned */
+#define NRPN_STEM_U8_XYZC 2   /* raw uint8 in the same on-disk order, 4-byte aligned; normalised by / 255 on the device as datasets.py:59-61
+                               * does on the host (.float() / 255.0): a quarter of the fp32 host-to-device traffic */
 typedef struct {
-    const float *grid;        /* device, fp32; 16-byte aligned when channels_last */
+    const void *grid;         /* device */
     int32_t x, y, z;          /* extent of this scene */
-    int32_t channels_last;    /* 0: contiguous (4,x,y,z); 1: the (4,x,y,z) view of a contiguous (x,y,z,4) array, datasets.py:55-56 */
+    int32_t layout;           /* NRPN_STEM_F32_NCDHW, NRPN_STEM_F32_XYZC or NRPN_STEM_U8_XYZC */
 } nrpn_stem_src;
-int nrpn_pack_stem_input_batch(const nrpn_stem_src *src /*host, n entries*/, int n, void *packed, int act_fp16, int density_to_alpha,
-                               nrpn_stream_t stream);
+int nrpn_pack_stem_input(const nrpn_stem_src *src /*host, n entries*/, int n, void *packed, int act_fp16, int density_to_alpha,
+                         nrpn_stream_t stream);
 
 /* F.max_pool3d(kernel 3, stride 2, padding 1) on (N,X,Y,Z,C) bf16, C % 8 == 0 (feature_extractor.py:219). */
 int nrpn_maxpool3d_k3s2(const void *in, int n, int x, int y, int z, int c, void *out, int act_fp16, nrpn_stream_t stream);

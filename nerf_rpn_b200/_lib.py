@@ -59,11 +59,12 @@ class WgradDesc(ctypes.Structure):
 
 
 class StemSrc(ctypes.Structure):
-    """nrpn_stem_src: one scene of a ragged batch for nrpn_pack_stem_input_batch."""
-    _fields_ = [("grid", ctypes.c_void_p), ("x", ctypes.c_int32), ("y", ctypes.c_int32), ("z", ctypes.c_int32), ("channels_last", ctypes.c_int32)]
+    """nrpn_stem_src: one scene for nrpn_pack_stem_input, with its layout (STEM_F32_NCDHW, STEM_F32_XYZC or STEM_U8_XYZC)."""
+    _fields_ = [("grid", ctypes.c_void_p), ("x", ctypes.c_int32), ("y", ctypes.c_int32), ("z", ctypes.c_int32), ("layout", ctypes.c_int32)]
 
 
 STEM_MAX_SCENES = 32
+STEM_F32_NCDHW, STEM_F32_XYZC, STEM_U8_XYZC = 0, 1, 2
 
 
 class GnLevel(ctypes.Structure):
@@ -126,13 +127,7 @@ _SIGNATURES = {
     "nrpn_bias_grad": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_long, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, ctypes.c_void_p,
                                       ctypes.c_size_t, c_stream]),
     "nrpn_relu_backward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, c_stream]),
-    "nrpn_pack_stem_input": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                            ctypes.c_void_p, ctypes.c_int, ctypes.c_int, c_stream]),
-    "nrpn_pack_stem_input_ex": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                               ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_stream]),
-    "nrpn_pack_stem_input_u8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                               ctypes.c_void_p, ctypes.c_int, c_stream]),
-    "nrpn_pack_stem_input_batch": (ctypes.c_int, [ctypes.POINTER(StemSrc), ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, c_stream]),
+    "nrpn_pack_stem_input": (ctypes.c_int, [ctypes.POINTER(StemSrc), ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, c_stream]),
     "nrpn_maxpool3d_k3s2": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                            ctypes.c_int, ctypes.c_void_p, ctypes.c_int, c_stream]),
     "nrpn_maxpool3d_k2s2_ceil": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,

@@ -16,17 +16,17 @@ __device__ __forceinline__ float density_to_alpha(float sigma) {
     return fminf(fmaxf(a, 0.0f), 1.0f);
 }
 
-// Per-chunk pieces shared by the fp32 stem packing kernels.
-// stem_chunk: coordinates of 16-byte chunk t of the packed (n, X2, Y2, Z2+1, 64) output -- scene b, first voxel (x, y, z) of the
-// chunk's z pair, and its space-to-depth block index kk along z (-1 / Z2 for the zero rows at either end).
-struct StemChunk { int b, x, y, z, kk; };
-__device__ __forceinline__ StemChunk stem_chunk(size_t t, int X2, int Y2, int Z2) {
+// Per-chunk pieces of the stem packing.
+// stem_chunk: coordinates of 16-byte chunk t of one scene's packed (X2, Y2, Z2+1, 64) rows -- first voxel (x, y, z) of the chunk's
+// z pair, and its space-to-depth block index kk along z (-1 / Z2 for the zero rows at either end).
+struct StemChunk { int x, y, z, kk; };
+__device__ __forceinline__ StemChunk stem_chunk(size_t t, int Y2, int Z2) {
     StemChunk q;
     const int s = (int)(t & 7);
     size_t v = t >> 3;
     const int k = (int)(v % (Z2 + 1)); v /= (Z2 + 1);
-    const int j = (int)(v % Y2); v /= Y2;
-    const int i = (int)(v % X2); q.b = (int)(v / X2);
+    const int j = (int)(v % Y2);
+    const int i = (int)(v / Y2);
     const int half = s >> 2, rx = (s >> 1) & 1, ry = s & 1;
     q.kk = k - 1 + half;                            // s2d block index along z
     q.x = 2 * i + rx; q.y = 2 * j + ry; q.z = 2 * q.kk;
@@ -51,95 +51,52 @@ __device__ __forceinline__ void stem_load_cl(const float4* __restrict__ p, bool 
     if (alpha) { a.w = density_to_alpha(a.w); if (second) c.w = density_to_alpha(c.w); }
 }
 
+// Same pair from a raw uint8 scene in its on-disk (X,Y,Z,4) order: one 32-bit load per voxel, each byte normalised with the
+// correctly rounded fp32 x / 255 that datasets.py:59-61 performs on the host (.float() / 255.0).  No density_to_alpha: uint8 grids
+// hold alphas already.
+__device__ __forceinline__ void stem_load_u8(const uint32_t* __restrict__ p, bool second, float4& a, float4& c) {
+    auto f = [](uint32_t w, int byte) { return __fdiv_rn((float)((w >> (8 * byte)) & 0xFFu), 255.0f); };
+    const uint32_t w0 = __ldg(p), w1 = second ? __ldg(p + 1) : 0u;
+    a = make_float4(f(w0, 0), f(w0, 1), f(w0, 2), f(w0, 3));
+    c = make_float4(f(w1, 0), f(w1, 1), f(w1, 2), f(w1, 3));
+}
+
 __device__ __forceinline__ void stem_store(__nv_bfloat16* __restrict__ out, size_t t, float4 a, float4 c, int fp16) {
     const uint32_t h0 = pack_act2(a.x, a.y, fp16), h1 = pack_act2(a.z, a.w, fp16);
     const uint32_t h2 = pack_act2(c.x, c.y, fp16), h3 = pack_act2(c.z, c.w, fp16);
     *reinterpret_cast<uint4*>(out + (t << 3)) = make_uint4(h0, h1, h2, h3);
 }
 
-__global__ void pack_stem_kernel(const float* __restrict__ grid, int n, int X, int Y, int Z, int X2, int Y2, int Z2,
-                                 __nv_bfloat16* __restrict__ out, int fp16, int alpha) {
-    const size_t total = (size_t)n * X2 * Y2 * (Z2 + 1) * 8;
-    const size_t plane = (size_t)X * Y * Z;
-    for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
-        const StemChunk q = stem_chunk(t, X2, Y2, Z2);
-        float val[8];                                   // order: rz major, c minor
-#pragma unroll
-        for (int e = 0; e < 8; ++e) val[e] = 0.f;
-        if (q.kk >= 0 && q.kk < Z2 && q.x < X && q.y < Y)
-            stem_load_ncdhw(grid + (size_t)q.b * 4 * plane + ((size_t)q.x * Y + q.y) * Z + q.z, plane, q.z + 1 < Z, alpha, val);
-        stem_store(out, t, make_float4(val[0], val[1], val[2], val[3]), make_float4(val[4], val[5], val[6], val[7]), fp16);
-    }
-}
-
-// Same packing from the grid as it is stored on disk and handed over by the reference's dataset (datasets.py:49-57: a
-// (4,W,L,H) VIEW of the (W,L,H,4) array): one 128-bit load per voxel instead of four scalar loads from four channel planes.
-__global__ void pack_stem_cl_kernel(const float4* __restrict__ grid, int n, int X, int Y, int Z, int X2, int Y2, int Z2,
-                                    __nv_bfloat16* __restrict__ out, int fp16, int alpha) {
-    const size_t total = (size_t)n * X2 * Y2 * (Z2 + 1) * 8;
-    for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
-        const StemChunk q = stem_chunk(t, X2, Y2, Z2);
-        float4 a = make_float4(0.f, 0.f, 0.f, 0.f), c = a;
-        if (q.kk >= 0 && q.kk < Z2 && q.x < X && q.y < Y)
-            stem_load_cl(grid + (((size_t)q.b * X + q.x) * Y + q.y) * Z + q.z, q.z + 1 < Z, alpha, a, c);
-        stem_store(out, t, a, c, fp16);
-    }
-}
-
-// A batch of differently sized scenes packed into the stem input of the batch padded to the element-wise maximum extent
-// (X2, Y2, Z2 of that maximum): each chunk reads its scene's own pointer, extent and memory order; a voxel outside the scene is
-// the reference's zero padding (nerf_rpn.py:140-146) in all four channels -- density_to_alpha is applied to real voxels only.
+// The stem input of gridDim.y scenes padded to the element-wise maximum extent (X2, Y2, Z2 of that maximum): block row b packs
+// scene b through its own pointer, extent and layout; a voxel outside the scene is the reference's zero padding
+// (nerf_rpn.py:140-146) in all four channels -- density_to_alpha is applied to real voxels only.  A stacked batch is the case
+// where every extent is the same.
 struct StemBatch { nrpn_stem_src src[NRPN_STEM_MAX_SCENES]; };
 
-__global__ void pack_stem_batch_kernel(const __grid_constant__ StemBatch B, int n, int X2, int Y2, int Z2, __nv_bfloat16* __restrict__ out,
-                                       int fp16, int alpha) {
-    const size_t total = (size_t)n * X2 * Y2 * (Z2 + 1) * 8;
-    for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
-        const StemChunk q = stem_chunk(t, X2, Y2, Z2);
-        const nrpn_stem_src& S = B.src[q.b];
+__global__ void pack_stem_kernel(const __grid_constant__ StemBatch B, int X2, int Y2, int Z2, __nv_bfloat16* __restrict__ out, int fp16,
+                                 int alpha) {
+    const nrpn_stem_src S = B.src[blockIdx.y];         // a copy: the scene's fields sit in uniform registers, read once per block
+    const size_t chunks = (size_t)X2 * Y2 * (Z2 + 1) * 8;
+    out += blockIdx.y * chunks * 8;
+    for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < chunks; t += (size_t)gridDim.x * blockDim.x) {
+        const StemChunk q = stem_chunk(t, Y2, Z2);
         float4 a = make_float4(0.f, 0.f, 0.f, 0.f), c = a;
         if (q.kk >= 0 && q.z < S.z && q.x < S.x && q.y < S.y) {
             const size_t vox = ((size_t)q.x * S.y + q.y) * S.z + q.z;
             const bool second = q.z + 1 < S.z;
-            if (S.channels_last) {
-                stem_load_cl(reinterpret_cast<const float4*>(S.grid) + vox, second, alpha, a, c);
+            if (S.layout == NRPN_STEM_F32_XYZC) {
+                stem_load_cl(static_cast<const float4*>(S.grid) + vox, second, alpha, a, c);
+            } else if (S.layout == NRPN_STEM_U8_XYZC) {
+                stem_load_u8(static_cast<const uint32_t*>(S.grid) + vox, second, a, c);
             } else {
                 float val[8];
 #pragma unroll
                 for (int e = 0; e < 8; ++e) val[e] = 0.f;
-                stem_load_ncdhw(S.grid + vox, (size_t)S.x * S.y * S.z, second, alpha, val);
+                stem_load_ncdhw(static_cast<const float*>(S.grid) + vox, (size_t)S.x * S.y * S.z, second, alpha, val);
                 a = make_float4(val[0], val[1], val[2], val[3]); c = make_float4(val[4], val[5], val[6], val[7]);
             }
         }
         stem_store(out, t, a, c, fp16);
-    }
-}
-
-// uint8 grids (datasets.py:59-61 normalises them with .float() / 255.0 on the host): the raw (N,X,Y,Z,4) bytes are copied to the
-// device (a quarter of the fp32 H2D traffic) and normalised here, one 32-bit load per voxel; the division is the same correctly
-// rounded fp32 x / 255 the reference performs.
-__global__ void pack_stem_cl_u8_kernel(const uint32_t* __restrict__ grid, int n, int X, int Y, int Z, int X2, int Y2, int Z2,
-                                       __nv_bfloat16* __restrict__ out, int fp16) {
-    const size_t total = (size_t)n * X2 * Y2 * (Z2 + 1) * 8;
-    for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
-        const int s = (int)(t & 7);
-        size_t v = t >> 3;
-        const int k = (int)(v % (Z2 + 1)); v /= (Z2 + 1);
-        const int j = (int)(v % Y2); v /= Y2;
-        const int i = (int)(v % X2); const int b = (int)(v / X2);
-        const int half = s >> 2, rx = (s >> 1) & 1, ry = s & 1;
-        const int kk = k - 1 + half;
-        const int x = 2 * i + rx, y = 2 * j + ry, z = 2 * kk;
-        uint32_t a = 0u, c = 0u;
-        if (kk >= 0 && kk < Z2 && x < X && y < Y) {
-            const uint32_t* p = grid + (((size_t)b * X + x) * Y + y) * Z + z;
-            a = __ldg(p);
-            if (z + 1 < Z) c = __ldg(p + 1);
-        }
-        auto f = [](uint32_t w, int byte) { return __fdiv_rn((float)((w >> (8 * byte)) & 0xFFu), 255.0f); };
-        const uint32_t h0 = pack_act2(f(a, 0), f(a, 1), fp16), h1 = pack_act2(f(a, 2), f(a, 3), fp16);
-        const uint32_t h2 = pack_act2(f(c, 0), f(c, 1), fp16), h3 = pack_act2(f(c, 2), f(c, 3), fp16);
-        *reinterpret_cast<uint4*>(out + (t << 3)) = make_uint4(h0, h1, h2, h3);
     }
 }
 
@@ -267,56 +224,33 @@ using namespace nrpn;
 extern "C" {
 #pragma GCC visibility push(default)
 
-int nrpn_pack_stem_input_ex(const float* grid, int n, int x, int y, int z, void* packed, int act_fp16, int channels_last, int density_to_alpha,
-                            nrpn_stream_t stream) {
-    const int alpha = density_to_alpha ? 1 : 0;
-    if (!grid || !packed || n < 1 || x < 1 || y < 1 || z < 1) return NRPN_ERR_INVALID;
-    const int X2 = (x + 1) / 2, Y2 = (y + 1) / 2, Z2 = (z + 1) / 2;
-    const size_t total = (size_t)n * X2 * Y2 * (Z2 + 1) * 8;
-    if (channels_last) {
-        if (reinterpret_cast<uintptr_t>(grid) % 16 != 0) return NRPN_ERR_INVALID;
-        pack_stem_cl_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float4*>(grid), n, x, y, z, X2, Y2, Z2,
-                                                                                   reinterpret_cast<__nv_bfloat16*>(packed), act_fp16 ? 1 : 0, alpha);
-        NRPN_LAUNCH_CHECK();
-        return NRPN_OK;
-    }
-    pack_stem_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(grid, n, x, y, z, X2, Y2, Z2,
-                                                                            reinterpret_cast<__nv_bfloat16*>(packed), act_fp16 ? 1 : 0, alpha);
-    NRPN_LAUNCH_CHECK();
-    return NRPN_OK;
-}
-
-int nrpn_pack_stem_input(const float* grid, int n, int x, int y, int z, void* packed, int act_fp16, int channels_last, nrpn_stream_t stream) {
-    return nrpn_pack_stem_input_ex(grid, n, x, y, z, packed, act_fp16, channels_last, 0, stream);
-}
-
-int nrpn_pack_stem_input_u8(const uint8_t* grid, int n, int x, int y, int z, void* packed, int act_fp16, nrpn_stream_t stream) {
-    if (!grid || !packed || n < 1 || x < 1 || y < 1 || z < 1) return NRPN_ERR_INVALID;
-    if (reinterpret_cast<uintptr_t>(grid) % 4 != 0) return NRPN_ERR_INVALID;
-    const int X2 = (x + 1) / 2, Y2 = (y + 1) / 2, Z2 = (z + 1) / 2;
-    const size_t total = (size_t)n * X2 * Y2 * (Z2 + 1) * 8;
-    pack_stem_cl_u8_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const uint32_t*>(grid), n, x, y, z, X2, Y2, Z2,
-                                                                                  reinterpret_cast<__nv_bfloat16*>(packed), act_fp16 ? 1 : 0);
-    NRPN_LAUNCH_CHECK();
-    return NRPN_OK;
-}
-
-int nrpn_pack_stem_input_batch(const nrpn_stem_src* src, int n, void* packed, int act_fp16, int density_to_alpha, nrpn_stream_t stream) {
-    if (!src || !packed || n < 1 || n > NRPN_STEM_MAX_SCENES) return NRPN_ERR_INVALID;
-    StemBatch B;
+int nrpn_pack_stem_input(const nrpn_stem_src* src, int n, void* packed, int act_fp16, int density_to_alpha, nrpn_stream_t stream) {
+    if (!src || !packed || n < 1) return NRPN_ERR_INVALID;
     int x = 0, y = 0, z = 0;
     for (int i = 0; i < n; ++i) {
         const nrpn_stem_src& S = src[i];
         if (!S.grid || S.x < 1 || S.y < 1 || S.z < 1) return NRPN_ERR_INVALID;
-        if (S.channels_last && reinterpret_cast<uintptr_t>(S.grid) % 16 != 0) return NRPN_ERR_INVALID;
-        B.src[i] = S;
+        const uintptr_t addr = reinterpret_cast<uintptr_t>(S.grid);
+        switch (S.layout) {
+            case NRPN_STEM_F32_NCDHW: break;
+            case NRPN_STEM_F32_XYZC: if (addr % 16 != 0) return NRPN_ERR_INVALID; break;
+            case NRPN_STEM_U8_XYZC: if (addr % 4 != 0 || density_to_alpha) return NRPN_ERR_INVALID; break;
+            default: return NRPN_ERR_INVALID;
+        }
         x = S.x > x ? S.x : x; y = S.y > y ? S.y : y; z = S.z > z ? S.z : z;
     }
     const int X2 = (x + 1) / 2, Y2 = (y + 1) / 2, Z2 = (z + 1) / 2;
-    const size_t total = (size_t)n * X2 * Y2 * (Z2 + 1) * 8;
-    pack_stem_batch_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(B, n, X2, Y2, Z2, reinterpret_cast<__nv_bfloat16*>(packed),
-                                                                                  act_fp16 ? 1 : 0, density_to_alpha ? 1 : 0);
-    NRPN_LAUNCH_CHECK();
+    const size_t chunks_per_scene = (size_t)X2 * Y2 * (Z2 + 1) * 8;
+    // one launch per NRPN_STEM_MAX_SCENES scenes (the size of the kernel's parameter table), each writing its slice of the padded batch
+    for (int i0 = 0; i0 < n; i0 += NRPN_STEM_MAX_SCENES) {
+        const int m = n - i0 < NRPN_STEM_MAX_SCENES ? n - i0 : NRPN_STEM_MAX_SCENES;
+        StemBatch B;
+        for (int i = 0; i < m; ++i) B.src[i] = src[i0 + i];
+        const dim3 grid((grid_for(m * chunks_per_scene, 256) + m - 1) / m, m);
+        pack_stem_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(B, X2, Y2, Z2, reinterpret_cast<__nv_bfloat16*>(packed) + i0 * chunks_per_scene * 8,
+                                                                 act_fp16 ? 1 : 0, density_to_alpha ? 1 : 0);
+        NRPN_LAUNCH_CHECK();
+    }
     return NRPN_OK;
 }
 

@@ -211,8 +211,9 @@ def _act16(t: torch.Tensor, name: str) -> int:
 
 
 def is_channels_last_grid(grid: torch.Tensor) -> bool:
-    """True for an (N,4,X,Y,Z) tensor whose memory is (N,X,Y,Z,4): what datasets.py:55-56 produces (np.transpose view)."""
-    return grid.dim() == 5 and not grid.is_contiguous() and grid.permute(0, 2, 3, 4, 1).is_contiguous()
+    """True for an (N,4,X,Y,Z) batch whose memory is (N,X,Y,Z,4), or a (4,X,Y,Z) scene whose memory is (X,Y,Z,4): what datasets.py:55-56
+    produces (np.transpose view)."""
+    return grid.dim() in (4, 5) and not grid.is_contiguous() and grid.movedim(-4, -1).is_contiguous()
 
 
 def wgrad_desc(dys: Sequence[torch.Tensor], xs: Sequence[torch.Tensor], taps: Sequence[Sequence[int]], cout: int, cin: int,
@@ -279,33 +280,28 @@ def relu_backward_(dy: torch.Tensor, act: torch.Tensor) -> torch.Tensor:
     return dy
 
 
-def pack_stem_input(grid: torch.Tensor, out: Optional[torch.Tensor] = None, dtype=torch.bfloat16, density_to_alpha: bool = False) -> torch.Tensor:
-    """(N,4,X,Y,Z) fp32 -> (N, ceil(X/2), ceil(Y/2), ceil(Z/2)+1, 64) bf16 (or fp16: dtype of `out`).
-    `grid` may be contiguous NCDHW or the channels-last view the reference's dataset yields (memory (N,X,Y,Z,4))."""
-    if isinstance(grid, torch.Tensor) and grid.is_cuda and grid.dtype == torch.uint8 and grid.dim() == 5:
-        # raw uint8 grid in its on-disk order: normalised (/ 255) on the device
-        if not is_channels_last_grid(grid):
+def _stem_layout(g, stacked: bool, copy_ok: bool = False) -> Optional[int]:
+    """The nrpn_stem_src layout in which the stem packing reads `g` in place: a stacked (N,4,X,Y,Z) batch (fp32, or the raw uint8 on-disk
+    view) or one (4,X,Y,Z) fp32 scene of a list.  Raises for any other input, except that an fp32 tensor in neither memory order gives None
+    when `copy_ok` (the caller packs a contiguous copy of it instead)."""
+    if stacked:
+        if not isinstance(g, torch.Tensor) or not g.is_cuda or g.dtype not in (torch.float32, torch.uint8) or g.dim() != 5:
+            raise RuntimeError("nerf_rpn_b200: grid must be a 5-D fp32 (or channels-last uint8) CUDA tensor")
+        if g.shape[1] != 4:
+            raise ValueError("stem packing expects 4 input channels (RGB + density)")
+    elif not isinstance(g, torch.Tensor) or not g.is_cuda or g.dtype != torch.float32 or g.dim() != 4 or g.shape[0] != 4:
+        raise RuntimeError("nerf_rpn_b200: every scene must be a (4,X,Y,Z) fp32 CUDA tensor")
+    cl = is_channels_last_grid(g)
+    if g.dtype == torch.uint8:
+        if not cl:
             raise ValueError("nerf_rpn_b200: uint8 grids must be the (N,4,X,Y,Z) view of a contiguous (N,X,Y,Z,4) array")
-        n, c, x, y, z = grid.shape
-        shape = (n, (x + 1) // 2, (y + 1) // 2, (z + 1) // 2 + 1, 64)
-        if out is None:
-            out = torch.empty(shape, dtype=dtype, device=grid.device)
-        check(lib().nrpn_pack_stem_input_u8(_ptr(grid), n, x, y, z, _ptr(out), _act16(out, "out"), _stream()), "pack_stem_input_u8")
-        return out
-    if not isinstance(grid, torch.Tensor) or not grid.is_cuda or grid.dtype != torch.float32 or grid.dim() != 5:
-        raise RuntimeError("nerf_rpn_b200: grid must be a 5-D fp32 (or channels-last uint8) CUDA tensor")
-    cl = is_channels_last_grid(grid)
-    if not cl and not grid.is_contiguous():
-        raise ValueError("nerf_rpn_b200: grid must be contiguous (N,4,X,Y,Z) or a permuted view of a contiguous (N,X,Y,Z,4) array")
-    n, c, x, y, z = grid.shape
-    if c != 4:
-        raise ValueError("stem packing expects 4 input channels (RGB + density)")
-    shape = (n, (x + 1) // 2, (y + 1) // 2, (z + 1) // 2 + 1, 64)
-    if out is None:
-        out = torch.empty(shape, dtype=dtype, device=grid.device)
-    check(lib().nrpn_pack_stem_input_ex(_ptr(grid), n, x, y, z, _ptr(out), _act16(out, "out"), int(cl), int(bool(density_to_alpha)), _stream()),
-          "pack_stem_input")
-    return out
+        return _lib.STEM_U8_XYZC
+    if cl or g.is_contiguous():
+        return _lib.STEM_F32_XYZC if cl else _lib.STEM_F32_NCDHW
+    if copy_ok:
+        return None
+    raise ValueError("nerf_rpn_b200: grid must be contiguous (N,4,X,Y,Z) or a permuted view of a contiguous (N,X,Y,Z,4) array" if stacked else
+                     "nerf_rpn_b200: a scene must be contiguous (4,X,Y,Z) or a permuted view of a contiguous (X,Y,Z,4) array")
 
 
 def padded_extent(grids: Sequence[torch.Tensor]):
@@ -313,30 +309,33 @@ def padded_extent(grids: Sequence[torch.Tensor]):
     return tuple(max(int(g.shape[-3 + a]) for g in grids) for a in range(3))
 
 
-def pack_stem_input_batch(grids: Sequence[torch.Tensor], out: Optional[torch.Tensor] = None, dtype=torch.bfloat16,
-                          density_to_alpha: bool = False) -> torch.Tensor:
-    """A list of differently sized (4,X_i,Y_i,Z_i) fp32 scenes -> the packed stem input of the batch zero-padded to the element-wise maximum
-    extent, (N, ceil(X/2), ceil(Y/2), ceil(Z/2)+1, 64), in one launch; the padded fp32 batch is never materialised.  Each scene is
-    contiguous NCDHW or the channels-last view the reference's dataset yields; density_to_alpha maps the real voxels only."""
-    n = len(grids)
-    if n < 1 or n > _lib.STEM_MAX_SCENES:
-        raise ValueError(f"pack_stem_input_batch: 1 to {_lib.STEM_MAX_SCENES} scenes, got {n}")
+def pack_stem_input(grids, out: Optional[torch.Tensor] = None, dtype=torch.bfloat16, density_to_alpha: bool = False) -> torch.Tensor:
+    """A stacked (N,4,X,Y,Z) grid or a list of N differently sized (4,X_i,Y_i,Z_i) scenes -> the packed stem input of the batch zero-padded
+    to the element-wise maximum extent, (N, ceil(X/2), ceil(Y/2), ceil(Z/2)+1, 64) bf16 (or fp16: dtype of `out`); the padded batch is never
+    materialised.  Every scene is read in place: fp32 contiguous NCDHW or the channels-last view the reference's dataset yields (memory
+    (X,Y,Z,4)), or, stacked only, that view of the raw uint8 grid (normalised / 255 on the device).  density_to_alpha maps the real voxels
+    of fp32 grids; uint8 grids hold alphas already and refuse it."""
+    if isinstance(grids, (list, tuple)):
+        scenes = [(g, _stem_layout(g, stacked=False)) for g in grids]
+    else:
+        layout = _stem_layout(grids, stacked=True)
+        if density_to_alpha and layout == _lib.STEM_U8_XYZC:
+            raise NotImplementedError("density_to_alpha on the device is fused into the fp32 stem packing (uint8 grids hold alphas already)")
+        scenes = [(g, layout) for g in grids.unbind(0)]
+    n = len(scenes)
+    if n < 1:
+        raise ValueError("pack_stem_input: no scenes")
     src = (_lib.StemSrc * n)()
-    for i, g in enumerate(grids):
-        if not isinstance(g, torch.Tensor) or not g.is_cuda or g.dtype != torch.float32 or g.dim() != 4 or g.shape[0] != 4:
-            raise RuntimeError("nerf_rpn_b200: every scene must be a (4,X,Y,Z) fp32 CUDA tensor")
-        cl = (not g.is_contiguous()) and g.permute(1, 2, 3, 0).is_contiguous()
-        if not cl and not g.is_contiguous():
-            raise ValueError("nerf_rpn_b200: a scene must be contiguous (4,X,Y,Z) or a permuted view of a contiguous (X,Y,Z,4) array")
-        src[i].grid, src[i].channels_last = g.data_ptr(), int(cl)
-        src[i].x, src[i].y, src[i].z = (int(v) for v in g.shape[1:])
-    x, y, z = padded_extent(grids)
+    for s, (g, layout) in zip(src, scenes):
+        s.grid, s.layout = g.data_ptr(), layout
+        s.x, s.y, s.z = (int(v) for v in g.shape[1:])
+    x, y, z = padded_extent([g for g, _ in scenes])
     shape = (n, (x + 1) // 2, (y + 1) // 2, (z + 1) // 2 + 1, 64)
     if out is None:
-        out = torch.empty(shape, dtype=dtype, device=grids[0].device)
+        out = torch.empty(shape, dtype=dtype, device=scenes[0][0].device)
     if tuple(out.shape) != shape:
-        raise ValueError(f"pack_stem_input_batch: out must be {shape}, got {tuple(out.shape)}")
-    check(lib().nrpn_pack_stem_input_batch(src, n, _ptr(out), _act16(out, "out"), int(bool(density_to_alpha)), _stream()), "pack_stem_input_batch")
+        raise ValueError(f"pack_stem_input: out must be {shape}, got {tuple(out.shape)}")
+    check(lib().nrpn_pack_stem_input(src, n, _ptr(out), _act16(out, "out"), int(bool(density_to_alpha)), _stream()), "pack_stem_input")
     return out
 
 

@@ -790,23 +790,19 @@ class _TrainPlan:
         return positive[perm1].contiguous(), negative[perm2].contiguous()
 
     def _pack_input(self):
-        if self._sizes is not None:
-            ops.pack_stem_input_batch(self._src, self.packed, density_to_alpha=self._alpha)
-        else:
-            ops.pack_stem_input(self._src, self.packed, density_to_alpha=self._alpha)
+        ops.pack_stem_input(self._src, self.packed, density_to_alpha=self._alpha)
 
     def _set_input(self, grids):
-        """The caller's batch for the stem packing: a stacked (N,4,X,Y,Z) grid, or a list of scenes whose padded extent is this plan's dims."""
+        """The caller's batch for the stem packing: a stacked (N,4,X,Y,Z) grid, or a list of scenes whose padded extent is this plan's dims.
+        An fp32 grid in neither memory order the packing reads in place is packed from a contiguous copy."""
         self._alpha = self.eng.density_to_alpha()
         if isinstance(grids, (list, tuple)):
             if len(grids) != self.n or ops.padded_extent(grids) != tuple(self.dims):
                 raise ValueError(f"nerf_rpn_b200: this plan trains {self.n} scenes padded to {self.dims}")
-            self._src = [g if (g.is_contiguous() or g.permute(1, 2, 3, 0).is_contiguous()) else g.contiguous() for g in grids]
+            self._src = [g if ops._stem_layout(g, stacked=False, copy_ok=True) is not None else g.contiguous() for g in grids]
             self._sizes = [tuple(int(v) for v in g.shape[-3:]) for g in grids]
             return
-        if self._alpha and grids.dtype == torch.uint8:
-            raise NotImplementedError("density_to_alpha on the device is fused into the fp32 stem packing (uint8 grids hold alphas already)")
-        self._src = grids if (ops.is_channels_last_grid(grids) or grids.is_contiguous()) else grids.contiguous()
+        self._src = grids if ops._stem_layout(grids, stacked=True, copy_ok=True) is not None else grids.contiguous()
         self._sizes = None
 
     def padding_masks(self):

@@ -69,17 +69,44 @@ int main(void) {
          offsetof(nrpn_rpn_desc, cell_anchors), offsetof(nrpn_rpn_desc, nms_thresh), offsetof(nrpn_rpn_desc, valid));
   printf("%zu %zu %zu %zu %zu %zu\n", sizeof(nrpn_wgrad_level), sizeof(nrpn_wgrad_desc), offsetof(nrpn_wgrad_desc, level),
          offsetof(nrpn_wgrad_desc, dw), offsetof(nrpn_wgrad_desc, workspace_bytes), offsetof(nrpn_wgrad_desc, dw_layout));
+  printf("%zu %zu %zu %d %d %d %d\n", sizeof(nrpn_stem_src), offsetof(nrpn_stem_src, x), offsetof(nrpn_stem_src, layout),
+         NRPN_STEM_MAX_SCENES, NRPN_STEM_F32_NCDHW, NRPN_STEM_F32_XYZC, NRPN_STEM_U8_XYZC);
   return 0; }'''
     with tempfile.TemporaryDirectory() as d:
         src, exe = os.path.join(d, "t.c"), os.path.join(d, "t")
         open(src, "w").write(code)
         subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), src, "-o", exe])
         vals = [int(v) for v in subprocess.check_output([exe]).split()]
-    C, R, W = _lib.ConvDesc, _lib.RpnDesc, _lib.WgradDesc
+    C, R, W, S = _lib.ConvDesc, _lib.RpnDesc, _lib.WgradDesc, _lib.StemSrc
     mine = [C.act_fp16.offset, C.wsplit.offset, ctypes.sizeof(_lib.ConvLevel), ctypes.sizeof(C), C.stride.offset, C.w.offset, C.level.offset,
             ctypes.sizeof(_lib.RpnLevel), ctypes.sizeof(R), R.cell_anchors.offset, R.nms_thresh.offset, R.valid.offset,
-            ctypes.sizeof(_lib.WgradLevel), ctypes.sizeof(W), W.level.offset, W.dw.offset, W.workspace_bytes.offset, W.dw_layout.offset]
+            ctypes.sizeof(_lib.WgradLevel), ctypes.sizeof(W), W.level.offset, W.dw.offset, W.workspace_bytes.offset, W.dw_layout.offset,
+            ctypes.sizeof(S), S.x.offset, S.layout.offset, _lib.STEM_MAX_SCENES, _lib.STEM_F32_NCDHW, _lib.STEM_F32_XYZC, _lib.STEM_U8_XYZC]
     assert mine == vals
+
+
+def test_stem_pack_validates_every_scene_before_launching():
+    """nrpn_pack_stem_input refuses a bad scene anywhere in the table (here the second) on the host: the pointers are checked, never
+    dereferenced, and nothing is launched."""
+    L = _lib.lib()
+    base = 1 << 32
+
+    def status(layout, grid=base, extent=(4, 4, 4), alpha=0):
+        src = (_lib.StemSrc * 2)()
+        src[0].grid, src[0].layout, src[0].x, src[0].y, src[0].z = base, _lib.STEM_F32_XYZC, 6, 6, 6
+        src[1].grid, src[1].layout = grid, layout
+        src[1].x, src[1].y, src[1].z = extent
+        before = L.nrpn_launch_count()
+        st = L.nrpn_pack_stem_input(src, 2, base, 0, alpha, None)
+        assert L.nrpn_launch_count() == before
+        return st
+
+    assert status(_lib.STEM_U8_XYZC, alpha=1) == -1                      # uint8 grids hold alphas already
+    assert status(_lib.STEM_U8_XYZC, grid=base + 2) == -1                # 32-bit voxel loads
+    assert status(_lib.STEM_F32_XYZC, grid=base + 4) == -1               # 128-bit voxel loads
+    assert status(3) == -1                                               # no such layout
+    assert status(_lib.STEM_F32_NCDHW, grid=0) == -1
+    assert status(_lib.STEM_F32_NCDHW, extent=(4, 0, 4)) == -1
 
 
 def test_missing_library_fails_loudly(monkeypatch):

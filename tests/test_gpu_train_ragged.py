@@ -1,9 +1,6 @@
 """GPU: training on batches of differently sized scenes (the reference pads a batch to its element-wise maximum, nerf_rpn.py:129-146, and
 labels the anchors in the padding -1, anchor.py:124-152 / rpn.py:231-238, 260-263, 283-285) and the engine's bounded plan pool.
 Reference pieces come from the staged oracle/_ref only."""
-import math
-
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
@@ -38,39 +35,6 @@ def _pad_stack(scenes, value_density=0.0):
         d = F.pad(s[3:].contiguous(), p, value=value_density)
         out.append(torch.cat([rgb, d], 0))
     return torch.stack(out, 0)
-
-
-# ------------------------------------------------------------------------------------------------ 1. stem packing
-@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-@pytest.mark.parametrize("alpha", [False, True])
-def test_ragged_stem_packing_bit_identical(dtype, alpha):
-    from nerf_rpn_b200 import ops
-    dims = [(13, 20, 9), (17, 11, 15), (7, 19, 21)]
-    scenes = [_scene(d, 10 + i, cl) for i, (d, cl) in enumerate(zip(dims, (True, False, True)))]
-    got = ops.pack_stem_input_batch(scenes, dtype=dtype, density_to_alpha=alpha)
-    if alpha:
-        # the existing kernel's fused map on a padded batch whose padding maps to exactly 0 (density -inf): the same bits.  (A map computed
-        # on the host -- torch or numpy exp -- differs from the kernel's expf in the last fp32 bit now and then, which can flip a 16-bit rounding.)
-        want = ops.pack_stem_input(_pad_stack(scenes, value_density=-math.inf), dtype=dtype, density_to_alpha=True)
-    else:
-        want = ops.pack_stem_input(_pad_stack(scenes), dtype=dtype)          # F.pad -> torch.stack -> the existing packing
-    torch.cuda.synchronize()
-    assert got.shape == want.shape == (3, 9, 10, 12, 64)
-    assert torch.equal(got.view(torch.int16), want.view(torch.int16))
-    if alpha:
-        torch_map = ops.pack_stem_input(_pad_stack([_alpha(s) for s in scenes]), dtype=dtype)
-        assert (got.float() - torch_map.float()).abs().max().item() <= (2.0 ** -10 if dtype == torch.float16 else 2.0 ** -7)
-        # numpy's map (BaseDataset.density_to_alpha on the host): within one 16-bit ulp of values in [0, 1]
-        host = []
-        for s in scenes:
-            a = s.cpu().numpy().copy()
-            a[3] = np.clip(1.0 - np.exp(-np.exp(a[3]) / 100.0), 0.0, 1.0)
-            host.append(torch.from_numpy(a).cuda())
-        ref_np = ops.pack_stem_input(_pad_stack(host), dtype=dtype)
-        assert (got.float() - ref_np.float()).abs().max().item() <= (2.0 ** -10 if dtype == torch.float16 else 2.0 ** -7)
-    # the padding is exactly zero: scene 2 (x extent 7 -> 4 packed rows of 9) has nothing beyond x row 4, scene 1 (y 11) nothing beyond y row 6
-    assert not got[2, 4:].any() and not got[1, :, 6:].any()
-    assert got[2, :4].any() and got[1, :, :6].any()
 
 
 # ------------------------------------------------------------------------------------------------ engine helpers
