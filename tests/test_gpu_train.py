@@ -1,172 +1,13 @@
-"""GPU: the training-step kernels (csrc/train.cu) against plain PyTorch fp32 autograd of the same op, and the whole
-training step (nerf_rpn_b200/train.py) against the UNMODIFIED reference's own `model(rgbsigma, boxes)` + `loss.backward()` run in fp32
-on the same GPU (oracle/_ref).  Tolerances are stated per test: 16-bit activations / gradients, fp32 accumulation."""
-import ctypes
+"""GPU: the whole training step (nerf_rpn_b200/train.py) against the UNMODIFIED reference's own `model(rgbsigma, boxes)` +
+`loss.backward()` run in fp32 on the same GPU (oracle/_ref).  Tolerances are stated per test: 16-bit activations / gradients, fp32
+accumulation.  The step's bandwidth kernels alone are checked against float64 references in tests/test_gpu_bandwidth_kernels.py."""
 import math
-import os
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
-
-
-def _p(t):
-    return ctypes.c_void_p(0 if t is None else t.data_ptr())
-
-
-def _s():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-@pytest.fixture(scope="module")
-def L():
-    from nerf_rpn_b200._lib import lib
-    return lib()
-
-
-def _ws(L, c=2048):
-    return torch.empty(L.nrpn_chan_reduce_workspace_bytes(c), dtype=torch.uint8, device="cuda")
-
-
-@pytest.mark.parametrize("c,rows,dtype", [(64, 40 * 64 * 16, torch.bfloat16), (256, 5000, torch.float16), (2048, 333, torch.bfloat16), (96, 1000, torch.float16)])
-def test_batchnorm_train_forward_backward_vs_autograd(L, c, rows, dtype):
-    """nrpn_bn_stats / nrpn_bn_apply / nrpn_bn_backward == F.batch_norm(training=True) (+ residual, ReLU) and its autograd, on the
-    same 16-bit inputs.  Outputs are 16-bit: tolerance one rounding (2^-8 bf16 / 2^-11 fp16) of the tensor's scale; statistics and
-    parameter gradients (fp32, fp64-accumulated) to 1e-4 relative."""
-    from nerf_rpn_b200._lib import check
-    g = torch.Generator(device="cuda").manual_seed(c + rows)
-    f16 = 1 if dtype == torch.float16 else 0
-    y = (torch.randn(rows, c, device="cuda", generator=g) * 1.5 + 0.3).to(dtype)
-    res = torch.randn(rows, c, device="cuda", generator=g).to(dtype)
-    gamma = torch.rand(c, device="cuda", generator=g) + 0.5
-    beta = torch.randn(c, device="cuda", generator=g) * 0.2
-    dout = (torch.randn(rows, c, device="cuda", generator=g) * 0.01).to(dtype)
-    rm, rv = torch.zeros(c, device="cuda"), torch.ones(c, device="cuda")
-    stats = torch.empty(3 * c, device="cuda")
-    out = torch.empty_like(y)
-    ws = _ws(L)
-    check(L.nrpn_bn_stats(_p(y), rows, c, f16, 1e-5, _p(stats), _p(rm), _p(rv), 0.1, _p(ws), ws.numel(), _s()), "bn_stats")
-    check(L.nrpn_bn_apply(_p(y), _p(res), _p(out), rows, c, _p(stats), _p(gamma), _p(beta), 1, f16, _s()), "bn_apply")
-    dy, dres, sums = torch.empty_like(y), torch.empty_like(y), torch.empty(2 * c, device="cuda")
-    check(L.nrpn_bn_backward(_p(dout), _p(out), _p(y), _p(dy), _p(dres), rows, c, _p(stats), _p(gamma), _p(sums), 1, f16, _p(ws), ws.numel(), _s()), "bn_backward")
-    torch.cuda.synchronize()
-    # reference
-    y32 = y.float().requires_grad_(True); r32 = res.float().requires_grad_(True)
-    g32, b32 = gamma.clone().requires_grad_(True), beta.clone().requires_grad_(True)
-    rm2, rv2 = torch.zeros(c, device="cuda"), torch.ones(c, device="cuda")
-    o32 = F.relu(F.batch_norm(y32, rm2, rv2, g32, b32, True, 0.1, 1e-5) + r32)
-    # the kernel's ReLU mask comes from ITS 16-bit output; use the same mask for the comparison (elements that round to 0 differ)
-    mask = (out.float() > 0).float()
-    (o32 * 0).sum().backward()                                            # materialise .grad fields
-    y32.grad = None; r32.grad = None; g32.grad = None; b32.grad = None
-    o_lin = F.batch_norm(y32, torch.zeros(c, device="cuda"), torch.ones(c, device="cuda"), g32, b32, True, 0.1, 1e-5) + r32
-    o_lin.backward(dout.float() * mask)
-    eps16 = 2.0 ** -8 if dtype == torch.bfloat16 else 2.0 ** -11
-    assert (out.float() - o32.detach()).abs().max().item() <= 1.5 * eps16 * o32.abs().max().item() + 1e-6
-    mean, var = y.float().mean(0), y.float().var(0, unbiased=False)
-    assert torch.allclose(stats[:c], mean, rtol=1e-4, atol=1e-5) and torch.allclose(stats[2 * c:], var, rtol=1e-4, atol=1e-6)
-    assert torch.allclose(rm, rm2, rtol=1e-4, atol=1e-6) and torch.allclose(rv, rv2, rtol=1e-4, atol=1e-6)
-    assert torch.allclose(sums[:c], g32.grad, rtol=2e-3, atol=2e-5 * rows ** 0.5), (sums[:c] - g32.grad).abs().max()
-    assert torch.allclose(sums[c:], b32.grad, rtol=2e-3, atol=2e-5 * rows ** 0.5)
-    scale = y32.grad.abs().max().item()
-    assert (dy.float() - y32.grad).abs().max().item() <= 2.5 * eps16 * scale + 1e-7, ((dy.float() - y32.grad).abs().max().item(), scale)
-    assert torch.equal(dres.float(), dout.float() * mask)
-
-
-@pytest.mark.parametrize("dims,c,dtype", [((9, 12, 10), 64, torch.bfloat16), ((16, 8, 7), 16, torch.float16)])
-def test_maxpool_argmax_and_backward_vs_autograd(L, dims, c, dtype):
-    from nerf_rpn_b200._lib import check
-    g = torch.Generator(device="cuda").manual_seed(sum(dims))
-    f16 = 1 if dtype == torch.float16 else 0
-    n = 2
-    x = torch.randn(n, *dims, c, device="cuda", generator=g).to(dtype)            # distinct values: ties are measure-zero but 16-bit makes them real
-    od = tuple((d - 1) // 2 + 1 for d in dims)
-    out = torch.empty(n, *od, c, dtype=dtype, device="cuda"); idx = torch.empty(n, *od, c, dtype=torch.uint8, device="cuda")
-    check(L.nrpn_maxpool3d_k3s2_argmax(_p(x), n, *dims, c, _p(out), _p(idx), f16, _s()), "maxpool_argmax")
-    dy = torch.randn(n, *od, c, device="cuda", generator=g).to(dtype)
-    dx = torch.empty_like(x)
-    check(L.nrpn_maxpool3d_k3s2_backward(_p(dy), _p(idx), n, *dims, c, _p(dx), f16, _s()), "maxpool_backward")
-    torch.cuda.synchronize()
-    x32 = x.float().permute(0, 4, 1, 2, 3).contiguous().requires_grad_(True)
-    o32 = F.max_pool3d(x32, 3, 2, 1)
-    assert torch.equal(out.float(), o32.detach().permute(0, 2, 3, 4, 1))
-    o32.backward(dy.float().permute(0, 4, 1, 2, 3))
-    ref = x32.grad.permute(0, 2, 3, 4, 1)
-    # torch also sends the gradient to the first maximum of each window; sums of <= 8 16-bit values rounded once at the end
-    eps16 = 2.0 ** -8 if dtype == torch.bfloat16 else 2.0 ** -11
-    assert (dx.float() - ref).abs().max().item() <= 2 * eps16 * ref.abs().max().item()
-
-
-@pytest.mark.parametrize("fine,coarse", [((13, 9, 7), (7, 5, 4)), ((40, 64, 64), (20, 32, 32)), ((25, 25, 17), (13, 13, 9))])
-def test_upsample_nearest_backward_adds_vs_autograd(L, fine, coarse):
-    from nerf_rpn_b200._lib import check
-    g = torch.Generator(device="cuda").manual_seed(sum(fine))
-    n, c = 1, 64
-    df = torch.randn(n, *fine, c, device="cuda", generator=g).to(torch.bfloat16)
-    dc = torch.randn(n, *coarse, c, device="cuda", generator=g).to(torch.bfloat16)
-    base = dc.clone()
-    check(L.nrpn_upsample_nearest_backward(_p(df), n, *fine, *coarse, c, _p(dc), 0, _s()), "upsample_backward")
-    torch.cuda.synchronize()
-    cz = torch.zeros(n, c, *coarse, device="cuda", requires_grad=True)
-    F.interpolate(cz, size=fine, mode="nearest").backward(df.float().permute(0, 4, 1, 2, 3))
-    ref = base.float() + cz.grad.permute(0, 2, 3, 4, 1)
-    assert (dc.float() - ref).abs().max().item() <= 2.0 ** -7 * ref.abs().max().item()
-
-
-def test_stride2_gather_scatter_and_add(L):
-    from nerf_rpn_b200._lib import check
-    g = torch.Generator(device="cuda").manual_seed(1)
-    n, dims, c = 2, (9, 12, 7), 128
-    x = torch.randn(n, *dims, c, device="cuda", generator=g).to(torch.bfloat16)
-    od = tuple((d + 1) // 2 for d in dims)
-    xs = torch.empty(n, *od, c, dtype=torch.bfloat16, device="cuda")
-    check(L.nrpn_stride2(_p(x), _p(xs), n, *dims, c, 0, _s()), "gather")
-    assert torch.equal(xs, x[:, ::2, ::2, ::2])
-    back = torch.full_like(x, 7.0)
-    check(L.nrpn_stride2(_p(xs), _p(back), n, *dims, c, 1, _s()), "scatter")
-    want = torch.zeros_like(x); want[:, ::2, ::2, ::2] = xs
-    assert torch.equal(back, want)
-    a = x.clone()
-    check(L.nrpn_add_inplace(_p(a), _p(back), a.numel(), 0, _s()), "add")
-    assert torch.equal(a, (x.float() + back.float()).to(torch.bfloat16))
-
-
-def test_pack_weights_matches_host_packing(L):
-    from nerf_rpn_b200 import packing
-    from nerf_rpn_b200._lib import check
-    g = torch.Generator(device="cuda").manual_seed(5)
-    for cout, cin, k in ((64, 256, 1), (256, 64, 3), (120, 256, 1)):
-        w = torch.randn(cout, cin, k, k, k, device="cuda", generator=g)
-        fwd_ref, taps = packing.pack_conv_weight(w.cpu())
-        bwd_ref, _ = packing.pack_conv_weight_dgrad(w.cpu())
-        fwd = torch.zeros(fwd_ref.shape, dtype=torch.bfloat16, device="cuda"); bwd = torch.zeros(bwd_ref.shape, dtype=torch.bfloat16, device="cuda")
-        check(L.nrpn_pack_weights(_p(w), cout, cin, k ** 3, _p(fwd), fwd.shape[1], fwd.shape[2], _p(bwd), bwd.shape[1], bwd.shape[2], 0, _s()), "pack")
-        assert torch.equal(fwd.cpu(), fwd_ref) and torch.equal(bwd.cpu(), bwd_ref)
-
-
-def test_clip_and_adamw_vs_torch(L):
-    """nrpn_grad_norm + nrpn_adamw_step == torch.nn.utils.clip_grad_norm_(0.1) + torch.optim.AdamW over 3 steps (fp32, rtol 1e-5)."""
-    from nerf_rpn_b200._lib import check
-    g = torch.Generator(device="cuda").manual_seed(9)
-    n = 1_000_003
-    p0 = torch.randn(n, device="cuda", generator=g)
-    p = p0.clone(); m = torch.zeros(n, device="cuda"); v = torch.zeros(n, device="cuda")
-    q = torch.nn.Parameter(p0.clone())
-    opt = torch.optim.AdamW([q], lr=3e-4, weight_decay=0.01)
-    norm = torch.zeros(1, device="cuda"); ws = torch.empty(L.nrpn_grad_norm_workspace_bytes(), dtype=torch.uint8, device="cuda")
-    for step in range(1, 4):
-        grad = torch.randn(n, device="cuda", generator=g) * (0.01 if step == 2 else 1e-5)      # step 2 is clipped, the others are not
-        q.grad = grad.clone()
-        tn = torch.nn.utils.clip_grad_norm_([q], 0.1)
-        opt.step()
-        check(L.nrpn_grad_norm(_p(grad), n, 1.0, _p(norm), _p(ws), ws.numel(), _s()), "norm")
-        check(L.nrpn_adamw_step(_p(p), _p(grad), _p(m), _p(v), n, _p(norm), 0.1, 1.0, 3e-4, 0.9, 0.999, 1e-8, 0.01, step, _s()), "adamw")
-        torch.cuda.synchronize()
-        assert abs(norm.item() - tn.item()) <= 1e-5 * tn.item()
-        assert torch.allclose(p, q.data, rtol=1e-5, atol=1e-7), (p - q.data).abs().max()
 
 
 def _planted(dims, n_gt, seed, rotated):
@@ -178,53 +19,6 @@ def _planted(dims, n_gt, seed, rotated):
     if rotated:
         return grid, torch.cat([ctr, size, (torch.rand(n_gt, 1, generator=g) - 0.5) * math.pi], 1)
     return grid, torch.cat([ctr - size / 2, ctr + size / 2], 1)
-
-
-def test_rpn_loss_kernel_vs_torch(L):
-    """nrpn_rpn_loss (BCE mean + smooth-L1(1/9) sum / sampled, rpn.py:394-417; encoders AABB_coder.py:14-56, midpoint_offset_coder.py:106-158)
-    against torch on the same samples; targets against oracle/loss_oracle.py; gradient against autograd."""
-    from nerf_rpn_b200 import ops
-    from nerf_rpn_b200._lib import check
-    from nerf_rpn_b200.model.anchor import AnchorGenerator3D
-    from oracle import loss_oracle as lo
-    from oracle import ref_gpu
-    ag = AnchorGenerator3D(ref_gpu.ANCHOR_SIZES, ref_gpu.ASPECT)
-    cells = ag.cell_anchors_np()
-    dims, fd = (32, 48, 40), [(8, 12, 10), (4, 6, 5), (2, 3, 3), (1, 2, 2)]
-    strides = [tuple(dims[k] // d[k] for k in range(3)) for d in fd]
-    g = torch.Generator(device="cuda").manual_seed(4)
-    for rotated in (False, True):
-        code = 8 if rotated else 6
-        preds = [torch.randn(d[0] * d[1] * d[2], 128, device="cuda", generator=g) * 0.5 for d in fd]
-        dpreds = [torch.zeros(p.shape, dtype=torch.float16, device="cuda") for p in preds]
-        feats = [torch.empty(1, 1, *d) for d in fd]
-        anchors = ag(torch.empty(1, 4, *dims), feats)[0][0].cuda()
-        _, gt = _planted(dims, 10, 3, rotated)
-        gt = gt.cuda()
-        labels, idx = ops.assign_targets(anchors, gt, None, 0.35, 0.2, True)
-        pos = torch.where(labels >= 1)[0][:100].contiguous(); neg = torch.where(labels == 0)[0][:150].contiguous()
-        gtp = gt[idx[pos]].contiguous()
-        desc = ops.make_rpn_desc(preds, fd, strides, cells, 13, rotated, 1, 1, 0.5, 0.0, 1e-3, dims)
-        losses = torch.zeros(2, device="cuda"); tout = torch.zeros(pos.numel(), code, device="cuda")
-        arr = (ctypes.c_void_p * 4)(*[t.data_ptr() for t in dpreds])
-        norm = float(pos.numel() + neg.numel())
-        check(L.nrpn_rpn_loss(ctypes.byref(desc), arr, _p(pos), pos.numel(), _p(neg), neg.numel(), _p(gtp), norm, 1.0, 5.0, 256.0, _p(losses), _p(tout), 1, _s()), "rpn_loss")
-        torch.cuda.synchronize()
-        enc = lo.encode_obb_midpoint(anchors[pos].cpu().numpy(), gtp.cpu().numpy()) if rotated else lo.encode_aabb(gtp.cpu().numpy(), anchors[pos].cpu().numpy())
-        assert np.allclose(tout.cpu().numpy(), enc, rtol=2e-5, atol=2e-6), np.abs(tout.cpu().numpy() - enc).max()
-        # torch reference on flattened predictions
-        logits = torch.cat([p[:, :13].reshape(-1) for p in preds]).requires_grad_(True)
-        deltas = torch.cat([p[:, 13:13 + 13 * code].reshape(-1, code) for p in preds]).requires_grad_(True)
-        samp = torch.cat([pos, neg])
-        lab = torch.cat([torch.ones(pos.numel(), device="cuda"), torch.zeros(neg.numel(), device="cuda")])
-        l_obj = F.binary_cross_entropy_with_logits(logits[samp], lab)
-        l_reg = F.smooth_l1_loss(deltas[pos], torch.from_numpy(enc).cuda(), beta=1 / 9, reduction="sum") / samp.numel()
-        (l_obj + 5.0 * l_reg).backward()
-        assert abs(losses[0].item() - l_obj.item()) <= 1e-5 * abs(l_obj.item()) + 1e-7 and abs(losses[1].item() - l_reg.item()) <= 1e-4 * abs(l_reg.item()) + 1e-7
-        got_l = torch.cat([p[:, :13].reshape(-1) for p in dpreds]).float() / 256.0
-        got_d = torch.cat([p[:, 13:13 + 13 * code].reshape(-1, code) for p in dpreds]).float() / 256.0
-        assert (got_l - logits.grad).abs().max().item() <= 2.0 ** -10 * logits.grad.abs().max().item()
-        assert (got_d - deltas.grad).abs().max().item() <= 2.0 ** -10 * deltas.grad.abs().max().item() + 1e-8
 
 
 def _reference_step(rotated, layers, grid, gt, autocast_dtype=None, optimise=False):
