@@ -381,6 +381,11 @@ int nrpn_bn_backward(const void *dout, const void *act, const void *y, void *dy,
  * backward as a deterministic gather over the <= 8 windows that contain an input voxel (feature_extractor.py:219). */
 int nrpn_maxpool3d_k3s2_argmax(const void *in, int n, int x, int y, int z, int c, void *out, uint8_t *idx, int act_fp16, nrpn_stream_t stream);
 int nrpn_maxpool3d_k3s2_backward(const void *dy, const uint8_t *idx, int n, int x, int y, int z, int c, void *dx, int act_fp16, nrpn_stream_t stream);
+/* nn.MaxPool3d(2, 2, ceil_mode=True) (VGG stages, feature_extractor.py:347): the pooled map of nrpn_maxpool3d_k2s2_ceil plus one byte
+ * per output element, the window position dx*4 + dy*2 + dz of the first maximum (x outer, z inner; a NaN counts as a maximum).  The
+ * backward writes every element of dx (x,y,z the INPUT extent): dy of its window where the byte names its position, else 0. */
+int nrpn_maxpool3d_k2s2_ceil_argmax(const void *in, int n, int x, int y, int z, int c, void *out, uint8_t *idx, int act_fp16, nrpn_stream_t stream);
+int nrpn_maxpool3d_k2s2_ceil_backward(const void *dy, const uint8_t *idx, int n, int x, int y, int z, int c, void *dx, int act_fp16, nrpn_stream_t stream);
 /* Backward of the FPN top-down merge fine += nearest_upsample(coarse) (feature_extractor.py:211-213): dcoarse += sum of dfine over
  * the fine voxels whose source index floor(f * coarse / fine) is the coarse voxel (same float expression as the forward epilogue). */
 int nrpn_upsample_nearest_backward(const void *dfine, int n, int xf, int yf, int zf, int xc, int yc, int zc, int c, void *dcoarse,

@@ -167,6 +167,10 @@ _SIGNATURES = {
                                                   ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, c_stream]),
     "nrpn_maxpool3d_k3s2_backward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                     ctypes.c_int, ctypes.c_void_p, ctypes.c_int, c_stream]),
+    "nrpn_maxpool3d_k2s2_ceil_argmax": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                       ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, c_stream]),
+    "nrpn_maxpool3d_k2s2_ceil_backward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                         ctypes.c_int, ctypes.c_void_p, ctypes.c_int, c_stream]),
     "nrpn_upsample_nearest_backward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                       ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, c_stream]),
     "nrpn_stride2": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,

@@ -60,6 +60,40 @@ __device__ __forceinline__ float2 unpack_act2(uint32_t u, int fp16) {
     if (fp16) return __half22float2(*reinterpret_cast<const __half2*>(&u));
     return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u));
 }
+
+// One window of nn.MaxPool3d(kernel 2, stride 2, ceil_mode=True): output voxel (b,i,j,k), channels [8g, 8g+8) of a channels-last
+// (n,X,Y,Z,C) 16-bit map.  Only positions inside the map are candidates (the last window along an odd extent is partial).
+// m: the maximum, fmaxf of the candidates except that a NaN wins (nn.MaxPool3d propagates it).  pos: window position dx*4 + dy*2 + dz of
+// the FIRST maximum in PyTorch's scan order (x outer, z inner): a candidate takes it when it exceeds the running maximum or is the first
+// NaN.  The inference pool ignores pos; the training pool records it for the backward pass.
+__device__ __forceinline__ void maxpool_k2s2_window(const __nv_bfloat16* __restrict__ in, int X, int Y, int Z, int C, int b, int i, int j, int k,
+                                                    int g, int fp16, float (&m)[8], int (&pos)[8]) {
+#pragma unroll
+    for (int q = 0; q < 8; ++q) { m[q] = -INFINITY; pos[q] = 0; }
+#pragma unroll
+    for (int dx = 0; dx < 2; ++dx) {
+        const int x = 2 * i + dx; if (x >= X) continue;
+#pragma unroll
+        for (int dy = 0; dy < 2; ++dy) {
+            const int y = 2 * j + dy; if (y >= Y) continue;
+#pragma unroll
+            for (int dz = 0; dz < 2; ++dz) {
+                const int z = 2 * k + dz; if (z >= Z) continue;
+                const uint4 raw = __ldg(reinterpret_cast<const uint4*>(in + ((((size_t)b * X + x) * Y + y) * Z + z) * C + g * 8));
+                const uint32_t* h = reinterpret_cast<const uint32_t*>(&raw);
+                const int p = dx * 4 + dy * 2 + dz;
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    const float2 f = unpack_act2(h[q >> 1], fp16);
+                    const float v = (q & 1) ? f.y : f.x;
+                    const bool mnan = m[q] != m[q], vnan = v != v;
+                    if (v > m[q] || (vnan && !mnan)) pos[q] = p;
+                    m[q] = mnan ? m[q] : (vnan ? v : fmaxf(m[q], v));
+                }
+            }
+        }
+    }
+}
 #endif
 
 template <typename T>

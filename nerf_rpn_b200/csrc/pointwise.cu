@@ -144,7 +144,7 @@ __global__ void maxpool_k3s2_kernel(const __nv_bfloat16* __restrict__ in, int n,
 }
 
 // nn.MaxPool3d(kernel 2, stride 2, ceil_mode=True) on channels-last bf16 (VGG stages, feature_extractor.py:347):
-// output extent ceil(in/2); the last window is clipped at the border.
+// output extent ceil(in/2); the last window is clipped at the border (maxpool_k2s2_window, common.cuh).
 __global__ void maxpool_k2s2_ceil_kernel(const __nv_bfloat16* __restrict__ in, int n, int X, int Y, int Z, int C, int Xo, int Yo,
                                          int Zo, __nv_bfloat16* __restrict__ out, int fp16) {
     const int cg = C >> 3;
@@ -154,25 +154,8 @@ __global__ void maxpool_k2s2_ceil_kernel(const __nv_bfloat16* __restrict__ in, i
         const int k = (int)(v % Zo); v /= Zo;
         const int j = (int)(v % Yo); v /= Yo;
         const int i = (int)(v % Xo); const int b = (int)(v / Xo);
-        float m[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) m[q] = -INFINITY;
-#pragma unroll
-        for (int dx = 0; dx < 2; ++dx) {
-            const int x = 2 * i + dx; if (x >= X) continue;
-#pragma unroll
-            for (int dy = 0; dy < 2; ++dy) {
-                const int y = 2 * j + dy; if (y >= Y) continue;
-#pragma unroll
-                for (int dz = 0; dz < 2; ++dz) {
-                    const int z = 2 * k + dz; if (z >= Z) continue;
-                    const uint4 raw = __ldg(reinterpret_cast<const uint4*>(in + ((((size_t)b * X + x) * Y + y) * Z + z) * C + g * 8));
-                    const uint32_t* h = reinterpret_cast<const uint32_t*>(&raw);
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) { const float2 f = unpack_act2(h[q], fp16); m[2 * q] = fmaxf(m[2 * q], f.x); m[2 * q + 1] = fmaxf(m[2 * q + 1], f.y); }
-                }
-            }
-        }
+        float m[8]; int pos[8];
+        maxpool_k2s2_window(in, X, Y, Z, C, b, i, j, k, g, fp16, m, pos);
         uint32_t o[4];
 #pragma unroll
         for (int q = 0; q < 4; ++q) o[q] = pack_act2(m[2 * q], m[2 * q + 1], fp16);

@@ -3,6 +3,7 @@
 //   BatchNorm3d in TRAIN mode  (feature_extractor.py:38-43,48-68 under model.train()): batch statistics, normalise (+ residual)
 //                               (+ ReLU), running-stat update; backward = two per-channel reductions + one pointwise pass
 //   F.max_pool3d(3,2,1)         forward with recorded argmax, backward as a deterministic gather (feature_extractor.py:219)
+//   MaxPool3d(2,2,ceil_mode)    the same for the pool that ends VGG stages 2-4 (feature_extractor.py:347)
 //   F.interpolate(nearest)+add  backward of the FPN top-down merge (feature_extractor.py:211-213)
 //   stride-2 1^3 convolutions   sub-sample (forward operand of wgrad) / zero-stuff (dgrad) helpers
 //   RPN losses                  BCE-with-logits + smooth-L1(beta 1/9) on the sampled anchors and their gradient w.r.t. the
@@ -297,6 +298,69 @@ __global__ void __launch_bounds__(256) maxpool_k3s2_backward_kernel(const __nv_b
 #pragma unroll
         for (int q = 0; q < 4; ++q) o[q] = pack_act2(acc[2 * q], acc[2 * q + 1], fp16);
         *reinterpret_cast<uint4*>(dx + ((((size_t)b * X + x) * Y + y) * Z + z) * C + g * 8) = make_uint4(o[0], o[1], o[2], o[3]);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------- max-pool (2,2, ceil mode) with argmax
+// Forward: the inference pool's window (maxpool_k2s2_window) + the window position 0..7 of its first maximum, one byte per element.
+__global__ void __launch_bounds__(256) maxpool_k2s2_ceil_argmax_kernel(const __nv_bfloat16* __restrict__ in, int n, int X, int Y, int Z, int C, int Xo,
+                                                                       int Yo, int Zo, __nv_bfloat16* __restrict__ out, uint8_t* __restrict__ idx, int fp16) {
+    const int cg = C >> 3;
+    const size_t total = (size_t)n * Xo * Yo * Zo * cg;
+    for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
+        const int g = (int)(t % cg); size_t v = t / cg;
+        const int k = (int)(v % Zo); v /= Zo;
+        const int j = (int)(v % Yo); v /= Yo;
+        const int i = (int)(v % Xo); const int b = (int)(v / Xo);
+        float m[8]; int pos[8];
+        maxpool_k2s2_window(in, X, Y, Z, C, b, i, j, k, g, fp16, m, pos);
+        uint32_t o[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) o[q] = pack_act2(m[2 * q], m[2 * q + 1], fp16);
+        const size_t off = ((((size_t)b * Xo + i) * Yo + j) * Zo + k) * C + g * 8;
+        *reinterpret_cast<uint4*>(out + off) = make_uint4(o[0], o[1], o[2], o[3]);
+        *reinterpret_cast<uint2*>(idx + off) = make_uint2((uint32_t)pos[0] | ((uint32_t)pos[1] << 8) | ((uint32_t)pos[2] << 16) | ((uint32_t)pos[3] << 24),
+                                                          (uint32_t)pos[4] | ((uint32_t)pos[5] << 8) | ((uint32_t)pos[6] << 16) | ((uint32_t)pos[7] << 24));
+    }
+}
+
+// Backward: the windows are disjoint and tile the input, so every input element has exactly one window and the backward is a gather with
+// no sums.  One thread per window and channel group reads dy and idx once and writes the 16-bit dy (bits unchanged) to the recorded
+// position and zeros to the other positions inside the input: every element of dx is written once, no memset, no atomics.
+__global__ void __launch_bounds__(256) maxpool_k2s2_ceil_backward_kernel(const __nv_bfloat16* __restrict__ dy, const uint8_t* __restrict__ idx, int n, int X,
+                                                                         int Y, int Z, int C, int Xo, int Yo, int Zo, __nv_bfloat16* __restrict__ dx) {
+    const int cg = C >> 3;
+    const size_t total = (size_t)n * Xo * Yo * Zo * cg;
+    for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
+        const int g = (int)(t % cg); size_t v = t / cg;
+        const int k = (int)(v % Zo); v /= Zo;
+        const int j = (int)(v % Yo); v /= Yo;
+        const int i = (int)(v % Xo); const int b = (int)(v / Xo);
+        const size_t off = ((((size_t)b * Xo + i) * Yo + j) * Zo + k) * C + g * 8;
+        const uint2 iv = __ldg(reinterpret_cast<const uint2*>(idx + off));
+        const uint4 gv = __ldg(reinterpret_cast<const uint4*>(dy + off));
+        const uint32_t gw[4] = {gv.x, gv.y, gv.z, gv.w};
+#pragma unroll
+        for (int dx_ = 0; dx_ < 2; ++dx_) {
+            const int x = 2 * i + dx_; if (x >= X) continue;
+#pragma unroll
+            for (int dy_ = 0; dy_ < 2; ++dy_) {
+                const int y = 2 * j + dy_; if (y >= Y) continue;
+#pragma unroll
+                for (int dz = 0; dz < 2; ++dz) {
+                    const int z = 2 * k + dz; if (z >= Z) continue;
+                    const uint32_t p = dx_ * 4 + dy_ * 2 + dz;
+                    uint32_t o[4];
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) {
+                        const uint32_t word = q < 2 ? iv.x : iv.y;
+                        const uint32_t ia = (word >> (16 * (q & 1))) & 0xFFu, ib = (word >> (16 * (q & 1) + 8)) & 0xFFu;
+                        o[q] = (ia == p ? (gw[q] & 0xFFFFu) : 0u) | (ib == p ? (gw[q] & 0xFFFF0000u) : 0u);
+                    }
+                    *reinterpret_cast<uint4*>(dx + ((((size_t)b * X + x) * Y + y) * Z + z) * C + g * 8) = make_uint4(o[0], o[1], o[2], o[3]);
+                }
+            }
+        }
     }
 }
 
@@ -655,6 +719,27 @@ int nrpn_maxpool3d_k3s2_backward(const void* dy, const uint8_t* idx, int n, int 
     const size_t total = (size_t)n * x * y * z * (c / 8);
     maxpool_k3s2_backward_kernel<<<grid1d(total, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __nv_bfloat16*>(dy), idx, n, x, y, z, c, Xo, Yo, Zo,
                                                                                        reinterpret_cast<__nv_bfloat16*>(dx), act_fp16 ? 1 : 0);
+    NRPN_LAUNCH_CHECK();
+    return NRPN_OK;
+}
+
+int nrpn_maxpool3d_k2s2_ceil_argmax(const void* in, int n, int x, int y, int z, int c, void* out, uint8_t* idx, int act_fp16, nrpn_stream_t stream) {
+    if (!in || !out || !idx || n < 1 || x < 1 || y < 1 || z < 1 || c < 8 || c % 8 != 0) return NRPN_ERR_INVALID;
+    const int Xo = (x + 1) / 2, Yo = (y + 1) / 2, Zo = (z + 1) / 2;
+    const size_t total = (size_t)n * Xo * Yo * Zo * (c / 8);
+    maxpool_k2s2_ceil_argmax_kernel<<<grid1d(total, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __nv_bfloat16*>(in), n, x, y, z, c, Xo, Yo, Zo,
+                                                                                          reinterpret_cast<__nv_bfloat16*>(out), idx, act_fp16 ? 1 : 0);
+    NRPN_LAUNCH_CHECK();
+    return NRPN_OK;
+}
+
+int nrpn_maxpool3d_k2s2_ceil_backward(const void* dy, const uint8_t* idx, int n, int x, int y, int z, int c, void* dx, int act_fp16, nrpn_stream_t stream) {
+    (void)act_fp16;                                     // moves 16-bit patterns: the same code for both formats
+    if (!dy || !dx || !idx || n < 1 || x < 1 || y < 1 || z < 1 || c < 8 || c % 8 != 0) return NRPN_ERR_INVALID;
+    const int Xo = (x + 1) / 2, Yo = (y + 1) / 2, Zo = (z + 1) / 2;
+    const size_t total = (size_t)n * Xo * Yo * Zo * (c / 8);
+    maxpool_k2s2_ceil_backward_kernel<<<grid1d(total, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __nv_bfloat16*>(dy), idx, n, x, y, z, c, Xo, Yo, Zo,
+                                                                                            reinterpret_cast<__nv_bfloat16*>(dx));
     NRPN_LAUNCH_CHECK();
     return NRPN_OK;
 }

@@ -163,7 +163,7 @@ class _BN:
 
 
 class RPNTrainEngine:
-    """Forward + backward + update for ResNet_FPN_256 + RPNHead (+ RegionProposalNetwork hyper-parameters)."""
+    """Forward + backward + update for ResNet_FPN_256 or VGG_FPN (strided stem) + RPNHead (+ RegionProposalNetwork hyper-parameters)."""
 
     def __init__(self, model, precision: str = "bf16", lr: float = 1e-4, weight_decay: float = 0.01, betas=(0.9, 0.999), eps: float = 1e-8,
                  clip_grad_norm: float = 0.1, reg_loss_weight: float = 5.0, process_group=None, bucket_mb: float = 32.0,
@@ -171,8 +171,15 @@ class RPNTrainEngine:
         if precision not in ("bf16", "fp16"):
             raise ValueError("training runs with bf16 (default) or fp16 (with a static loss scale) 16-bit activations / gradients")
         bb, rpn = model.backbone, model.rpn
-        if type(bb).__name__ != "ResNet_FPN_256":
-            raise NotImplementedError("nerf_rpn_b200: the training engine implements ResNet_FPN_256 + RPNHead (BASELINE config 4)")
+        built = ("nerf_rpn_b200: the training engine implements RPNHead on ResNet_FPN_256 (BASELINE config 4) or on VGG_FPN with cfg AF / DF / EF, "
+                 "batch_norm=True and the strided stem (input_size >= 160)")
+        if type(bb).__name__ == "VGG_FPN":
+            mods = list(bb.layers.children())
+            convs = [(grp, i) for grp in mods[-4:] for i, m in enumerate(grp) if isinstance(m, torch.nn.Conv3d)]
+            if mods[0].stride[0] != 2 or not all(i + 1 < len(grp) and isinstance(grp[i + 1], torch.nn.BatchNorm3d) for grp, i in convs):
+                raise NotImplementedError(built)
+        elif type(bb).__name__ != "ResNet_FPN_256":
+            raise NotImplementedError(built)
         if rpn.reg_loss_type not in ("smooth_l1", "iou", "linear_iou", "giou", "diou"):
             raise NotImplementedError(f"nerf_rpn_b200: unknown reg_loss_type {rpn.reg_loss_type!r}")
         if rpn.reg_loss_type != "smooth_l1" and not rpn.rotate:
@@ -269,22 +276,45 @@ class RPNTrainEngine:
         return self.flat_g[off:off + n]
 
     def _build_layers(self):
+        """The backbone's trainable layers.  ResNet: self.blocks (Bottleneck dicts).  VGG: self.vgg_stages, four lists of
+        ("conv", _TConv, _BN) / ("pool",) items.  Either neck: self.lat, the lateral convs coarsest level first, and self.fpn_out, the output
+        conv of each of those levels, None where the level is its lateral (ResNet's P5)."""
         bb, hd = self.bb, self.head
 
         def conv(m: torch.nn.Conv3d, **kw):
             return _TConv(self, m.weight, m.bias, stride=m.stride[0], **kw)
-        self.stem = conv(bb.conv1, need_dgrad=False, stem=True)
-        self.stem_bn = _BN(self, bb.bn1)
-        self.blocks = []
-        for stage in bb.layers:
-            for blk in stage:
-                e = dict(c1=conv(blk.conv1), bn1=_BN(self, blk.bn1), c2=conv(blk.conv2), bn2=_BN(self, blk.bn2),
-                         c3=conv(blk.conv3), bn3=_BN(self, blk.bn3), ds=None, bnd=None, stride=blk.stride)
-                if blk.downsample is not None:
-                    e["ds"] = conv(blk.downsample[0]); e["bnd"] = _BN(self, blk.downsample[1])
-                self.blocks.append(e)
-        self.lat = [conv(m) for m in bb.latlayers]
-        self.smooth = [conv(m) for m in bb.smooths]
+        self.blocks, self.vgg_stages = [], None
+        if type(bb).__name__ == "ResNet_FPN_256":
+            self.stem = conv(bb.conv1, need_dgrad=False, stem=True)
+            self.stem_bn = _BN(self, bb.bn1)
+            for stage in bb.layers:
+                for blk in stage:
+                    e = dict(c1=conv(blk.conv1), bn1=_BN(self, blk.bn1), c2=conv(blk.conv2), bn2=_BN(self, blk.bn2),
+                             c3=conv(blk.conv3), bn3=_BN(self, blk.bn3), ds=None, bnd=None, stride=blk.stride)
+                    if blk.downsample is not None:
+                        e["ds"] = conv(blk.downsample[0]); e["bnd"] = _BN(self, blk.downsample[1])
+                    self.blocks.append(e)
+            body = [e[k] for e in self.blocks for k in ("c1", "c2", "c3", "ds") if e[k] is not None]
+            self.lat = [conv(m) for m in bb.latlayers]
+            self.fpn_out = [None] + [conv(m) for m in bb.smooths]
+        else:                                           # VGG_FPN with a strided stem and BatchNorm (checked by __init__)
+            mods = list(bb.layers.children())
+            self.stem = conv(mods[0], need_dgrad=False, stem=True)
+            self.stem_bn = _BN(self, mods[1])
+            self.vgg_stages = []
+            for grp in mods[-4:]:
+                seq, items = list(grp.children()), []
+                for i, m in enumerate(seq):
+                    if isinstance(m, torch.nn.Conv3d):
+                        items.append(("conv", conv(m), _BN(self, seq[i + 1])))
+                    elif isinstance(m, torch.nn.MaxPool3d):
+                        items.append(("pool",))
+                # cfgs AF / DF / EF: a pool only ever ends a stage, so a stage's backward needs two scratch buffers
+                assert all(it[0] == "conv" for it in items[:-1]), "unexpected VGG stage layout"
+                self.vgg_stages.append(items)
+            body = [it[1] for items in self.vgg_stages for it in items if it[0] == "conv"]
+            self.lat = [conv(m) for m in reversed(bb.fpn_neck.lateral_convs)]
+            self.fpn_out = [conv(m) for m in reversed(bb.fpn_neck.fpn_convs)]
         self.hconv = [conv(m) for m in hd.conv if isinstance(m, torch.nn.Conv3d)]
         # fused cls | bbox predictor (anchor.py:196-198): one 1^3 conv with 128 (padded) output channels on fp32 staging copies of the two
         # layers' weights and biases (_repack_head); its gradients land in staging buffers that head_bwd splits into the two layers' gradients
@@ -294,7 +324,7 @@ class RPNTrainEngine:
         f32 = dict(dtype=torch.float32, device=self.device)
         self.predictor = _TConv(self, torch.zeros((128, 256, 1, 1, 1), **f32), torch.zeros(128, **f32),
                                 dw=torch.zeros((128, 256), **f32), db=torch.zeros(128, **f32))
-        self.all_convs = [self.stem] + [e[k] for e in self.blocks for k in ("c1", "c2", "c3", "ds") if e[k] is not None] + self.lat + self.smooth + self.hconv
+        self.all_convs = [self.stem] + body + self.lat + [c for c in self.fpn_out if c is not None] + self.hconv
 
     def repack(self, head_only: bool = False):
         """fp32 master weights -> 16-bit GEMM operands (after every optimiser step / checkpoint load); head_only: the head's convs and the
@@ -429,11 +459,11 @@ class RPNTrainEngine:
 
 class _TrainPlan:
     """Buffers and the launch lists (forward, backward) for n scenes of one size.  frozen: the backbone gets no gradient, so the backward list
-    is the head's alone and every backbone activation that only its backward would read lives in a few reused slots."""
+    is the head's alone and every backbone activation that only its backward would read lives in a few reused slots.
+    Built in four parts: the stem, the backbone body (ResNet blocks or VGG stages), the FPN and the head."""
 
     def __init__(self, eng: RPNTrainEngine, n: int, dims, frozen: bool = False):
         self.eng, self.n, self.dims, self.frozen = eng, n, dims, frozen
-        dev, dt = eng.device, eng.act_dtype
         self.fwd: List = []
         self.bwd: List = []                      # built in forward order, executed reversed
         self.bwd_lo: List[int] = []              # lowest flat-parameter offset whose gradient is final once bwd[i] has run
@@ -441,74 +471,106 @@ class _TrainPlan:
         self._scratch = eng._scratch             # shared by every plan (engine-level, grows to the largest batch)
         self._graphs = {}
         self._grew = False
-        X, Y, Z = dims
-        L = lib()
-        n_req = [0]
-
-        def req(shape, dtype=dt):
-            t = eng._pool_view(n_req[0], tuple(shape), dtype, self)
-            n_req[0] += 1
-            return t
-
-        def buf(d, c, dtype=dt):
-            return req((n, *d, c), dtype)
-
+        self._n_req = 0
         self.input = None
         d1 = _down(dims)
         d2 = _down(d1)
-        # the blocks in order: (stage, block, its input dims, its output dims, is the stage's first / last block)
+        geo = self._resnet_geometry(d2) if eng.vgg_stages is None else self._vgg_geometry(d2)
+        self.packed = self._req((n, d1[0], d1[1], d1[2] + 1, 64))
+        self.fwd.append(self._pack_input)
+        if frozen:
+            self._act = self._frozen_slots(*(self._resnet_slot_uses(geo, d1, d2) if eng.vgg_stages is None else self._vgg_slot_uses(geo, d1, d2)))
+        else:
+            self._act = lambda slot, d, c: self._buf(d, c)
+        p0, dp0 = self._build_stem(d1, d2)
+        c_out = self._build_resnet_body(geo, p0, dp0) if eng.vgg_stages is None else self._build_vgg_body(geo, p0, dp0)
+        self._build_head(*self._build_fpn(c_out))
+        self._src = None
+        self._sizes = None
+        self._alpha = False
+        self.valid = None
+        self.anchors = None
+        if self._grew:
+            torch.cuda.empty_cache()            # hand the replaced (smaller) slots back instead of keeping them cached next to the new ones
+
+    # ------------------------------------------------------------------------------------------------ buffers of the plan
+    def _req(self, shape, dtype=None):
+        """The next buffer of the plan: every plan requests its buffers in the same order (see RPNTrainEngine._pool_view)."""
+        t = self.eng._pool_view(self._n_req, tuple(shape), self.eng.act_dtype if dtype is None else dtype, self)
+        self._n_req += 1
+        return t
+
+    def _buf(self, d, c, dtype=None):
+        return self._req((self.n, *d, c), dtype)
+
+    def _frozen_slots(self, use, names):
+        """Slots of a frozen plan's forward-only activations: use[k] = [(dims, channels)] of every activation placed in slot kind k; names =
+        [(slot, kind)] in request order, each slot sized for its kind's largest use.  Returns act(slot, dims, channels)."""
+        n = self.n
+        size = {k: max([n * math.prod(d) * c for d, c in u] + [1]) for k, u in use.items()}
+        slots = {s: self._req((size[k],)) for s, k in names}
+
+        def act(slot, d, c):
+            return slots[slot][:n * math.prod(d) * c].view(n, *d, c)
+        return act
+
+    # ------------------------------------------------------------------------------------------------ stem
+    def _build_stem(self, d1, d2):
+        """Stem conv (+ its bias, VGG) + BN + ReLU + max-pool (3, 2, 1).  Returns the pooled map and the buffer receiving its gradient."""
+        eng, n, L = self.eng, self.n, lib()
+        y0 = self._act("y", d1, 64); a0 = self._act("a", d1, 64)
+        self._conv_fwd(eng.stem, [self.packed], [(d1[0], d1[1], d1[2] + 1)], [y0], [d1])
+        self._bn_fwd(eng.stem_bn, y0, None, a0, True)
+        p0 = self._act("x0", d2, 64)
+        if self.frozen:
+            self.fwd.append(lambda: check(L.nrpn_maxpool3d_k3s2(_p(a0), n, d1[0], d1[1], d1[2], 64, _p(p0), self.f16, _stream()), "maxpool"))
+            return p0, None
+        self.pool_idx = self._buf(d2, 64, torch.uint8)
+        self.fwd.append(lambda: check(L.nrpn_maxpool3d_k3s2_argmax(_p(a0), n, d1[0], d1[1], d1[2], 64, _p(p0), _p(self.pool_idx), self.f16, _stream()),
+                                      "maxpool_argmax"))
+        dp0 = self._buf(d2, 64)                          # gradient w.r.t. the pooled map
+        da0 = self._buf(d1, 64); dy0 = self._buf(d1, 64)
+
+        # backward of the stem (runs LAST): pool backward -> BN backward -> stem wgrad (on the packed input) and bias gradient
+        def stem_bwd():
+            check(L.nrpn_maxpool3d_k3s2_backward(_p(dp0), _p(self.pool_idx), n, d1[0], d1[1], d1[2], 64, _p(da0), self.f16, _stream()), "maxpool_backward")
+            self._bn_bwd(eng.stem_bn, da0, a0, y0, dy0, None, True)
+            self._wgrad_stem(dy0)
+            if eng.stem.db is not None:                 # VGG's stem conv has a bias, ResNet's has none
+                self._bias_grad(eng.stem, [dy0])
+        self.bwd.append(stem_bwd)
+        self.bwd_lo.append(0)
+        return p0, dp0
+
+    # ------------------------------------------------------------------------------------------------ ResNet body
+    def _resnet_geometry(self, d2):
+        """The blocks in order: (stage, block, its input dims, its output dims, is the stage's first / last block)."""
         geo, xd = [], d2
-        for si, stage in enumerate(eng.bb.layers):
+        for si, stage in enumerate(self.eng.bb.layers):
             for j in range(len(stage)):
-                e = eng.blocks[len(geo)]
+                e = self.eng.blocks[len(geo)]
                 od = _down(xd) if e["stride"] == 2 else xd
                 geo.append((si, e, xd, od, j == 0, j == len(stage) - 1))
                 xd = od
-        self.packed = req((n, d1[0], d1[1], d1[2] + 1, 64))
-        self.fwd.append(self._pack_input)
-        if frozen:
-            # activations read only by the forward: the stem's y0 / a0 share slots "y" / "a" with the blocks' y3 / yd, every block's y1, y2
-            # share "y1" and a1, a2 share "a1", and the max-pool output and the outputs that are not a stage's last alternate between "x0"
-            # and "x1" (sized alike).  Each slot is requested once, at its largest use.
-            use = {"y": [(d1, 64)], "a": [(d1, 64)], "r": [], "y1": [], "a1": [], "x": [(d2, 64)]}
-            for si, e, xd_, od, first, last in geo:
-                use["y1"].append((od, e["c1"].cout)); use["a1"].append((od, e["c1"].cout)); use["y"].append((od, e["c3"].cout))
-                if e["ds"] is not None:
-                    use["a"].append((od, e["c3"].cout)); use["r"].append((od, e["c3"].cout))
-                if not last:
-                    use["x"].append((od, e["c3"].cout))
-            size = {k: max([n * math.prod(d) * c for d, c in u] + [1]) for k, u in use.items()}
-            slots = {k: req((size[k],)) for k in ("y", "a", "r", "y1", "a1")}
-            slots["x0"], slots["x1"] = req((size["x"],)), req((size["x"],))
+        return geo
 
-            def act(slot, d, c):
-                return slots[slot][:n * math.prod(d) * c].view(n, *d, c)
-        else:
-            def act(slot, d, c):
-                return buf(d, c)
-        y0 = act("y", d1, 64); a0 = act("a", d1, 64)
-        self._conv_fwd(eng.stem, [self.packed], [(d1[0], d1[1], d1[2] + 1)], [y0], [d1])
-        self._bn_fwd(eng.stem_bn, y0, None, a0, True)
-        p0 = act("x0", d2, 64)
-        if frozen:
-            self.fwd.append(lambda: check(L.nrpn_maxpool3d_k3s2(_p(a0), n, d1[0], d1[1], d1[2], 64, _p(p0), self.f16, _stream()), "maxpool"))
-        else:
-            self.pool_idx = buf(d2, 64, torch.uint8)
-            self.fwd.append(lambda: check(L.nrpn_maxpool3d_k3s2_argmax(_p(a0), n, d1[0], d1[1], d1[2], 64, _p(p0), _p(self.pool_idx), self.f16, _stream()),
-                                          "maxpool_argmax"))
-            dp0 = buf(d2, 64)                          # gradient w.r.t. the pooled map
-            da0 = buf(d1, 64); dy0 = buf(d1, 64)
+    def _resnet_slot_uses(self, geo, d1, d2):
+        # activations read only by the forward: the stem's y0 / a0 share slots "y" / "a" with the blocks' y3 / yd, every block's y1, y2
+        # share "y1" and a1, a2 share "a1", and the max-pool output and the outputs that are not a stage's last alternate between "x0"
+        # and "x1" (sized alike).  Each slot is requested once, at its largest use.
+        use = {"y": [(d1, 64)], "a": [(d1, 64)], "r": [], "y1": [], "a1": [], "x": [(d2, 64)]}
+        for si, e, xd_, od, first, last in geo:
+            use["y1"].append((od, e["c1"].cout)); use["a1"].append((od, e["c1"].cout)); use["y"].append((od, e["c3"].cout))
+            if e["ds"] is not None:
+                use["a"].append((od, e["c3"].cout)); use["r"].append((od, e["c3"].cout))
+            if not last:
+                use["x"].append((od, e["c3"].cout))
+        return use, [("y", "y"), ("a", "a"), ("r", "r"), ("y1", "y1"), ("a1", "a1"), ("x0", "x"), ("x1", "x")]
 
-            # backward of the stem (runs LAST): pool backward -> BN backward -> stem wgrad (on the packed input)
-            def stem_bwd():
-                check(L.nrpn_maxpool3d_k3s2_backward(_p(dp0), _p(self.pool_idx), n, d1[0], d1[1], d1[2], 64, _p(da0), self.f16, _stream()), "maxpool_backward")
-                self._bn_bwd(eng.stem_bn, da0, a0, y0, dy0, None, True)
-                self._wgrad_stem(dy0)
-            self.bwd.append(stem_bwd)
-            self.bwd_lo.append(0)
-
-        # ---- bottom-up
-        x, dx, xs = p0, (None if frozen else dp0), "x0"     # block input, the buffer that receives its gradient, and its slot (frozen)
+    def _build_resnet_body(self, geo, p0, dp0):
+        """Bottleneck blocks.  Returns the four stage outputs [(tensor, dims, gradient buffer)], finest first."""
+        eng, frozen, act, buf = self.eng, self.frozen, self._act, self._buf
+        x, dx, xs = p0, dp0, "x0"     # block input, the buffer that receives its gradient, and its slot (frozen)
         c_out = []
         for si, e, xd, od, first, last in geo:
             # a stage's first block -- and only it -- has a downsample, strided in every stage but the first (ResNet_FPN_256._make_layer):
@@ -544,50 +606,152 @@ class _TrainPlan:
             x, dx = out, dout
             if last:
                 c_out.append((x, od, dx))
+        return c_out
 
-        # ---- FPN top-down (feature_extractor.py:224-235)
+    # ------------------------------------------------------------------------------------------------ VGG body
+    def _vgg_geometry(self, d2):
+        """Per stage: [(item, its input dims, its output dims, its output channels)]; a ceil-mode pool halves the extent rounding up."""
+        geo, xd, c = [], d2, 64
+        for items in self.eng.vgg_stages:
+            st = []
+            for it in items:
+                od = _down(xd) if it[0] == "pool" else xd
+                c = it[1].cout if it[0] == "conv" else c
+                st.append((it, xd, od, c))
+                xd = od
+            geo.append(st)
+        return geo
+
+    def _vgg_slot_uses(self, geo, d1, d2):
+        # activations read only by the forward: every conv's raw output shares slot "y" with the stem's y0, the stem's a0 has slot "a", and
+        # the max-pool output and the activations that are not a stage's output alternate between "x0" and "x1"
+        use = {"y": [(d1, 64)], "a": [(d1, 64)], "x": [(d2, 64)]}
+        for st in geo:
+            for j, (it, xd, od, c) in enumerate(st):
+                if it[0] == "conv":
+                    use["y"].append((xd, c))
+                if j < len(st) - 1:
+                    use["x"].append((od, c))
+        return use, [("y", "y"), ("a", "a"), ("x0", "x"), ("x1", "x")]
+
+    def _build_vgg_body(self, geo, p0, dp0):
+        """Stages of conv (+ bias) -> batch statistics -> BN + ReLU, a stage of cfg AF / DF / EF ending in MaxPool3d(2, 2, ceil_mode=True)
+        from the second on (feature_extractor.py:343-357).  Returns the four stage outputs [(tensor, dims, gradient buffer)], finest first."""
+        eng, n, L, frozen = self.eng, self.n, lib(), self.frozen
+        x, dx, xs = p0, dp0, "x0"
+        c_out = []
+        for si, st in enumerate(geo):
+            recs = []                             # what the stage's backward reads, in forward order
+            for j, (it, xd, od, c) in enumerate(st):
+                if frozen and j < len(st) - 1:
+                    xs = "x1" if xs == "x0" else "x0"
+                    out = self._act(xs, od, c)
+                else:
+                    out = self._buf(od, c)        # a stage output (read by its FPN lateral) persists
+                if it[0] == "conv":
+                    _, conv, bn = it
+                    y = self._act("y", xd, c)     # raw conv output, conv bias included (_TConv.shift)
+                    self._conv_fwd(conv, [x], [xd], [y], [xd])
+                    self._bn_fwd(bn, y, None, out, True)
+                    recs.append(("conv", conv, bn, x, xd, y, out))
+                elif frozen:
+                    self.fwd.append(lambda a=x, o=out, d=xd, ch=c: check(L.nrpn_maxpool3d_k2s2_ceil(_p(a), n, d[0], d[1], d[2], ch, _p(o), self.f16, _stream()),
+                                                                        "maxpool_k2s2"))
+                else:
+                    idx = self._buf(od, c, torch.uint8)
+                    self.fwd.append(lambda a=x, o=out, i=idx, d=xd, ch=c: check(
+                        L.nrpn_maxpool3d_k2s2_ceil_argmax(_p(a), n, d[0], d[1], d[2], ch, _p(o), _p(i), self.f16, _stream()), "maxpool_k2s2_argmax"))
+                    recs.append(("pool", x, xd, idx))
+                x = out
+            dout = None
+            if not frozen:
+                dout = self._buf(st[-1][2], st[-1][3])  # gradient w.r.t. the stage output: fpn_bwd writes the lateral part first
+                self.bwd.append(self._make_vgg_stage_bwd(recs, dx, dout, accumulate=si > 0))
+                self.bwd_lo.append(min(eng.offsets[id(r[1].weight)][0] for r in recs if r[0] == "conv"))
+            c_out.append((x, st[-1][2], dout))
+            dx = dout
+        return c_out
+
+    def _make_vgg_stage_bwd(self, recs, dx, dout, accumulate):
+        """Backward of one VGG stage, items in reverse: pool backward; BN backward (ReLU masked), weight and bias gradients, data gradient.
+        dx receives the gradient of the stage input.  accumulate: dx is the previous stage's output gradient, which already holds the lateral
+        part fpn_bwd wrote, and the first conv's data gradient is added to it."""
+        L, n, dt = lib(), self.n, self.eng.act_dtype
+
+        def f():
+            g = dout                                                            # gradient w.r.t. the current item's output
+            for k in range(len(recs) - 1, -1, -1):
+                r = recs[k]
+                if r[0] == "pool":
+                    _, a, ad, idx = r
+                    da = self._scratch_buf("vgg_g", a.numel(), dt).view_as(a)
+                    check(L.nrpn_maxpool3d_k2s2_ceil_backward(_p(g), _p(idx), n, ad[0], ad[1], ad[2], a.shape[-1], _p(da), self.f16, _stream()),
+                          "maxpool_k2s2_backward")
+                    g = da
+                    continue
+                _, conv, bn, x, xd, y, a = r
+                dy = self._scratch_buf("vgg_dy", y.numel(), dt).view_as(y)
+                self._bn_bwd(bn, g, a, y, dy, None, True)
+                self._param_grad(conv, [dy], [x])
+                dst = dx if k == 0 and not accumulate else self._scratch_buf("vgg_g", x.numel(), dt).view_as(x)
+                self._dgrad(conv, [dy], [dst], [xd])
+                g = dst
+            if accumulate:
+                check(L.nrpn_add_inplace(_p(dx), _p(g), dx.numel(), self.f16, _stream()), "add_inplace")
+        return f
+
+    # ------------------------------------------------------------------------------------------------ FPN
+    def _build_fpn(self, c_out):
+        """Top-down FPN of either neck (feature_extractor.py:224-235, fpn.py:134-161) on the stage outputs c_out (finest first): level i,
+        coarsest first, is eng.lat[i] on its stage output plus the nearest up-sampled level i - 1, then eng.fpn_out[i] on it (None: the
+        level itself is the feature map).  Returns ([P2..P5], their gradient buffers, their dims)."""
+        eng, n, L, frozen, buf = self.eng, self.n, lib(), self.frozen, self._buf
         grad = (lambda d, c: None) if frozen else buf      # the FPN's gradient buffers (none when the backbone is frozen)
-        (c5, d5, dc5) = c_out[-1]
-        q = [None] * 4; dq = [None] * 4; qd = [None] * 4
-        q[0] = buf(d5, 256); dq[0] = grad(d5, 256); qd[0] = d5
-        self._conv_fwd(eng.lat[0], [c5], [d5], [q[0]], [d5])
-        for i in range(1, 4):
-            (c, cd, _) = c_out[-1 - i]
-            q[i] = buf(cd, 256); dq[i] = grad(cd, 256); qd[i] = cd
-            self._conv_fwd(eng.lat[i], [c], [cd], [q[i]], [cd], res=q[i - 1], res_dims=qd[i - 1])
-        feats, dfeats, fdims = [q[0]], [dq[0]], [d5]           # P5 = q5 (no smooth conv); its gradient accumulates in dq[0]
-        for i, sm in enumerate(eng.smooth):
-            f = buf(qd[i + 1], 256); df = grad(qd[i + 1], 256)
-            self._conv_fwd(sm, [q[i + 1]], [qd[i + 1]], [f], [qd[i + 1]])
-            feats.append(f); dfeats.append(df); fdims.append(qd[i + 1])
-        feats.reverse(); dfeats.reverse(); fdims.reverse()      # [P2, P3, P4, P5]
-        self.features, self.feat_dims = feats, fdims
+        lvl = c_out[::-1]
+        q, dq, qd = [], [], []
+        for i, ((c, cd, _), lat) in enumerate(zip(lvl, eng.lat)):
+            q.append(buf(cd, 256)); dq.append(grad(cd, 256)); qd.append(cd)
+            if i == 0:
+                self._conv_fwd(lat, [c], [cd], [q[0]], [cd])
+            else:
+                self._conv_fwd(lat, [c], [cd], [q[i]], [cd], res=q[i - 1], res_dims=qd[i - 1])
+        feats, dfeats = [], []
+        for i, oc in enumerate(eng.fpn_out):
+            if oc is None:                                  # the level's gradient accumulates in dq[i]
+                feats.append(q[i]); dfeats.append(dq[i])
+                continue
+            f = buf(qd[i], 256); df = grad(qd[i], 256)
+            self._conv_fwd(oc, [q[i]], [qd[i]], [f], [qd[i]])
+            feats.append(f); dfeats.append(df)
 
-        # FPN backward (executed after the head's backward): smooth convs, top-down merge, laterals
+        # FPN backward (executed after the head's backward): output convs and the top-down merge from the finest level, then the laterals
         def fpn_bwd():
-            # dfeats = [dP2, dP3, dP4, dP5(=dq[0])]
-            for i in (2, 1, 0):                                 # smooth[i] acts on q[i+1]; finest level first
-                lvl_feat = 2 - i                                # index into feats / dfeats ([P2,P3,P4,P5]): smooth[2]->P2, [1]->P3, [0]->P4
-                self._param_grad(eng.smooth[i], [dfeats[lvl_feat]], [q[i + 1]])
-                self._dgrad(eng.smooth[i], [dfeats[lvl_feat]], [dq[i + 1]], [qd[i + 1]])
-                if i < 2:                                       # the finer level's merged map took up(q[i+1]) as its residual
-                    fd, cd_ = qd[i + 2], qd[i + 1]
-                    check(L.nrpn_upsample_nearest_backward(_p(dq[i + 2]), n, fd[0], fd[1], fd[2], cd_[0], cd_[1], cd_[2], 256, _p(dq[i + 1]), self.f16, _stream()),
+            for i in range(len(q) - 1, -1, -1):
+                oc = eng.fpn_out[i]
+                if oc is not None:
+                    self._param_grad(oc, [dfeats[i]], [q[i]])
+                    self._dgrad(oc, [dfeats[i]], [dq[i]], [qd[i]])
+                if i + 1 < len(q):                          # the finer level's merged map took up(q[i]) as its residual
+                    fd, cd_ = qd[i + 1], qd[i]
+                    check(L.nrpn_upsample_nearest_backward(_p(dq[i + 1]), n, fd[0], fd[1], fd[2], cd_[0], cd_[1], cd_[2], 256, _p(dq[i]), self.f16, _stream()),
                           "upsample_backward")
-            fd, cd_ = qd[1], qd[0]
-            check(L.nrpn_upsample_nearest_backward(_p(dq[1]), n, fd[0], fd[1], fd[2], cd_[0], cd_[1], cd_[2], 256, _p(dq[0]), self.f16, _stream()),
-                  "upsample_backward")
-            for i in range(4):
-                (c, cd, dc) = c_out[-1 - i]
-                self._param_grad(eng.lat[i], [dq[i]], [c])
-                self._dgrad(eng.lat[i], [dq[i]], [dc], [cd])    # dc = gradient of the stage output from the lateral branch
-        # NOTE: the stage outputs c2..c4 also receive the next stage's data gradient: _make_block_bwd ADDS into dx for the first block
-        # of stages 1..3, because fpn_bwd (which runs earlier) has already written the lateral part.
+            for i, ((c, cd, dc), lat) in enumerate(zip(lvl, eng.lat)):
+                self._param_grad(lat, [dq[i]], [c])
+                self._dgrad(lat, [dq[i]], [dc], [cd])      # dc = gradient of the stage output from the lateral branch
+        # NOTE: the stage outputs c2..c4 also receive the next stage's data gradient: the body's backward ADDS it into dc, because fpn_bwd
+        # (which runs earlier) has already written the lateral part.
         if not frozen:
             self.bwd.append(fpn_bwd)
-            self.bwd_lo.append(min(eng.offsets[id(c.weight)][0] for c in eng.lat + eng.smooth))
+            self.bwd_lo.append(min(eng.offsets[id(c.weight)][0] for c in eng.lat + [o for o in eng.fpn_out if o is not None]))
+        self.dbg = dict(q=q, dq=dq, c_out=c_out)           # tools/debug_train.py
+        self.features, self.feat_dims = feats[::-1], qd[::-1]   # [P2, P3, P4, P5]; fpn_bwd keeps reading dfeats coarsest level first
+        return self.features, dfeats[::-1], self.feat_dims
 
-        # ---- head: all levels in one launch per layer, activations of all levels in ONE buffer (bias gradients are one reduction)
+    # ------------------------------------------------------------------------------------------------ head
+    def _build_head(self, feats, dfeats, fdims):
+        """All levels in one launch per layer, activations of all levels in ONE buffer (bias gradients are one reduction)."""
+        eng, n, L, frozen, req = self.eng, self.n, lib(), self.frozen, self._req
+        dims = self.dims
         vox = [d[0] * d[1] * d[2] for d in fdims]
         self.total_vox = n * sum(vox)
 
@@ -607,7 +771,7 @@ class _TrainPlan:
             self._conv_fwd(layer, cur, fdims, nxt, fdims, relu=True)
             cur = nxt
         self._conv_fwd(eng.predictor, cur, fdims, self.pred_levels, fdims, out_fp32=True)
-        self.dbg = dict(hs=h_lv, dhs=dh_lv, dfeats=dfeats, q=q, dq=dq, c_out=c_out)   # tools/debug_train.py
+        self.dbg.update(hs=h_lv, dhs=dh_lv, dfeats=dfeats)
         self.strides = [tuple(dims[k] // d[k] for k in range(3)) for d in fdims]
         # the head's layers with the input and the output of each, all levels, and their gradients
         layers, ins, dins, douts = eng.hconv + [eng.predictor], [feats] + h_lv, [dfeats] + dh_lv, dh_lv + [self.dpred_levels]
@@ -625,13 +789,6 @@ class _TrainPlan:
             eng.grad_of(hd.cls_logits.bias).copy_(pr.db[:A]); eng.grad_of(hd.bbox_pred.bias).copy_(pr.db[A:eng.n_pred])
         self.bwd.append(head_bwd)
         self.bwd_lo.append(min(eng.offsets[id(p_)][0] for p_ in eng.head.parameters()))
-        self._src = None
-        self._sizes = None
-        self._alpha = False
-        self.valid = None
-        self.anchors = None
-        if self._grew:
-            torch.cuda.empty_cache()            # hand the replaced (smaller) slots back instead of keeping them cached next to the new ones
 
     def release(self):
         """Drops everything this plan holds -- pool views, anchors, launch lists, CUDA graphs -- when the engine evicts it or replaces the pool
@@ -701,10 +858,13 @@ class _TrainPlan:
         rows of one buffer."""
         self._wgrad(dys, xs, layer.taps, layer.cout, layer.cin_real, layer.dw, layout=1)
         if layer.db is not None:
-            L = lib()
-            ws = self._workspace(L.nrpn_bias_grad_workspace_bytes(layer.cout))
-            rows = sum(dy.numel() for dy in dys) // layer.cout
-            check(L.nrpn_bias_grad(_p(dys[0]), rows, layer.cout, layer.cout, self.f16, _p(layer.db), _p(ws), ws.numel(), _stream()), "bias_grad")
+            self._bias_grad(layer, dys)
+
+    def _bias_grad(self, layer: _TConv, dys):
+        L = lib()
+        ws = self._workspace(L.nrpn_bias_grad_workspace_bytes(layer.cout))
+        rows = sum(dy.numel() for dy in dys) // layer.cout
+        check(L.nrpn_bias_grad(_p(dys[0]), rows, layer.cout, layer.cout, self.f16, _p(layer.db), _p(ws), ws.numel(), _stream()), "bias_grad")
 
     def _dgrad(self, layer: _TConv, dys, dxs, dims, res=None):
         """Data gradient of a stride-1 layer: its mirrored / transposed operand run forward over the levels dys[i] -> dxs[i] (both dims[i]),
